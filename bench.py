@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Benchmark of the few-shot-detection meta-training hot path (BASELINE.json).
 
-    python bench.py --gpus N --steps K --warmup W            # this repo (CUDA, sm_100a)
+    python bench.py --gpus N --steps K --warmup W            # this repo (CUDA, sm_90a)
+    python bench.py ... --dump-outputs DIR                     # + what the last timed step computed, as DIR/<name>.npy
     python bench.py --impl reference --gpus N --steps K ...  # the reference's algorithm on the host CPU
 
 One "step" = one meta-training iteration on one synthetic batch per GPU:
@@ -43,7 +44,36 @@ def parse():
     ap.add_argument('--ref-batch', type=int, default=8, help='query images per CPU reference step (bounded sample)')
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-graph', action='store_true', help='launch every kernel eagerly instead of replaying a CUDA graph')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last one computed (loss, seeded samples of the updated '
+                         'parameters and of their gradients) as DIR/<name>.npy')
     return ap.parse_args()
+
+
+DUMP_SAMPLE = 7000000      # values per sampled array: two float32 arrays of 28 MB, under 64 MB in all
+
+
+def dump_outputs(d, loss, model):
+    """What a caller of the training step holds after the last timed step: its loss and the model's parameters and
+    gradients (all parameters flattened in model.parameters() order; larger than DUMP_SAMPLE values -> the same seeded
+    sample of positions every run; a parameter without a gradient contributes zeros).  float64 / float32 .npy files,
+    so two builds can be compared output for output."""
+    os.makedirs(d, exist_ok=True)
+    np.save(os.path.join(d, 'loss.npy'), np.array([float(loss.item())], dtype=np.float64))
+    params = list(model.parameters())
+    flat = torch.cat([p.detach().reshape(-1).float() for p in params])
+    idx = None
+    if flat.numel() > DUMP_SAMPLE:
+        g = torch.Generator().manual_seed(0)
+        idx = torch.randperm(flat.numel(), generator=g)[:DUMP_SAMPLE].sort()[0].to(flat.device)
+    pick = (lambda t: t) if idx is None else (lambda t: t[idx])
+    np.save(os.path.join(d, 'params.npy'), pick(flat).cpu().numpy().astype(np.float32))
+    missing = [n for n, p in model.named_parameters() if p.grad is None]
+    if missing:      # written as zeros, so the file always covers every parameter; said on stderr
+        sys.stderr.write('dump-outputs: %d parameter(s) without a gradient, written as zeros: %s\n'
+                         % (len(missing), ', '.join(missing[:8]) + (' ...' if len(missing) > 8 else '')))
+    grads = torch.cat([(p.grad.detach() if p.grad is not None else torch.zeros_like(p)).reshape(-1).float() for p in params])
+    np.save(os.path.join(d, 'grads.npy'), pick(grads).cpu().numpy().astype(np.float32))
 
 
 def synth_batch(B, ncls, side, seed):
@@ -258,7 +288,7 @@ _JSON_FD = None
 def quiet_stdout():
     """Point fd 1 at stderr for the whole run and keep the original for the JSON line: NCCL's version / INFO lines,
     the reference-style 'class_scale' print and anything a library writes to stdout would otherwise sit beside the
-    one line the driver parses."""
+    one line a caller parses."""
     global _JSON_FD
     if _JSON_FD is None:
         sys.stdout.flush()
@@ -405,9 +435,15 @@ def main():
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
-    ms = timed(lambda i: step(*resident[i % 2]), args.steps, 'value')
+    last = {}
+
+    def timed_step(i):
+        last['loss'] = step(*resident[i % 2])
+    ms = timed(timed_step, args.steps, 'value')
     clocks = sampler.stop() if rank == 0 else None
     value = global_batch * args.steps / (ms / 1e3)
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        dump_outputs(args.dump_outputs, last['loss'], model)
 
     # per-kernel timing + launch count: the same kernels launched eagerly (a CUDA-graph replay has no per-kernel
     # CUDA events), in the same run, right after the timed region
@@ -441,23 +477,17 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
     except Exception:
         pass
-    peak_tf = peaks.get('bf16_tflops_sustained', 1400.0)
-    peak_src = 'measured (MEASURED_PEAKS.json bf16_tflops_sustained)' if peaks else 'fallback 1.4 PF (B200_PROFILING.md)'
+    peak_tf = peaks.get('bf16_tflops_sustained', 989.4)
+    peak_src = 'measured (MEASURED_PEAKS.json bf16_tflops_sustained)' if peaks else 'H100 SXM data-sheet dense fp16 / bf16 peak (989 TFLOP/s)'
     dom = max(kern, key=lambda k: kern[k]['ms_per_step']) if kern else None
     traffic = None
-    try:
-        rj = json.load(open(os.path.join(ROOT, 'profiles', 'roofline_r02.json' if os.path.exists(os.path.join(ROOT, 'profiles', 'roofline_r02.json')) else 'roofline_r01.json')))
-        if rj.get('kernel') == dom:
-            traffic = rj['traffic_bytes_per_launch']
-    except Exception:
-        pass
     roofline = None
     if dom:
         a = kern[dom]['tflops_algorithmic']
         roofline = {'kernel': dom, 'bound': 'tensor', 'achieved': a, 'peak': peak_tf, 'unit': 'TFLOP/s',
                     'frac': a / peak_tf, 'traffic': traffic, 'peak_source': peak_src,
                     'share_of_step': kern[dom]['ms_per_step'] / (ms / args.steps), 'kernels': kern,
-                    'note': 'tcgen05 implicit GEMM (forward + input gradient) with fp16 hi/lo operand splitting: 3 tensor-core MMAs '
+                    'note': 'wgmma implicit GEMM (forward + input gradient) with fp16 hi/lo operand splitting: 3 tensor-core MMAs '
                             'per fp32-equivalent MAC, i.e. the tensor pipe does 3x the algorithmic FLOPs; measured against the bf16 peak. '
                             'Per-kernel times are CUDA-event timed eager launches in this run (the timed region '
                             'replays the same kernels from a CUDA graph)'}
@@ -466,7 +496,7 @@ def main():
     # (fused algorithmic bytes: every layer reads its input and writes its output once, x3 for a training step, + 8
     # passes over the 265 MB of parameters) next to the tensor-pipe figure of the MMA layers.
     step_rooflines = None
-    hbm_gbs = float(peaks.get('hbm_gbs', 6577.7))
+    hbm_gbs = float(peaks.get('hbm_gbs', 3350.0))      # H100 SXM HBM3 data-sheet bandwidth unless measured
 
     def whole_step(Bq, nc, sd, ms_step):
         alg_flops, alg_bytes = step_costs(Bq, nc, sd)
@@ -483,7 +513,7 @@ def main():
                 'tensor': {'algorithmic_flops_per_step_per_gpu': alg_flops, 'achieved_TFLOPs': alg_flops / t / 1e12,
                            'peak_TFLOPs': peak_tf, 'frac': alg_flops / t / 1e12 / peak_tf,
                            'note': 'forward / input-gradient GEMMs: fp32-equivalent arithmetic = 3 tensor-core MACs per MAC; '
-                                   'weight-gradient GEMMs: 1 (engine.TC_TERMS, profiles/precision_budget_r02.log)'}}
+                                   'weight-gradient GEMMs: 1 (engine.TC_TERMS)'}}
             if roofline is not None:
                 roofline['whole_step'] = step_rooflines
     except Exception as e:  # never lose the bench line over a derived figure
@@ -688,7 +718,7 @@ def main():
                    'batch_per_gpu': B, 'global_batch': global_batch, 'n_cls': ncls, 'neg': 'full',
                    'parallelism': 'dp%d' % world, 'weights': 'seeded random init (no checkpoint offline)',
                    'launch': 'eager' if graphed is None else 'cuda-graph replay of the whole step',
-                   'l2': 'inputs larger than L2: ~%.1f GB of activations are streamed per step (L2 = 126 MB)'
+                   'l2': 'inputs larger than L2: ~%.1f GB of activations are streamed per step (L2 = 50 MB)'
                          % (B * 105e6 / 1e9)},
         'e2e': {'value': e2e_value, 'unit': 'images/s', 'ms_per_step': ms_e2e / args.steps,
                 'h2d_bytes_per_step': h2d, 'd2h_bytes_per_step': 4,

@@ -1,3 +1,3 @@
-"""Drop-in shim: `import pooling` resolves to the B200-native implementation
+"""Drop-in shim: `import pooling` resolves to the H100-native implementation
 (put this directory first on sys.path instead of the reference checkout)."""
 from fewshot_detection_b200.pooling import *  # noqa: F401,F403

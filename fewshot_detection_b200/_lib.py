@@ -20,6 +20,7 @@ SIGNATURES = {
     'fsdet_version': ('', 'i'),
     'fsdet_last_error': ('', 's'),
     'fsdet_compiled_arch': ('', 'i'),
+    'fsdet_num_sms': ('', 'i'),
     'fsdet_nchw_to_nhwc': ('pipipiiiip', 'i'),
     'fsdet_nhwc_to_nchw': ('pippiiip', 'i'),
     'fsdet_conv_fwd': ('pipppip iiiiiii p'.replace(' ', ''), 'i'),
@@ -91,7 +92,7 @@ def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             'libfsdet.so not found at %s. Build it with `python -c "import __graft_entry__ as g; g.build()"` '
-            '(nvcc -gencode arch=compute_100a,code=sm_100a). There is no CPU or PyTorch fallback.' % LIB_PATH)
+            '(nvcc -gencode arch=compute_90a,code=sm_90a). There is no CPU or PyTorch fallback.' % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
     for name, (args, res) in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing: fail loudly

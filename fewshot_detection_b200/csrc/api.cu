@@ -15,4 +15,5 @@ void set_error(const char* fmt, ...) {
 
 extern "C" int fsdet_version(void) { return 100; }  // 0.1.0
 extern "C" const char* fsdet_last_error(void) { return fsdet::g_err; }
-extern "C" int fsdet_compiled_arch(void) { return 100; }
+extern "C" int fsdet_compiled_arch(void) { return 90; }   // sm_90a
+extern "C" int fsdet_num_sms(void) { return fsdet::kNumSMs; }

@@ -1,4 +1,4 @@
-// Shared helpers for libfsdet.so (sm_100a only).
+// Shared helpers for libfsdet.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -32,7 +32,7 @@ inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
 
 __device__ __forceinline__ float leaky(float u, float slope) { return u > 0.f ? u : u * slope; }
 

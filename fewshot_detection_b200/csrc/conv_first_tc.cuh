@@ -5,25 +5,31 @@
 // Why: at 416x416 the first layer's pre-BN tensor z is the largest tensor of the network (64 x 173056 x 32 fp32 =
 // 1.4 GB) while its input is 12 B per pixel.  Round 1 wrote z once and read it four more times (statistics, BN-apply,
 // BN-backward reduce, BN-backward apply) plus a 1.4 GB dz round trip into the weight-gradient kernel: 4.5 ms of a
-// 27 ms step for 1.6 % of its FLOPs.  Here every pass RECOMPUTES z from the input images with one small tcgen05 GEMM
-// per 128-pixel tile (K = 9 taps x 4 channels = 36, padded to 64) and consumes it from TMEM in the same kernel:
+// 27 ms step for 1.6 % of its FLOPs.  Here every pass RECOMPUTES z from the input images with one small wgmma GEMM
+// per 128-pixel tile (K = 9 taps x 4 channels = 36, padded to 48) and consumes it in the same kernel:
 //   MODE 0  statistics   : per-channel sum / sum of squares / min / max of z           -> fsdet_bn_finalize
 //   MODE 1  apply        : y = leaky(z*scale+shift), 2x2 max-pool -> pooled fp16 planes (and/or fp32) of the next layer
 //   MODE 2  bwd reduce   : du = dy_pool routed to the arg-max pixel x leaky'; sum(du), sum(du*xhat), max|du|
 //   MODE 3  bwd wgrad    : dz = scale*(du - c1 - xhat*c2) written to SHARED memory only and contracted with the same
-//                          im2col tile by a second tcgen05 GEMM (pixels = K) into a TMEM accumulator that lives for
+//                          im2col tile by a second wgmma GEMM (pixels = K) into register accumulators that live for
 //                          the whole CTA: dW partials per CTA, no dz in HBM at all.
 // The recomputed z is bit-identical in all four passes (same tiles, same MMAs), so arg-max decisions agree.
 //
-// Tile: 8 rows x 16 columns = 128 pixels = 128 TMEM lanes; warp q (0..3) owns the 4 x 8 sub-block of lanes 32q..32q+31
+// Tile: 8 rows x 16 columns = 128 pixels = 128 GEMM rows; warp q (0..3) owns the 4 x 8 sub-block of rows 32q..32q+31
 // (lane l -> row l>>3, column l&7), so the four pixels of a pooling window are lanes l, l^1, l^8, l^9 of one warp.
+// The accumulators come out of wgmma in its fragment layout and pass through a shared-memory tile to the thread that
+// owns the pixel.
 // Operand layout: A = im2col rows [pixel][64 halves] (128 B, 128-byte swizzle) as TWO fp16 planes (hi, lo) of the
 // input scaled by a power of two; the forward GEMM reads them K-major, the weight-gradient GEMM reads the very same
 // bytes MN-major with M = 128 = [hi plane | lo plane] (so the input stays exact to 22 bits and only dz is rounded to
 // fp16 - the "x exact, dz rounded" weight-gradient mode).  B = weights [32][64] hi/lo.  Three forward terms
 // (hi*hi + lo*hi + hi*lo) as everywhere else in the forward chain.
-// Threads: warps 0-3 = one thread per pixel (builds its im2col row, later owns its TMEM lane), warp 4 = input staging
-// (cp.async, one tile ahead) + the MMA-issuing thread.  Persistent CTAs walk the tile list.
+// Threads: warps 0-3 = one warpgroup, one thread per pixel (builds its im2col row, issues the wgmma GEMMs, owns its
+// pixel's accumulator row), warp 4 = input staging (cp.async, one tile ahead).  Persistent CTAs walk the tile list.
+// Registers: two CTAs per SM (launch bounds 160, 2) cap a thread at 168 registers.  Modes 0 and 1 fit (96 / 126); the
+// backward modes hold z and du (32 channels each) and, in mode 3, the two 64 x 64 dW fragments (64 more) across the
+// tile loop, and spill 58 (mode 2) / 64 (mode 3) bytes to the stack - L1-resident, and on an opt-in path.  One CTA per
+// SM would remove the spill but halve the warps that hide the per-tile barriers.
 #pragma once
 
 constexpr int FT_TH = 8, FT_TW = 16;                        // tile rows x columns (128 pixels)
@@ -32,6 +38,7 @@ constexpr int FT_HALO = FT_HH * FT_HW;                      // 180 pixels (float
 constexpr int FT_PLANE = 128 * 128;                         // one A plane: 128 rows x 128 B
 constexpr int FT_BPLANE = 32 * 128;                         // one B plane: 32 rows x 128 B
 constexpr int FT_THREADS = 160;
+constexpr int FT_ZLD = 33;                                  // row pitch (floats) of the z tile: conflict-free row reads
 
 enum { FT_STATS = 0, FT_APPLY = 1, FT_BWD_REDUCE = 2, FT_BWD_WGRAD = 3 };
 
@@ -66,12 +73,12 @@ struct FtCfg {
     static constexpr int OFF_DZ = OFF_BLO + FT_BPLANE;                              // MODE 3: [128 px][64 co] fp16
     static constexpr int OFF_EPI = OFF_DZ + (MODE == FT_BWD_WGRAD ? FT_PLANE : 0);  // 4 warps x 4 KB transposition tiles
     static constexpr int EPI_BYTES = (MODE == FT_STATS || MODE == FT_BWD_REDUCE) ? 4 * 4096 : 0;
-    static constexpr int OFF_HALO = OFF_EPI + EPI_BYTES;                            // [2][180] float4
+    static constexpr int OFF_ZT = OFF_EPI + EPI_BYTES;                              // z tile [128 px][FT_ZLD] fp32
+    static constexpr int OFF_HALO = OFF_ZT + 128 * FT_ZLD * 4;                      // [2][180] float4
     static constexpr int OFF_CONST = OFF_HALO + 2 * FT_HALO * 16;                   // 7 x 32 floats
     static constexpr int OFF_COMB = OFF_CONST + 7 * 32 * 4;                         // cross-warp combine: 4 x 32 x 32 B
     static constexpr int OFF_BAR = OFF_COMB + 4 * 32 * 32;
     static constexpr int SMEM_BYTES = OFF_BAR + 64 + 1024 /*align*/;
-    static constexpr int TMEM_COLS = MODE == FT_BWD_WGRAD ? 128 : 64;               // fwd hi|lo (64) [+ dW accumulator (64)]
 };
 
 __device__ __forceinline__ float ft_leaky(float u, float slope) { return u > 0.f ? u : u * slope; }
@@ -101,10 +108,8 @@ __global__ void __launch_bounds__(FT_THREADS, 2) conv_first_tc_kernel(const FtAr
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     float4* halo = reinterpret_cast<float4*>(smem + Cfg::OFF_HALO);
     float* cst = reinterpret_cast<float*>(smem + Cfg::OFF_CONST);     // x32: scale, shift, mean, invstd, c1 (hi), c2, c1 (lo)
-    uint64_t* acc_full = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
-    uint64_t* wg_done = acc_full + 1;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wg_done + 1);
-    float* red = reinterpret_cast<float*>(tmem_slot + 1);             // small block reductions
+    float* zt = reinterpret_cast<float*>(smem + Cfg::OFF_ZT);
+    float* red = reinterpret_cast<float*>(smem + Cfg::OFF_BAR);       // small block reductions
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int HW = p.H * p.W;
@@ -117,16 +122,7 @@ __global__ void __launch_bounds__(FT_THREADS, 2) conv_first_tc_kernel(const FtAr
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) wmax = fmaxf(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
     if (lane == 0) red[warp] = wmax;
-    if (tid == 0) {
-        mbar_init(acc_full, 1);
-        mbar_init(wg_done, 1);
-        fence_barrier_init();
-    }
-    if (warp == 4) tmem_alloc(tmem_slot, (uint32_t)Cfg::TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     wmax = fmaxf(fmaxf(red[0], red[1]), fmaxf(fmaxf(red[2], red[3]), red[4]));
     const float sw = scale_from_amax(wmax);
     const float sx = scale_from_amax(p.amax_x ? ldg_f32(p.amax_x) : 0.f);
@@ -186,13 +182,17 @@ __global__ void __launch_bounds__(FT_THREADS, 2) conv_first_tc_kernel(const FtAr
 
     // per-lane persistent accumulators of the reduction modes (lane = channel after the transposition)
     float s1 = 0.f, e1 = 0.f, s2 = 0.f, e2 = 0.f, vmin = INFINITY, vmax = -INFINITY;
+    // MODE 3: dW^T accumulators [hi plane k 0..63 | lo plane k 0..63] x 64 co, one 64 x 64 wgmma fragment each
+    float dwh[32], dwl[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) dwh[i] = dwl[i] = 0.f;
+    const uint32_t sa = smem_u32(smem);
 
     if (warp == 4 && (int)blockIdx.x < p.tiles) stage(blockIdx.x, 0);
     unsigned it = 0;
     int buf = 0;
     for (int t = blockIdx.x; t < p.tiles; t += gridDim.x, ++it, buf ^= 1) {
         if (warp == 4) cp_async_wait_all();
-        if (MODE == FT_BWD_WGRAD && it > 0 && warp < 4) mbar_wait(wg_done, (it - 1) & 1u);   // A / dz tiles are free again
         __syncthreads();                                   // S1: halo(t) landed; everyone is done with the previous tile
         const int tw = t % p.tiles_w;
         const int rest = t / p.tiles_w;
@@ -227,37 +227,46 @@ __global__ void __launch_bounds__(FT_THREADS, 2) conv_first_tc_kernel(const FtAr
             }
             fence_proxy_async();
         }
-        tc_fence_before();
         __syncthreads();                                   // S2: the A tile is complete
-        if (warp == 4) {
-            if (lane == 0) {
-                tc_fence_after();
-                // D=f32, A=B=f16, both K-major, N=32, M=128
-                const uint32_t idesc = (1u << 4) | ((uint32_t)(32 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-                const uint32_t sa = smem_u32(smem);
-                const uint64_t ahi = umma_desc_k_sw128(sa + Cfg::OFF_AHI), alo = umma_desc_k_sw128(sa + Cfg::OFF_ALO);
-                const uint64_t bhi = umma_desc_k_sw128(sa + Cfg::OFF_BHI), blo = umma_desc_k_sw128(sa + Cfg::OFF_BLO);
+        if (warp < 4) {
+            {
+                // z = A * B^T: M = 128 (two 64-row halves), N = 32, K = 48 >= 36; both operands K-major, 128-byte swizzle
+                float dh[2][16], dl[2][16];
+                const uint64_t bhi = gmma_desc(sa + Cfg::OFF_BHI, 0, 1024, GMMA_SW128), blo = gmma_desc(sa + Cfg::OFF_BLO, 0, 1024, GMMA_SW128);
+                wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < 3; ++k) {                 // K = 48 >= 36
-                    const uint64_t adv = (uint64_t)(k * 32 >> 4);
-                    umma_f16(tmem_base, ahi + adv, bhi + adv, idesc, k > 0 ? 1u : 0u);
-                    umma_f16(tmem_base + 32, alo + adv, bhi + adv, idesc, k > 0 ? 1u : 0u);
-                    umma_f16(tmem_base + 32, ahi + adv, blo + adv, idesc, 1u);
+                for (int h = 0; h < 2; ++h) {
+                    const uint64_t ahi = gmma_desc(sa + Cfg::OFF_AHI + h * 64 * 128, 0, 1024, GMMA_SW128);
+                    const uint64_t alo = gmma_desc(sa + Cfg::OFF_ALO + h * 64 * 128, 0, 1024, GMMA_SW128);
+#pragma unroll
+                    for (int k = 0; k < 3; ++k) {
+                        const uint64_t adv = (uint64_t)(k * 32 >> 4);
+                        wgmma<32>(dh[h], ahi + adv, bhi + adv, k > 0 ? 1u : 0u);
+                        wgmma<32>(dl[h], alo + adv, bhi + adv, k > 0 ? 1u : 0u);
+                        wgmma<32>(dl[h], ahi + adv, blo + adv, 1u);
+                    }
                 }
-                umma_commit(acc_full);
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_use<16>(dh[0]); wgmma_use<16>(dh[1]); wgmma_use<16>(dl[0]); wgmma_use<16>(dl[1]);
+                // fragment -> z tile (row = pixel): lo terms first, as (lo + hi) * inv
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r0 = 64 * h + 16 * warp + (lane >> 2);
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const int c = 8 * j + 2 * (lane & 3);
+                        zt[r0 * FT_ZLD + c] = (dl[h][4 * j] + dh[h][4 * j]) * inv;
+                        zt[r0 * FT_ZLD + c + 1] = (dl[h][4 * j + 1] + dh[h][4 * j + 1]) * inv;
+                        zt[(r0 + 8) * FT_ZLD + c] = (dl[h][4 * j + 2] + dh[h][4 * j + 2]) * inv;
+                        zt[(r0 + 8) * FT_ZLD + c + 1] = (dl[h][4 * j + 3] + dh[h][4 * j + 3]) * inv;
+                    }
+                }
             }
-        } else {
-            mbar_wait(acc_full, it & 1u);
-            tc_fence_after();
-            uint32_t r[32];
+            named_bar_sync(1, 128);
             float z[32];
-            const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16);
-            tmem_ld32(taddr + 32, r);                         // lo terms first
 #pragma unroll
-            for (int c = 0; c < 32; ++c) z[c] = __uint_as_float(r[c]);
-            tmem_ld32(taddr, r);
-#pragma unroll
-            for (int c = 0; c < 32; ++c) z[c] = (z[c] + __uint_as_float(r[c])) * inv;
+            for (int c = 0; c < 32; ++c) z[c] = zt[tid * FT_ZLD + c];
             uint8_t* tb = smem + Cfg::OFF_EPI + warp * 4096;      // this warp's 32 x 32 transposition tile (modes 0, 2)
 
             if (MODE == FT_STATS) {
@@ -374,25 +383,22 @@ __global__ void __launch_bounds__(FT_THREADS, 2) conv_first_tc_kernel(const FtAr
                         *reinterpret_cast<uint4*>(smem + Cfg::OFF_DZ + m * 128 + ((j ^ (m & 7)) << 4)) = hi;
                     }
                     fence_proxy_async();
-                }
-            }
-        }
-        if (MODE == FT_BWD_WGRAD) {
-            tc_fence_before();
-            __syncthreads();                               // S3: the dz tile is complete
-            if (warp == 4 && lane == 0) {
-                tc_fence_after();
-                // dW^T[k][co] += sum_p A[p][k] * dz[p][co]: both operands MN-major (pixel = K), M = 128 = [A_hi | A_lo], N = 64
-                const uint32_t idesc = (1u << 4) | (1u << 15) | (1u << 16) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-                const uint32_t sa = smem_u32(smem);
-                const uint64_t ad = umma_desc_mn_sw128(sa + Cfg::OFF_AHI, FT_PLANE);
-                const uint64_t bd = umma_desc_mn_sw128(sa + Cfg::OFF_DZ, FT_PLANE);
+                    named_bar_sync(1, 128);                // the dz tile is complete
+                    // dW^T[k][co] += sum_p A[p][k] * dz[p][co]: both operands MN-major (pixel = K), M = 64 per plane, N = 64
+                    const uint64_t ah = gmma_desc(sa + Cfg::OFF_AHI, FT_PLANE, 1024, GMMA_SW128);
+                    const uint64_t al = gmma_desc(sa + Cfg::OFF_ALO, FT_PLANE, 1024, GMMA_SW128);
+                    const uint64_t bd = gmma_desc(sa + Cfg::OFF_DZ, FT_PLANE, 1024, GMMA_SW128);
+                    wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < 8; ++k) {                 // 8 x 16 pixels
-                    const uint64_t adv = (uint64_t)(k * 2048 >> 4);
-                    umma_f16(tmem_base + 64, ad + adv, bd + adv, idesc, (it > 0 || k > 0) ? 1u : 0u);
+                    for (int k = 0; k < 8; ++k) {             // 8 x 16 pixels
+                        const uint64_t adv = (uint64_t)(k * 2048 >> 4);
+                        wgmma<64, 1, 1>(dwh, ah + adv, bd + adv, 1u);
+                        wgmma<64, 1, 1>(dwl, al + adv, bd + adv, 1u);
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();                       // the A / dz tiles are rewritten by the next tile
+                    wgmma_use<32>(dwh); wgmma_use<32>(dwl);
                 }
-                umma_commit(wg_done);
             }
         }
     }
@@ -424,45 +430,22 @@ __global__ void __launch_bounds__(FT_THREADS, 2) conv_first_tc_kernel(const FtAr
             }
         }
     }
-    if (MODE == FT_BWD_WGRAD) {
-        // dW accumulator: TMEM lane = row of [hi plane k = 0..63 | lo plane k = 0..63], columns 64.. = co.  Rows k and
-        // 64 + k belong together: warps 2, 3 park their rows in shared memory (the A tile is free now), warps 0, 1 add
-        // and write this CTA's partial [k < 36][co < 32] (unscaled: the reduce kernel divides by the operand scales).
-        float* park = reinterpret_cast<float*>(smem + Cfg::OFF_AHI);          // [64][32]
-        uint32_t r[32];
-        if (warp < 4) {
-            if (it > 0) {
-                mbar_wait(wg_done, (it - 1) & 1u);
-                tc_fence_after();
-                tmem_ld32(tmem_base + 64 + ((uint32_t)(warp * 32) << 16), r);
-            } else {
+    if (MODE == FT_BWD_WGRAD && warp < 4) {
+        // dW fragments: row = k (hi and lo plane rows of the same k sit in the same thread), column = co.  This CTA's
+        // partial [k < 36][co < 32] (unscaled: the reduce kernel divides by the operand scales).
 #pragma unroll
-                for (int c = 0; c < 32; ++c) r[c] = 0u;
-            }
-            if (warp >= 2) {
+        for (int j = 0; j < 4; ++j) {                      // columns 0..31 = the output channels
 #pragma unroll
-                for (int c = 0; c < 32; ++c) park[((warp - 2) * 32 + lane) * 32 + c] = __uint_as_float(r[c]);
+            for (int h = 0; h < 2; ++h) {
+                const int k = 16 * warp + (lane >> 2) + 8 * h;
+                const int co = 8 * j + 2 * (lane & 3);
+                if (k < 36) {
+                    float* dst = p.dw_partial + ((long long)blockIdx.x * 36 + k) * 32 + co;
+                    *reinterpret_cast<float2*>(dst) = make_float2(dwh[4 * j + 2 * h] + dwl[4 * j + 2 * h],
+                                                                  dwh[4 * j + 2 * h + 1] + dwl[4 * j + 2 * h + 1]);
+                }
             }
         }
-        __syncthreads();
-        if (warp < 2) {
-            const int k = warp * 32 + lane;
-            if (k < 36) {
-                float* dst = p.dw_partial + ((long long)blockIdx.x * 36 + k) * 32;
-#pragma unroll
-                for (int c = 0; c < 32; c += 4)
-                    *reinterpret_cast<float4*>(dst + c) = make_float4(__uint_as_float(r[c]) + park[k * 32 + c],
-                                                                      __uint_as_float(r[c + 1]) + park[k * 32 + c + 1],
-                                                                      __uint_as_float(r[c + 2]) + park[k * 32 + c + 2],
-                                                                      __uint_as_float(r[c + 3]) + park[k * 32 + c + 3]);
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, (uint32_t)Cfg::TMEM_COLS);
     }
 }
 

@@ -1,39 +1,37 @@
-// Halo-tile tcgen05 convolution (3x3, stride 1, "same" padding) for the HIGH-RESOLUTION layers - included by conv_tc.cu
+// Halo-tile wgmma convolution (3x3, stride 1, "same" padding) for the HIGH-RESOLUTION layers - included by conv_tc.cu
 // after the PTX wrappers and by tools/host_emul/conv_halo_emul.cpp after functional models of the same wrappers.
 //
 // Why: the im2col kernel (conv_tc_kernels.cuh) fetches the activation tile once PER FILTER TAP (9 x) and the weight tile
-// once per 128-pixel tile.  With 3-term operands (two fp16 planes each) a 128 x 128 tile asks the L2 -> SM fabric for
-// ~85 B per SM-clock at full tensor rate while the chip sustains ~42 B (B300_MICROARCH: 6300 B/clk over 148 SMs): the
-// short-K, high-resolution layers (conv2 at 208 x 208, conv3/5 at 104 x 104, forward and input gradient) ran at the L2
-// limit, not the tensor limit (profiles/ncu_r02.md: tensor pipe 24-47 %).  Here the activation tile is fetched with
-// its halo ONCE per 128 output pixels and all nine taps are served from shared memory:
+// once per 128-pixel tile.  With 3-term operands (two fp16 planes each) the short-K, high-resolution layers (conv2 at
+// 208 x 208, conv3/5 at 104 x 104, forward and input gradient) ask the L2 for more operand bytes per MMA than it
+// delivers.  Here the activation tile is fetched with its halo ONCE per 128 output pixels and all nine taps are served
+// from shared memory:
 //
 //   * tile = 8 x 16 output pixels (x fastest): GEMM row m = py * 8 + px, so every 8-row swizzle atom of the K-major
 //     operand is one spatial row of 8 pixels;
 //   * the halo tile is stored as three x-shifted copies [dx][18 rows][8 px][32 channels] (64-byte rows, 64-byte swizzle,
 //     a plain tiled TMA box of (32 c, 8 w, 18 h) at x0 + dx - 1, y0 - 1 with zero fill outside the image);
 //     filter tap (dy, dx) is then the ordinary K-major tile that starts dy atoms (dy * 512 B) into copy dx - the
-//     shared-memory descriptor, swizzle and instruction descriptor are those of the im2col kernel, only the start
-//     address moves by whole atoms;
+//     shared-memory descriptor and swizzle are those of the im2col kernel, only the start address moves by whole atoms;
 //   * activation traffic per tile: 3 x 18/16 = 3.4 tile-equivalents instead of 9;
-//   * one persistent CTA per SM; accumulators double buffered in TMEM (epilogue of tile i under the MMAs of tile i+1);
-//     where the whole weight operand fits (Cin/32 * BN <= 64: conv2 forward and input gradient, 72 KB) it is loaded
-//     ONCE per CTA and stays resident, otherwise it streams through a ring of (tap, chunk) stages filled by a second
-//     producer warp.
+//   * persistent CTAs (one per SM); where the whole weight operand fits (Cin/32 * BN <= 64: conv2 forward and input
+//     gradient, 72 KB) it is loaded ONCE per CTA and stays resident, otherwise it streams through a ring of (tap, chunk)
+//     stages filled by a second producer warp.
 //
 // Arithmetic: 3-term fp16 hi/lo scheme (conv_tc_kernels.cuh, TERMS = 3) - D_hi += A_hi * B_hi, D_lo += A_lo * B_hi +
 // A_hi * B_lo, summed in the epilogue.  K <= 1152 here, so one hi accumulator (the im2col short-K flavour's choice).
 //
-// Warps (352 threads): 0 = activation producer (+ resident weights), 1 = MMA issuer / TMEM owner, 2-9 = epilogue (two
-// warps per TMEM lane quarter, alternating 32-column chunks: at these tile shapes the epilogue's instruction stream, not
-// the tensor pipe, paces a 4-warp epilogue - profiles/ncu_r02b.md), 10 = weight-ring producer (idle when the weights
-// are resident).
+// Warps (384 threads): 0 = activation producer (+ resident weights), 1 = weight-ring producer (idle when the weights
+// are resident), 2-3 idle (the producer warpgroup hands its registers to the MMA warpgroups); warpgroups 1 and 2 =
+// MMA + epilogue for tile rows 0-63 (pixel rows 0-7) and 64-127 (pixel rows 8-15).
 #pragma once
 
 struct HaloArgs {
     const float* amax_a;
     const float* amax_b;
+    float* z;            // fp32 output [B][H][W][ldz] (first Cout channels)
     float* stats;        // optional [gridDim.x][4*Cout] = (sum | sum of squares | min | max), row = blockIdx.x
+    int ldz;
     int H, W, Cout;
     int cpitch;          // channel pitch of the weight planes' K axis: k = tap * cpitch + c
     int tiles_x, tiles_y;
@@ -48,6 +46,7 @@ constexpr int HALO_TW = 8, HALO_TH = 16;
 constexpr int HALO_ROWS = (HALO_TH + 2) * HALO_TW;          // 144 rows of 64 B per (plane, dx) copy
 constexpr int HALO_COPY_BYTES = HALO_ROWS * 64;             // 9216
 constexpr int HALO_ASTAGE_BYTES = 2 * 3 * HALO_COPY_BYTES;  // hi + lo planes, three x-shifts: 55296
+constexpr int HALO_THREADS = 384;
 
 template <int BN, int NCH, bool BRES>
 struct HaloCfg {
@@ -55,111 +54,95 @@ struct HaloCfg {
     static constexpr int BBLK = BN * 64;                           // one (tap, chunk) weight block of one plane
     static constexpr int BSTAGE = 2 * BBLK;                        // hi + lo
     static constexpr int NKB = 9 * NCH;                            // k-blocks (tap, chunk) per tile
-    static constexpr int EPI_BYTES = 8 * 4096;                     // one 32 x 32 fp32 staging block per epilogue warp
-    static constexpr int STAT_BYTES = 4 * BN * 16;
+    static constexpr int STAT_BYTES = 8 * BN * 16;                 // 8 MMA warps x BN channels x float4
     static constexpr int BUDGET = 227 * 1024 - 1024 - 256;
-    static constexpr int FREE_FOR_B = BUDGET - SA * HALO_ASTAGE_BYTES - EPI_BYTES - STAT_BYTES;
+    static constexpr int FREE_FOR_B = BUDGET - SA * HALO_ASTAGE_BYTES - STAT_BYTES;
     static constexpr int SB = BRES ? NKB : ((FREE_FOR_B / BSTAGE) > 8 ? 8 : (FREE_FOR_B / BSTAGE));
     static constexpr int OFF_B = SA * HALO_ASTAGE_BYTES;
-    static constexpr int OFF_EPI = OFF_B + SB * BSTAGE;
-    static constexpr int OFF_BAR = OFF_EPI + EPI_BYTES + STAT_BYTES;
+    static constexpr int OFF_STAT = OFF_B + SB * BSTAGE;
+    static constexpr int OFF_BAR = OFF_STAT + STAT_BYTES;
     static constexpr int SMEM_BYTES = OFF_BAR + 1024 + 256;
-    static constexpr int ACC_COLS = 2 * BN;                        // hi + lo accumulators of one set
-    static constexpr int TMEM_COLS = tmem_cols(2 * ACC_COLS);
     static_assert(SB >= 3, "weight ring too small");
     static_assert(!BRES || NKB * BSTAGE <= FREE_FOR_B, "resident weights do not fit");
-    static_assert(2 * ACC_COLS <= 512, "accumulators must fit in TMEM");
     static_assert(BSTAGE % 1024 == 0 || BN == 32, "swizzle atoms need 512-byte alignment");
 };
 
 template <int BN, int NCH, bool BRES>
-__global__ void __launch_bounds__(352, 1)
+__global__ void __launch_bounds__(HALO_THREADS, 1)
 conv_halo_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__ CUtensorMap tmAlo,
-                 const __grid_constant__ CUtensorMap tmBhi, const __grid_constant__ CUtensorMap tmBlo,
-                 const __grid_constant__ CUtensorMap tmZ, const HaloArgs p) {
+                 const __grid_constant__ CUtensorMap tmBhi, const __grid_constant__ CUtensorMap tmBlo, const HaloArgs p) {
     using Cfg = HaloCfg<BN, NCH, BRES>;
     constexpr int SA = Cfg::SA, SB = Cfg::SB;
     FSDET_TC_DYN_SMEM(smem_raw);
     uint8_t* smem = tc_align_smem(smem_raw);
-    uint8_t* epi = smem + Cfg::OFF_EPI;
+    float4* sstat = reinterpret_cast<float4*>(smem + Cfg::OFF_STAT);   // [8 MMA warps][BN]
     uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
     uint64_t* a_empty = a_full + SA;
     uint64_t* b_full = a_empty + SA;              // [SB] ring, or [0] only when the weights are resident
     uint64_t* b_empty = b_full + 8;
-    uint64_t* acc_full = b_empty + 8;             // [2] MMA issuer -> epilogue
-    uint64_t* acc_empty = acc_full + 2;           // [2] epilogue (8 warps) -> MMA issuer
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int tiles_total = p.tiles_total;
     const int tiles_img = p.tiles_x * p.tiles_y;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmAhi);
         tma_prefetch_desc(&tmAlo);
         tma_prefetch_desc(&tmBhi);
         tma_prefetch_desc(&tmBlo);
-        tma_prefetch_desc(&tmZ);
         for (int s = 0; s < SA; ++s) {
             mbar_init(&a_full[s], 1);
-            mbar_init(&a_empty[s], 1);
+            mbar_init(&a_empty[s], 8);                 // the 8 MMA warps
         }
         for (int s = 0; s < 8; ++s) {
             mbar_init(&b_full[s], 1);
-            mbar_init(&b_empty[s], 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&acc_full[a], 1);
-            mbar_init(&acc_empty[a], 8);
+            mbar_init(&b_empty[s], 8);
         }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, (uint32_t)Cfg::TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    // The three issuing roles run with their whole warp converged and issue under elect_one() (see tc_ptx.cuh).
-    if (warp == 0) {
-        if (BRES) {          // the whole weight operand, once
-            if (elect_one()) {
-                mbar_expect_tx(&b_full[0], (uint32_t)(Cfg::NKB * Cfg::BSTAGE));
-#pragma unroll 1
-                for (int kb = 0; kb < Cfg::NKB; ++kb) {
-                    const int chunk = kb / 9, tap = kb - chunk * 9;
-                    uint8_t* st = smem + Cfg::OFF_B + kb * Cfg::BSTAGE;
-                    tma_load_2d(st, &tmBhi, &b_full[0], tap * p.cpitch + chunk * 32, 0);
-                    tma_load_2d(st + Cfg::BBLK, &tmBlo, &b_full[0], tap * p.cpitch + chunk * 32, 0);
-                }
-            }
-            __syncwarp();
-        }
-        unsigned it = 0;                                   // activation stages issued so far
-        for (int tile = (int)blockIdx.x; tile < tiles_total; tile += (int)gridDim.x) {
-            const int img = tile / tiles_img;
-            const int r = tile - img * tiles_img;
-            const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
-            const int x0 = tx * HALO_TW - 1, y0 = ty * HALO_TH - 1;
-#pragma unroll 1
-            for (int chunk = 0; chunk < NCH; ++chunk, ++it) {
-                const int s = it % SA;
-                mbar_wait_warp(&a_empty[s], ((it / SA) & 1) ^ 1);
+    // The producer warps run converged and issue under elect_one() (see tc_ptx.cuh).
+    if (warp < 4) {
+        regs_dec<40>();
+        if (warp == 0) {
+            if (BRES) {          // the whole weight operand, once
                 if (elect_one()) {
-                    uint8_t* st = smem + s * HALO_ASTAGE_BYTES;
-                    const int ncopy = (p.flags & 1) ? 1 : 3;
-                    mbar_expect_tx(&a_full[s], (uint32_t)(ncopy * 2 * HALO_COPY_BYTES));
-                    for (int dx = 0; dx < ncopy; ++dx) {
-                        tma_load_tiled_4d(st + dx * HALO_COPY_BYTES, &tmAhi, &a_full[s], chunk * 32, x0 + dx, y0, img);
-                        tma_load_tiled_4d(st + (3 + dx) * HALO_COPY_BYTES, &tmAlo, &a_full[s], chunk * 32, x0 + dx, y0, img);
+                    mbar_expect_tx(&b_full[0], (uint32_t)(Cfg::NKB * Cfg::BSTAGE));
+#pragma unroll 1
+                    for (int kb = 0; kb < Cfg::NKB; ++kb) {
+                        const int chunk = kb / 9, tap = kb - chunk * 9;
+                        uint8_t* st = smem + Cfg::OFF_B + kb * Cfg::BSTAGE;
+                        tma_load_2d(st, &tmBhi, &b_full[0], tap * p.cpitch + chunk * 32, 0);
+                        tma_load_2d(st + Cfg::BBLK, &tmBlo, &b_full[0], tap * p.cpitch + chunk * 32, 0);
                     }
                 }
                 __syncwarp();
             }
-        }
-    } else if (warp == 10) {
-        if (!BRES) {
+            unsigned it = 0;                                   // activation stages issued so far
+            for (int tile = (int)blockIdx.x; tile < tiles_total; tile += (int)gridDim.x) {
+                const int img = tile / tiles_img;
+                const int r = tile - img * tiles_img;
+                const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
+                const int x0 = tx * HALO_TW - 1, y0 = ty * HALO_TH - 1;
+#pragma unroll 1
+                for (int chunk = 0; chunk < NCH; ++chunk, ++it) {
+                    const int s = it % SA;
+                    mbar_wait_warp(&a_empty[s], ((it / SA) & 1) ^ 1);
+                    if (elect_one()) {
+                        uint8_t* st = smem + s * HALO_ASTAGE_BYTES;
+                        const int ncopy = (p.flags & 1) ? 1 : 3;
+                        mbar_expect_tx(&a_full[s], (uint32_t)(ncopy * 2 * HALO_COPY_BYTES));
+                        for (int dx = 0; dx < ncopy; ++dx) {
+                            tma_load_tiled_4d(st + dx * HALO_COPY_BYTES, &tmAhi, &a_full[s], chunk * 32, x0 + dx, y0, img);
+                            tma_load_tiled_4d(st + (3 + dx) * HALO_COPY_BYTES, &tmAlo, &a_full[s], chunk * 32, x0 + dx, y0, img);
+                        }
+                    }
+                    __syncwarp();
+                }
+            }
+        } else if (warp == 1 && !BRES) {
             unsigned it = 0;                                   // weight stages issued so far
             for (int tile = (int)blockIdx.x; tile < tiles_total; tile += (int)gridDim.x) {
 #pragma unroll 1
@@ -177,31 +160,41 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constan
                 }
             }
         }
-    } else if (warp == 1) {
-        // instruction descriptors: D=f32, A=B=f16, both K-major, M=128; N=BN, and N=2*BN for the fused hi|lo MMA
-        const uint32_t idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        const uint32_t idesc2 = (1u << 4) | ((uint32_t)(2 * BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        const bool fused = !(p.flags & 4);                 // flags bit 2 now selects the three-MMA form (A / B experiments)
+    } else {
+        regs_inc<232>();
+        const int cw = (warp >> 2) - 1;                        // MMA warpgroup: pixel rows 8 cw .. 8 cw + 7 of the tile
+        const int wq = warp & 3;
+        const int ct = (int)threadIdx.x - 128;
+        constexpr int NR = BN / 2;
+        const bool fused = !(p.flags & 4);                     // flags bit 2 selects the three-MMA form (A / B experiments)
         const bool hi_only = (p.flags & 8) != 0;
-        if (BRES) {
-            mbar_wait_warp(&b_full[0], 0);
-            tc_fence_after();
-        }
+        const float inv = 1.f / (scale_from_amax(p.amax_a ? ldg_f32(p.amax_a) : 0.f) * scale_from_amax(p.amax_b ? ldg_f32(p.amax_b) : 0.f));
+        const bool want_stats = p.stats != nullptr;
+        float ssum = 0.f, esum = 0.f, ssq = 0.f, esq = 0.f, smin = INFINITY, smax = -INFINITY;
+        float acc[2 * NR];                                     // [hi | lo]
+        if (BRES) mbar_wait(&b_full[0], 0);
         const uint32_t smem_base = smem_u32(smem);
-        unsigned ita = 0, itb = 0, t = 0;
-        for (int tile = (int)blockIdx.x; tile < tiles_total; tile += (int)gridDim.x, ++t) {
-            const unsigned a = t & 1u;
-            mbar_wait_warp(&acc_empty[a], ((t >> 1) & 1u) ^ 1u);    // the epilogue has drained this accumulator set
-            tc_fence_after();
-            const uint32_t dhi = tmem_base + a * (uint32_t)Cfg::ACC_COLS;
-            const uint32_t dlo = dhi + (uint32_t)BN;
+        // this warp has read activation stage `sa_` / weight stage `sb_` (< 0: none)
+        auto release = [&](int sa_, int sb_) {
+            __syncwarp();
+            if (lane == 0) {
+                if (sa_ >= 0) mbar_arrive(&a_empty[sa_]);
+                if (sb_ >= 0) mbar_arrive(&b_empty[sb_]);
+            }
+        };
+        int pend_a = -1, pend_b = -1;                          // stages whose last wgmma group may still be in flight
+        unsigned ita = 0, itb = 0;
+        for (int tile = (int)blockIdx.x; tile < tiles_total; tile += (int)gridDim.x) {
             uint32_t started = 0;
+            if (hi_only) {
+#pragma unroll
+                for (int i = NR; i < 2 * NR; ++i) acc[i] = 0.f;
+            }
 #pragma unroll 1
             for (int chunk = 0; chunk < NCH; ++chunk, ++ita) {
                 const int sa = ita % SA;
-                mbar_wait_warp(&a_full[sa], (ita / SA) & 1);
-                tc_fence_after();
-                const uint32_t a0 = umma_desc_lo(smem_base + sa * HALO_ASTAGE_BYTES);
+                mbar_wait(&a_full[sa], (ita / SA) & 1);
+                const uint32_t a0 = smem_base + sa * HALO_ASTAGE_BYTES + cw * 8 * (HALO_TW * 64);
 #pragma unroll 1
                 for (int dy = 0; dy < 3; ++dy) {
 #pragma unroll
@@ -211,142 +204,58 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constan
                             sb = chunk * 9 + dy * 3 + dx;
                         } else {
                             sb = itb % SB;
-                            mbar_wait_warp(&b_full[sb], (itb / SB) & 1);
-                            tc_fence_after();
+                            mbar_wait(&b_full[sb], (itb / SB) & 1);
                         }
-                        if (elect_one()) {
-                            const uint32_t ah = a0 + (uint32_t)((dx * HALO_COPY_BYTES + dy * (HALO_TW * 64)) >> 4);
-                            const uint32_t al = ah + (uint32_t)((3 * HALO_COPY_BYTES) >> 4);
-                            const uint32_t bh = umma_desc_lo(smem_base + Cfg::OFF_B + sb * Cfg::BSTAGE);
-                            const uint32_t bl = bh + (uint32_t)(Cfg::BBLK >> 4);
-                            constexpr uint32_t HI = UMMA_DESC_HI_K_SW64;
+                        const uint64_t ah = gmma_desc(a0 + dx * HALO_COPY_BYTES + dy * (HALO_TW * 64), 0, 512, GMMA_SW64);
+                        const uint64_t al = ah + (uint64_t)((3 * HALO_COPY_BYTES) >> 4);
+                        const uint64_t bh = gmma_desc(smem_base + Cfg::OFF_B + sb * Cfg::BSTAGE, 0, 512, GMMA_SW64);
+                        const uint64_t bl = bh + (uint64_t)(Cfg::BBLK >> 4);
+                        wgmma_fence();
 #pragma unroll
-                            for (uint32_t k = 0; k < 2; ++k) {     // 16 halves = 32 B along K inside the swizzle atom: + 2 in the descriptor
-                                if (hi_only) {
-                                    umma_f16_lohi(dhi, ah + 2 * k, HI, bh + 2 * k, HI, idesc, started);
-                                } else if (fused) {
-                                    // [D_hi | D_lo] (+)= A_hi * [B_hi | B_lo]: ONE MMA of width 2*BN (the lo block follows the hi block
-                                    // in shared memory, the lo accumulator follows the hi accumulator in TMEM); D_lo += A_lo * B_hi
-                                    umma_f16_lohi(dhi, ah + 2 * k, HI, bh + 2 * k, HI, idesc2, started);
-                                    umma_f16_lohi(dlo, al + 2 * k, HI, bh + 2 * k, HI, idesc, 1u);
-                                } else {
-                                    umma_f16_lohi(dhi, ah + 2 * k, HI, bh + 2 * k, HI, idesc, started);
-                                    umma_f16_lohi(dlo, al + 2 * k, HI, bh + 2 * k, HI, idesc, started);
-                                    umma_f16_lohi(dlo, ah + 2 * k, HI, bl + 2 * k, HI, idesc, 1u);
-                                }
-                                started = 1u;
+                        for (int k = 0; k < 2; ++k) {          // 16 halves = 32 B along K inside the swizzle atom: + 2 in the descriptor
+                            const uint64_t adv = (uint64_t)(2 * k);
+                            if (hi_only) {
+                                wgmma<BN>(acc, ah + adv, bh + adv, started);
+                            } else if (fused) {
+                                // [D_hi | D_lo] (+)= A_hi * [B_hi | B_lo]: ONE MMA of width 2*BN (the lo block follows the hi block
+                                // in shared memory, the lo accumulator follows the hi accumulator in registers); D_lo += A_lo * B_hi
+                                wgmma<2 * BN>(acc, ah + adv, bh + adv, started);
+                                wgmma<BN>(acc + NR, al + adv, bh + adv, 1u);
+                            } else {
+                                wgmma<BN>(acc, ah + adv, bh + adv, started);
+                                wgmma<BN>(acc + NR, al + adv, bh + adv, started);
+                                wgmma<BN>(acc + NR, ah + adv, bl + adv, 1u);
                             }
-                            if (!BRES) umma_commit(&b_empty[sb]);
+                            started = 1u;
                         }
-                        started = 1u;
-                        __syncwarp();
+                        wgmma_commit();
+                        // one tap stays in flight: every earlier group is complete, so the stages it read are free
+                        wgmma_wait<1>();
+                        release(pend_a, pend_b);
+                        pend_a = -1;
+                        pend_b = BRES ? -1 : sb;
                     }
                 }
-                if (elect_one()) umma_commit(&a_empty[sa]);     // frees the activation stage when these MMAs have read it
-                __syncwarp();
+                pend_a = sa;                                   // freed once the chunk's last tap has completed
             }
-            if (elect_one()) umma_commit(&acc_full[a]);         // accumulator set complete
-            __syncwarp();
-        }
-    } else {
-        // epilogue warps 2..9 -> TMEM lane quarter warp % 4 (4 spatial rows x 8 pixels of the tile), column chunks ch with
-        // ch % 2 == half (BN = 32: the second warp of a quarter only hands the accumulators back)
-        const int quarter = warp & 3;
-        const bool leader = elect_one();                       // issues (and later waits for) this warp's TMA stores
-        const int half = (warp - 2) >> 2;
-        const float inv = 1.f / (scale_from_amax(p.amax_a ? ldg_f32(p.amax_a) : 0.f) * scale_from_amax(p.amax_b ? ldg_f32(p.amax_b) : 0.f));
-        uint8_t* buf = epi + (warp - 2) * 4096;
-        const bool want_stats = p.stats != nullptr;
-        constexpr int NCHW = BN >= 64 ? BN / 64 : 1;           // chunks per warp
-        float ssum[NCHW], esum[NCHW], ssq[NCHW], esq[NCHW], smin[NCHW], smax[NCHW];
-#pragma unroll
-        for (int c = 0; c < NCHW; ++c) { ssum[c] = esum[c] = ssq[c] = esq[c] = 0.f; smin[c] = INFINITY; smax[c] = -INFINITY; }
-        unsigned t = 0, stores = 0;                            // tiles done, TMA stores issued by this warp
-        for (int tile = (int)blockIdx.x; tile < tiles_total; tile += (int)gridDim.x, ++t) {
-            const unsigned a = t & 1u;
+            wgmma_wait<0>();
+            wgmma_use<2 * NR>(acc);
+            release(pend_a, pend_b);
+            pend_a = pend_b = -1;
+            // epilogue: rows 16 wq + lane / 4 (+ 8) of this warpgroup's 64 = pixel rows 8 cw + 2 wq (+ 1), column lane / 4
             const int img = tile / tiles_img;
             const int r = tile - img * tiles_img;
             const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
-            const int x0 = tx * HALO_TW, y0 = ty * HALO_TH + quarter * 4;   // this warp's 8 x 4 pixel block
-            mbar_wait(&acc_full[a], (t >> 1) & 1u);
-            tc_fence_after();
-            if (y0 < p.H && (BN >= 64 || half == 0)) {         // warp-uniform: some of its rows are inside the image
-                // statistics row mask: bit rr set <=> row rr of the block (pixel x0 + rr % 8, y0 + rr / 8) is inside the image
-                uint32_t vmask = 0xffffffffu;
-                if (y0 + 4 > p.H || x0 + HALO_TW > p.W) {
-                    vmask = 0;
-                    for (int rr = 0; rr < 32; ++rr)
-                        if (y0 + (rr >> 3) < p.H && x0 + (rr & 7) < p.W) vmask |= 1u << rr;
-                }
-#pragma unroll
-                for (int cw = 0; cw < NCHW; ++cw) {
-                    const int ch = BN >= 64 ? cw * 2 + half : 0;
-                    const int n0 = ch * 32;
-                    if (n0 < p.Cout) {                         // warp-uniform
-                        float acc[32];
-                        const uint32_t taddr = tmem_base + a * (uint32_t)Cfg::ACC_COLS + ((uint32_t)(quarter * 32) << 16) + ch * 32;
-                        epi_load_scaled<true>(taddr, taddr + BN, inv, acc);
-                        if (stores >= 1) {                     // the previous store must have read the staging block
-                            if (leader) tma_store_wait_read<0>();
-                            __syncwarp();
-                        }
-                        epi_stage_row(buf, lane, acc);
-                        fence_proxy_async();
-                        __syncwarp();
-                        if (leader && !(p.flags & 2)) {
-                            if (p.accumulate) tma_reduce_add_4d(&tmZ, buf, n0, x0, y0, img);
-                            else tma_store_4d(&tmZ, buf, n0, x0, y0, img);
-                            tma_store_commit();
-                        }
-                        ++stores;
-                        if (want_stats) {
-                            float s1, q1, mn, mx;
-                            epi_col_stats(buf, lane, vmask, s1, q1, mn, mx);
-                            tc_kahan_add(ssum[cw], esum[cw], s1);
-                            tc_kahan_add(ssq[cw], esq[cw], q1);
-                            smin[cw] = fminf(smin[cw], mn);
-                            smax[cw] = fmaxf(smax[cw], mx);
-                        }
-                    }
-                }
-            }
-            // this warp's TMEM reads of set `a` are complete (tcgen05.wait::ld in epi_load_scaled): hand the set back
-            tc_fence_before();
-            __syncwarp();
-            if (leader) mbar_arrive(&acc_empty[a]);
+            const int x = tx * HALO_TW + (lane >> 2);
+            const int ya = ty * HALO_TH + 8 * cw + 2 * wq, yb = ya + 1;
+            float* z0 = (ya < p.H && !(p.flags & 2)) ? p.z + (((long long)img * p.H + ya) * p.W + x) * p.ldz : nullptr;
+            float* z1 = (yb < p.H && !(p.flags & 2)) ? p.z + (((long long)img * p.H + yb) * p.W + x) * p.ldz : nullptr;
+            epi_tile<BN, true>(acc, acc + NR, inv, z0, z1, p.Cout, p.accumulate, want_stats ? sstat + (warp - 4) * BN : nullptr);
+            if (want_stats) epi_fold_stats<BN>(sstat, ct, ssum, esum, ssq, esq, smin, smax);
         }
-        if (leader) tma_store_wait_read<0>();               // shared memory must outlive the bulk reads
-        __syncwarp();
-        if (want_stats) {
-            // fold the four pixel quarters in a fixed order and write this CTA's partial row
-            float4* sbuf = reinterpret_cast<float4*>(epi + Cfg::EPI_BYTES);   // [4][BN]
-            if (BN >= 64 || half == 0) {
-#pragma unroll
-                for (int cw = 0; cw < NCHW; ++cw) {
-                    const int ch = BN >= 64 ? cw * 2 + half : 0;
-                    sbuf[quarter * BN + ch * 32 + lane] = make_float4(ssum[cw] - esum[cw], ssq[cw] - esq[cw], smin[cw], smax[cw]);
-                }
-            }
-            named_bar_sync(1, 256);
-            const int e = (warp - 2) * 32 + lane;
-            for (int c = e; c < BN; c += 256) {
-                float4 tt = sbuf[c];
-#pragma unroll
-                for (int qq = 1; qq < 4; ++qq) {
-                    const float4 o = sbuf[qq * BN + c];
-                    tt.x += o.x; tt.y += o.y; tt.z = fminf(tt.z, o.z); tt.w = fmaxf(tt.w, o.w);
-                }
-                if (c < p.Cout) {
-                    float* dst = p.stats + (long long)blockIdx.x * 4 * p.Cout + c;
-                    dst[0] = tt.x; dst[p.Cout] = tt.y; dst[2 * p.Cout] = tt.z; dst[3 * p.Cout] = tt.w;
-                }
-            }
+        if (want_stats && ct < BN && ct < p.Cout) {
+            float* dst = p.stats + (long long)blockIdx.x * 4 * p.Cout + ct;
+            dst[0] = ssum - esum; dst[p.Cout] = ssq - esq; dst[2 * p.Cout] = smin; dst[3 * p.Cout] = smax;
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, (uint32_t)Cfg::TMEM_COLS);
     }
 }

@@ -433,29 +433,14 @@ __device__ __forceinline__ float in_px(const float* __restrict__ in0, int C0, co
     return 0.f;
 }
 
-// packed fp32 pairs: FFMA2 (fma.rn.f32x2) issues two IEEE fp32 FMAs per lane from one instruction slot, each half
-// rounding exactly like fmaf()
+// fp32 pairs: two scalar FFMAs per pair (each rounding exactly like fmaf()); a packed operand pair is unpacked from 64 bits
 typedef unsigned long long f32x2;
-__device__ __forceinline__ void fma2(f32x2& acc, f32x2 a, f32x2 b) { asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(a), "l"(b)); }
-__device__ __forceinline__ f32x2 pack2(float lo, float hi) {
-    f32x2 r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
 __device__ __forceinline__ float2 unpack2(f32x2 v) {
     float2 r;
     asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(v));
     return r;
 }
-// pair arithmetic in two flavours (same rounding): packed FFMA2 or two scalar FFMAs
 template <bool PACKED> struct Pair;
-template <> struct Pair<true> {
-    f32x2 v;
-    __device__ __forceinline__ static Pair make(float lo, float hi) { Pair p; p.v = pack2(lo, hi); return p; }
-    __device__ __forceinline__ static Pair raw(f32x2 bits) { Pair p; p.v = bits; return p; }
-    __device__ __forceinline__ void fma(const Pair& a, const Pair& b) { fma2(v, a.v, b.v); }
-    __device__ __forceinline__ float2 get() const { return unpack2(v); }
-};
 template <> struct Pair<false> {
     float2 v;
     __device__ __forceinline__ static Pair make(float lo, float hi) { Pair p; p.v = make_float2(lo, hi); return p; }
@@ -489,7 +474,7 @@ template <bool PK> __device__ __forceinline__ Px4<PK> lds_px(const float4* p) {
 // STATS: the BatchNorm partial row of this CTA (sum | sum of squares | min | max per channel, the layout
 // fsdet_bn_finalize reads) is taken from the values while they are in registers - a thread owns ONE output channel, so
 // there is nothing to transpose - instead of a separate pass over the 1.4 GB tensor (fsdet_colstats).
-// (two CTAs per SM at 122 registers; three at 80 registers measured slower: 1.12 vs 1.02 ms per step, tools/r2b_callE.sh)
+// (two CTAs per SM)
 template <bool PK, bool STATS>
 __global__ void __launch_bounds__(256, 2) conv_first_fwd_kernel(const float* __restrict__ in0, int C0, const float* __restrict__ in1,
                                                                 int C1, const float* __restrict__ w /* [Cout][9][4] */,
@@ -873,8 +858,7 @@ extern "C" int fsdet_conv_first_fwd(const float* in0, int C0, const float* in1, 
     if (tiles == 0) return 0;
     FSDET_CHECK_ARG(tiles < (1ll << 31), "conv_first_fwd: too many tiles");
     const unsigned ctas = (unsigned)(tiles < 2LL * kNumSMs ? tiles : 2LL * kNumSMs);
-    // packed FFMA2 flavour: fewer issue slots per pixel (measured 705 us vs 750 us at B=64, 416x416)
-    conv_first_fwd_kernel<true, false><<<ctas, 256, 0, (cudaStream_t)stream>>>(in0, C0, in1, C1, w_pad4, z, ldz, B, H, W, Cout, nullptr);
+    conv_first_fwd_kernel<false, false><<<ctas, 256, 0, (cudaStream_t)stream>>>(in0, C0, in1, C1, w_pad4, z, ldz, B, H, W, Cout, nullptr);
     return launch_status("conv_first_fwd");
 }
 
@@ -893,7 +877,7 @@ extern "C" int fsdet_conv_first_fwd_stats(const float* in0, int C0, const float*
     if (tiles == 0) return 0;
     FSDET_CHECK_ARG(tiles < (1ll << 31), "conv_first_fwd_stats: too many tiles");
     const unsigned ctas = (unsigned)fsdet_conv_first_stat_rows(B, H, W);
-    conv_first_fwd_kernel<true, true><<<ctas, 256, 0, (cudaStream_t)stream>>>(in0, C0, in1, C1, w_pad4, z, ldz, B, H, W, Cout,
+    conv_first_fwd_kernel<false, true><<<ctas, 256, 0, (cudaStream_t)stream>>>(in0, C0, in1, C1, w_pad4, z, ldz, B, H, W, Cout,
                                                                               stat_partial);
     return launch_status("conv_first_fwd_stats");
 }
@@ -915,7 +899,6 @@ extern "C" int fsdet_conv_first_wgrad(const float* in0, int C0, const float* in1
         cudaError_t e = cudaFuncSetAttribute(conv_first_wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         if (e != cudaSuccess) { set_error("conv_first_wgrad: %s", cudaGetErrorString(e)); return (int)e; }
     }
-    // scalar FFMA flavour (the packed one is register-bandwidth bound here: 900 us vs 873 us)
     conv_first_wgrad_kernel<false><<<ctas, FW_THREADS, smem, s>>>(in0, C0, in1, C1, dz, lddz, workspace, B, H, W, Cout);
     int st = launch_status("conv_first_wgrad");
     if (st) return st;

@@ -1,24 +1,22 @@
-// tcgen05 implicit-GEMM convolution for sm_100a (forward and input-gradient).
+// wgmma implicit-GEMM convolution for sm_90a (forward, input gradient and weight gradient).
 //
 //   z[p][n] = sum_{tap,ci} x[p+tap][ci] * w[n][tap][ci]      (stride 1, "same" padding, k in {1,3})
 //
-// Tensor-core path of nn.Conv2d (darknet_meta.py:236-252) for every layer with Cin % 64 == 0.
+// Tensor-core path of nn.Conv2d (darknet_meta.py:236-252) for every layer with Cin % 32 == 0.
 //
 // Precision: the reference is fp32 end to end and the parity bar is 1e-3 relative through a 23-layer
 // train-mode-BN stack with max-pool / LeakyReLU kinks (every rounding error also flips arg-max decisions), which
 // single-pass bf16/tf32 operands do not meet.  Operands are therefore split into two fp16 planes of the tensor
 // scaled by a power of two so that its max lies in [512, 1024)  (hi = fp16(s*x), lo = fp16(s*x - hi): 22 mantissa
 // bits in the same 4 B/element as fp32) and each K step issues three MMAs  Ahi*Bhi + Alo*Bhi + Ahi*Blo  into fp32
-// TMEM accumulators; the k-blocks rotate over four accumulators (summed in the epilogue) because the tensor
-// core's fp32 accumulation truncates and its error grows with the number of accumulation steps.
+// register accumulators; on long K the hi*hi sums of every k-block are added to a register total with
+// round-to-nearest, because the tensor core's fp32 accumulation truncates and its error grows with the number of
+// accumulation steps.
 //
-// Structure (one CTA = one 128-pixel x BN-channel output tile, 192 threads):
-//   warp 0   : TMA producer.  A tiles come straight from the NHWC activation planes through an *im2col*
-//              tensor map (cp.async.bulk.tensor.4d...im2col: 128 consecutive output pixels x 64 channels of
-//              one filter tap, zero-filled halo), B tiles from the [Cout][K] weight planes (2-D tiled map);
-//              both land in shared memory in the 128-byte-swizzled K-major layout tcgen05 consumes.
-//   warp 1   : allocates TMEM, issues tcgen05.mma (one elected thread), commits to mbarriers.
-//   warps 2-5: epilogue, tcgen05.ld the fp32 accumulator (lane = pixel) and store z rows.
+// Structure (conv_tc_kernels.cuh): a producer warp fills a ring of shared-memory stages with TMA - A tiles straight
+// from the NHWC activation planes through an *im2col* tensor map (128 consecutive output pixels x BK channels of one
+// filter tap, zero-filled halo), B tiles from the [Cout][K] weight planes - in the swizzled K-major layout wgmma
+// consumes; two MMA warpgroups (64 tile rows each) issue wgmma and run the epilogue from their registers.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <stdlib.h>
@@ -121,7 +119,6 @@ __global__ void __launch_bounds__(256) colstats_kernel(const float* __restrict__
     }
 }
 
-constexpr int NHI = 3;    // hi*hi accumulators of the long-K fp32-grade flavour (k-blocks rotate over them)
 constexpr int TC_BK = 64;                       // halves per 128-byte row (im2col debug tile, weight-gradient tiles)
 constexpr int TC_A_BYTES = 128 * TC_BK * 2;     // 16 KB per plane
 
@@ -132,7 +129,9 @@ constexpr int TC_A_BYTES = 128 * TC_BK * 2;     // 16 KB per plane
 //   dw[co][tap][ci] = sum_p dz[p][co] * x[p + tap][ci]
 // GEMM with the pixel index as K: both operands are "MN-major" in shared memory (a row = one pixel, 64 channels
 // = 128 B), A = dz tile via a 2-D tiled map, B = x tile of ONE filter tap via the im2col map (zero-filled halo).
-// One CTA = 128 co x BN ci x one tap over a range of pixels (split-K across blockIdx.z).
+// One CTA = 128 co x BN ci x one tap over a range of pixels (split-K across blockIdx.z): a producer warp and two MMA
+// warpgroups of 64 co each.  The hi*hi products of every 64-pixel stage are summed in a fresh accumulator and added to
+// a register total (round-to-nearest; see the file header).
 
 struct TcWgArgs {
     float* out;  // [splits][Cout][K]
@@ -145,12 +144,13 @@ struct TcWgArgs {
 
 constexpr int WG_BP = 64;                      // pixels per stage
 constexpr int WG_BLK = WG_BP * 128;            // one [64 pixels][64 channels] fp16 block = 8 KB
+constexpr int WG_BN = 128;                     // N tile: 1 or 2 filter taps x 128 or 64 input channels
 
 // TERMS as in conv_tc_kernel (A = dz, B = x): bit 0 adds dz_lo * x_hi, bit 1 adds dz_hi * x_lo
-template <int BN, int TERMS, int NH>
+template <int TERMS>
 struct WgCfg {
     static constexpr int A_BYTES = 2 * WG_BLK;            // 128 co
-    static constexpr int B_BYTES = (BN / 64) * WG_BLK;
+    static constexpr int B_BYTES = (WG_BN / 64) * WG_BLK;
     static constexpr int NA = 1 + (TERMS & 1);
     static constexpr int NBP = 1 + ((TERMS >> 1) & 1);
     static constexpr int STAGE_BYTES = NA * A_BYTES + NBP * B_BYTES;
@@ -159,29 +159,25 @@ struct WgCfg {
     static constexpr int OFF_BLO = OFF_BHI + B_BYTES;
     static constexpr int BUDGET = 227 * 1024 - 1024 - 256;
     static constexpr int STAGES = (BUDGET / STAGE_BYTES) > 6 ? 6 : (BUDGET / STAGE_BYTES);
-    static constexpr int NACC = NH + (TERMS ? 1 : 0);
-    static constexpr int TMEM_COLS = tmem_cols(NACC * BN);
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
-    static_assert(NACC * BN <= 512, "accumulators must fit in TMEM");
     static_assert(STAGES >= 2, "at least two pipeline stages");
 };
 
-template <int BN, int TAPS, int TERMS, int NH>   // N tile = TAPS filter taps x (BN / TAPS) input channels
-__global__ void __launch_bounds__(192, 1)
+template <int TAPS, int TERMS>   // N tile = TAPS filter taps x (WG_BN / TAPS) input channels
+__global__ void __launch_bounds__(384, 1)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDhi, const __grid_constant__ CUtensorMap tmDlo,
                 const __grid_constant__ CUtensorMap tmXhi, const __grid_constant__ CUtensorMap tmXlo, const TcWgArgs p) {
-    using Cfg = WgCfg<BN, TERMS, NH>;
+    using Cfg = WgCfg<TERMS>;
     constexpr int STAGES = Cfg::STAGES;
+    constexpr int BN = WG_BN;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* tmem_full_bar = empty_bar + STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    constexpr int CIB = BN / TAPS;                      // input channels per tap in this tile (64, 128 or 256)
+    constexpr int CIB = BN / TAPS;                      // input channels per tap in this tile (64 or 128)
     const int kk = p.ks * p.ks;
     const int ci_tiles = (p.Cin + CIB - 1) / CIB;
     const int tap0 = (blockIdx.x / ci_tiles) * TAPS;
@@ -192,136 +188,114 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDhi, const __grid_constant
     if (pend > p.M) pend = p.M;
     const int nk = pend > pbeg ? (int)((pend - pbeg + WG_BP - 1) / WG_BP) : 0;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmDhi);
         if (TERMS & 1) tma_prefetch_desc(&tmDlo);
         tma_prefetch_desc(&tmXhi);
         if (TERMS & 2) tma_prefetch_desc(&tmXlo);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], 8);                // the 8 MMA warps
         }
-        mbar_init(tmem_full_bar, 1);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, (uint32_t)Cfg::TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    // issuing roles: whole warp converged, instructions under elect_one() (tc_ptx.cuh)
-    if (warp == 0) {
-        const int HW = p.H * p.W;
+    if (warp < 4) {
+        regs_dec<40>();
+        if (warp == 0) {                                // producer: whole warp converged, instructions under elect_one()
+            const int HW = p.H * p.W;
 #pragma unroll 1
-        for (int kb = 0; kb < nk; ++kb) {
-            const int s = kb % STAGES;
-            mbar_wait_warp(&empty_bar[s], ((kb / STAGES) & 1) ^ 1);
-            if (elect_one()) {
-                uint8_t* st = smem + s * Cfg::STAGE_BYTES;
-                mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
-                const long long p0 = pbeg + (long long)kb * WG_BP;
-                const int img = (int)(p0 / HW);
-                const int rem = (int)(p0 - (long long)img * HW);
-                const int ph = rem / p.W, pw = rem - ph * p.W;
+            for (int kb = 0; kb < nk; ++kb) {
+                const int s = kb % STAGES;
+                mbar_wait_warp(&empty_bar[s], ((kb / STAGES) & 1) ^ 1);
+                if (elect_one()) {
+                    uint8_t* st = smem + s * Cfg::STAGE_BYTES;
+                    mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
+                    const long long p0 = pbeg + (long long)kb * WG_BP;
+                    const int img = (int)(p0 / HW);
+                    const int rem = (int)(p0 - (long long)img * HW);
+                    const int ph = rem / p.W, pw = rem - ph * p.W;
 #pragma unroll
-                for (int j = 0; j < 2; ++j) {
-                    tma_load_2d(st + j * WG_BLK, &tmDhi, &full_bar[s], co0 + 64 * j, (int)p0);
-                    if (TERMS & 1) tma_load_2d(st + Cfg::OFF_ALO + j * WG_BLK, &tmDlo, &full_bar[s], co0 + 64 * j, (int)p0);
-                }
+                    for (int j = 0; j < 2; ++j) {
+                        tma_load_2d(st + j * WG_BLK, &tmDhi, &full_bar[s], co0 + 64 * j, (int)p0);
+                        if (TERMS & 1) tma_load_2d(st + Cfg::OFF_ALO + j * WG_BLK, &tmDlo, &full_bar[s], co0 + 64 * j, (int)p0);
+                    }
 #pragma unroll
-                for (int j = 0; j < BN / 64; ++j) {
-                    int tap = tap0 + (j * 64) / CIB;
-                    if (tap >= kk) tap = kk - 1;      // tail group: duplicate load, its columns are not stored
-                    const int r = tap / p.ks, sx = tap - r * p.ks;
-                    const int ci = ci0 + (j * 64) % CIB;
-                    tma_load_im2col_4d(st + Cfg::OFF_BHI + j * WG_BLK, &tmXhi, &full_bar[s], ci, pw - p.pad, ph - p.pad, img,
-                                       (uint16_t)sx, (uint16_t)r);
-                    if (TERMS & 2)
-                        tma_load_im2col_4d(st + Cfg::OFF_BLO + j * WG_BLK, &tmXlo, &full_bar[s], ci, pw - p.pad, ph - p.pad, img,
+                    for (int j = 0; j < BN / 64; ++j) {
+                        int tap = tap0 + (j * 64) / CIB;
+                        if (tap >= kk) tap = kk - 1;      // tail group: duplicate load, its columns are not stored
+                        const int r = tap / p.ks, sx = tap - r * p.ks;
+                        const int ci = ci0 + (j * 64) % CIB;
+                        tma_load_im2col_4d(st + Cfg::OFF_BHI + j * WG_BLK, &tmXhi, &full_bar[s], ci, pw - p.pad, ph - p.pad, img,
                                            (uint16_t)sx, (uint16_t)r);
+                        if (TERMS & 2)
+                            tma_load_im2col_4d(st + Cfg::OFF_BLO + j * WG_BLK, &tmXlo, &full_bar[s], ci, pw - p.pad, ph - p.pad, img,
+                                               (uint16_t)sx, (uint16_t)r);
+                    }
                 }
+                __syncwarp();
             }
-            __syncwarp();
         }
-    } else if (warp == 1) {
-        // D=f32, A=B=f16, both MN-major, N=BN, M=128
-        const uint32_t idesc = (1u << 4) | (1u << 15) | (1u << 16) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        // MN-major 128-byte-swizzle descriptors as (lo, hi): lo = address >> 4 | (distance to the next 64-element block) >> 4 << 16
-        constexpr uint32_t HI = UMMA_DESC_HI_K_SW128;          // SBO 1024 B (next group of 8 pixels along K), version, SWIZZLE_128B
-        constexpr uint32_t LBO = (uint32_t)(WG_BLK >> 4) << 16;
+    } else {
+        regs_inc<232>();
+        const int cw = (warp >> 2) - 1;                 // MMA warpgroup: output channels co0 + 64 cw .. + 63
+        const int wq = warp & 3;
+        constexpr int NR = BN / 2;
+        float acc[TERMS ? 2 * NR : NR];                 // [hi | lo]
+        float tot[NR];
+#pragma unroll
+        for (int i = 0; i < NR; ++i) tot[i] = 0.f;
+#pragma unroll
+        for (int i = 0; i < (TERMS ? 2 * NR : NR); ++i) acc[i] = 0.f;
         const uint32_t smem_base = smem_u32(smem);
 #pragma unroll 1
         for (int kb = 0; kb < nk; ++kb) {
             const int s = kb % STAGES;
-            mbar_wait_warp(&full_bar[s], (kb / STAGES) & 1);
-            tc_fence_after();
-            if (elect_one()) {
-                const uint32_t ah = (((smem_base + s * Cfg::STAGE_BYTES) & 0x3FFFF) >> 4) | LBO;
-                const uint32_t al = ah + (uint32_t)(Cfg::OFF_ALO >> 4);
-                const uint32_t bh = ah + (uint32_t)(Cfg::OFF_BHI >> 4);
-                const uint32_t bl = ah + (uint32_t)(Cfg::OFF_BLO >> 4);
-                const uint32_t dhi = tmem_base + (uint32_t)((kb % NH) * BN);
-                const uint32_t dlo = tmem_base + (uint32_t)(NH * BN);
+            mbar_wait(&full_bar[s], (kb / STAGES) & 1);
+            const uint32_t st = smem_base + s * Cfg::STAGE_BYTES;
+            // MN-major, 128-byte swizzle: LBO = next 64-channel block, SBO = next group of 8 pixels
+            const uint64_t ah = gmma_desc(st + cw * WG_BLK, WG_BLK, 1024, GMMA_SW128);
+            const uint64_t al = ah + (uint64_t)(Cfg::OFF_ALO >> 4);
+            const uint64_t bh = gmma_desc(st + Cfg::OFF_BHI, WG_BLK, 1024, GMMA_SW128);
+            const uint64_t bl = bh + (uint64_t)(Cfg::B_BYTES >> 4);
+            wgmma_fence();
 #pragma unroll
-                for (uint32_t k = 0; k < WG_BP / 16; ++k) {
-                    const uint32_t adv = k * (2048u >> 4);         // 16 pixels = two 8-row groups of 1024 B
-                    const uint32_t first_hi = (kb >= NH || k > 0) ? 1u : 0u;
-                    const uint32_t first_lo = (kb > 0 || k > 0) ? 1u : 0u;
-                    umma_f16_lohi(dhi, ah + adv, HI, bh + adv, HI, idesc, first_hi);
-                    if (TERMS & 1) umma_f16_lohi(dlo, al + adv, HI, bh + adv, HI, idesc, first_lo);
-                    if (TERMS & 2) umma_f16_lohi(dlo, ah + adv, HI, bl + adv, HI, idesc, (TERMS & 1) ? 1u : first_lo);
-                }
-                umma_commit(&empty_bar[s]);
+            for (int k = 0; k < WG_BP / 16; ++k) {
+                const uint64_t adv = (uint64_t)(k * (2048 >> 4));   // 16 pixels = two 8-row groups of 1024 B
+                const uint32_t first_lo = (kb > 0 || k > 0) ? 1u : 0u;
+                wgmma<BN, 1, 1>(acc, ah + adv, bh + adv, k > 0 ? 1u : 0u);
+                if (TERMS & 1) wgmma<BN, 1, 1>(acc + NR, al + adv, bh + adv, first_lo);
+                if (TERMS & 2) wgmma<BN, 1, 1>(acc + NR, ah + adv, bl + adv, (TERMS & 1) ? 1u : first_lo);
             }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_use<TERMS ? 2 * NR : NR>(acc);
             __syncwarp();
-        }
-        if (elect_one()) umma_commit(tmem_full_bar);
-        __syncwarp();
-    } else {
-        const int quarter = warp & 3;
-        const int co = co0 + quarter * 32 + lane;
-        const long long K = (long long)p.ks * p.ks * p.Cin;
-        float* orow = p.out + ((long long)blockIdx.z * p.Cout + (co < p.Cout ? co : 0)) * K;
-        if (nk > 0) {
-            mbar_wait(tmem_full_bar, 0);
-            tc_fence_after();
+            if (lane == 0) mbar_arrive(&empty_bar[s]);
+#pragma unroll
+            for (int i = 0; i < NR; ++i) tot[i] += acc[i];
         }
         const float inv = 1.f / (scale_from_amax(p.amax_a ? __ldg(p.amax_a) : 0.f) * scale_from_amax(p.amax_b ? __ldg(p.amax_b) : 0.f));
-        const int nhi = nk < NH ? nk : NH;
-#pragma unroll 1
-        for (int ch = 0; ch < BN / 32; ++ch) {
-            uint32_t r[32];
-            float acc[32];
+        const long long K = (long long)p.ks * p.ks * p.Cin;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-            const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + ch * 32;
-            if (TERMS != 0 && nk > 0) {
-                tmem_ld32(taddr + NH * BN, r);
+        for (int h = 0; h < 2; ++h) {
+            const int co = co0 + 64 * cw + 16 * wq + (lane >> 2) + 8 * h;
+            if (co >= p.Cout) continue;
+            float* orow = p.out + ((long long)blockIdx.z * p.Cout + co) * K;
 #pragma unroll
-                for (int j = 0; j < 32; ++j) acc[j] = __uint_as_float(r[j]);
-            }
-            for (int a = nhi - 1; a >= 0; --a) {
-                tmem_ld32(taddr + a * BN, r);
-#pragma unroll
-                for (int j = 0; j < 32; ++j) acc[j] += __uint_as_float(r[j]);
-            }
-            const int tap = tap0 + (ch * 32) / CIB;
-            const int c = ci0 + (ch * 32) % CIB;
-            if (co < p.Cout && tap < kk) {
-                float* o = orow + (long long)tap * p.Cin + c;
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                    if (c + j < p.Cin)  // Cin % 4 == 0
-                        *reinterpret_cast<float4*>(o + j) = make_float4(acc[j] * inv, acc[j + 1] * inv, acc[j + 2] * inv, acc[j + 3] * inv);
+            for (int j = 0; j < BN / 8; ++j) {
+                const int n = 8 * j + 2 * (lane & 3);
+                const int tap = tap0 + n / CIB;
+                const int c = ci0 + n % CIB;
+                if (tap < kk && c < p.Cin) {            // Cin % 64 == 0: c + 1 < Cin as well
+                    const int e = 4 * j + 2 * h;
+                    const float v0 = TERMS ? (acc[NR + e] + tot[e]) * inv : tot[e] * inv;
+                    const float v1 = TERMS ? (acc[NR + e + 1] + tot[e + 1]) * inv : tot[e + 1] * inv;
+                    *reinterpret_cast<float2*>(orow + (long long)tap * p.Cin + c) = make_float2(v0, v1);
+                }
             }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, (uint32_t)Cfg::TMEM_COLS);
     }
 }
 
@@ -451,7 +425,8 @@ static int make_tiled_map(CUtensorMap* map, const void* base, long long rows, lo
 // ---- tile plan of one convolution: which kernel flavour runs, its grid and the number of statistics rows
 //   mode bits 0-1 = TERMS (operand precision, see conv_tc_kernels.cuh), bit 4 = persistent tile loop (short-K only)
 struct TcPlan {
-    int bn, bk, nh, terms;
+    int bn, bk, terms;
+    bool fold;                       // long K: hi*hi k-blocks added to a register total (conv_tc_kernels.cuh)
     bool persist, cluster;
     int tiles_n, tiles_m, grid;      // tiles_m counts the padding tile of an odd tile count in cluster mode
     bool halo;                       // halo-tile kernel (conv_halo_kernels.cuh): 8 x 16 pixel tiles, persistent grid
@@ -477,7 +452,7 @@ static TcPlan tc_plan(long long M, int Cin, int Cout, int ksize, int mode, int B
     pl.tiles_x = pl.tiles_y = 0;
     if (pl.halo) {
         pl.bn = Cout <= 32 ? 32 : (Cout <= 64 ? 64 : 128);
-        pl.bk = 32; pl.nh = 1; pl.persist = true; pl.cluster = false;
+        pl.bk = 32; pl.fold = false; pl.persist = true; pl.cluster = false;
         pl.tiles_n = 1;
         pl.tiles_x = W / HALO_TW;
         pl.tiles_y = ceil_div(H, HALO_TH);
@@ -486,12 +461,12 @@ static TcPlan tc_plan(long long M, int Cin, int Cout, int ksize, int mode, int B
         pl.grid = (int)(total < kNumSMs ? total : kNumSMs);
         return pl;
     }
-    // layers up to this K run the short-K flavour (64-byte rows, two CTAs per SM).  FSDET_TC_SMALLK_MAX: developer knob for A/B runs
+    // layers up to this K run the short-K flavour (64-byte rows, one accumulation chain).  FSDET_TC_SMALLK_MAX: developer knob for A/B runs
     static const int small_k_max = [] { const char* e = getenv("FSDET_TC_SMALLK_MAX"); return e ? atoi(e) : 2304; }();
     const bool small_k = (Cin % 64 != 0) || (ksize * ksize * Cin <= small_k_max);
     pl.bn = Cout >= 128 ? 128 : 64;
     pl.bk = small_k ? 32 : 64;
-    pl.nh = (!small_k && pl.terms == 3) ? NHI : 1;
+    pl.fold = !small_k;
     pl.persist = small_k && (mode & 16);
     pl.tiles_n = ceil_div(Cout, pl.bn);
     pl.tiles_m = ceil_div(M, TC_BM);
@@ -508,13 +483,13 @@ static TcPlan tc_plan(long long M, int Cin, int Cout, int ksize, int mode, int B
     return pl;
 }
 
-template <int BN, int BK, int NH, int TERMS, bool PERSIST, int MINB>
+template <int BN, int BK, int TERMS, bool PERSIST, bool FOLD>
 static int launch_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi, const CUtensorMap& b_lo,
-                     const CUtensorMap& zmap, const TcArgs& a, int grid, bool cluster, cudaStream_t s) {
-    using Cfg = TcCfg<BN, BK, NH, TERMS, PERSIST, MINB>;
+                     const TcArgs& a, int grid, bool cluster, cudaStream_t s) {
+    using Cfg = TcCfg<BN, BK, TERMS, PERSIST>;
     if constexpr (!PERSIST) {
         if (cluster) {      // CTA pairs sharing the weight tile (TMA multicast)
-            auto kern = conv_tc_kernel<BN, BK, NH, TERMS, false, MINB, 2>;
+            auto kern = conv_tc_kernel<BN, BK, TERMS, false, FOLD, 2>;
             cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
             if (e != cudaSuccess) {
                 set_error("conv_tc(cluster): cudaFuncSetAttribute(%d bytes): %s", Cfg::SMEM_BYTES, cudaGetErrorString(e));
@@ -522,7 +497,7 @@ static int launch_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUt
             }
             cudaLaunchConfig_t cfg = {};
             cfg.gridDim = dim3((unsigned)grid);
-            cfg.blockDim = dim3(192);
+            cfg.blockDim = dim3(TC_THREADS);
             cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
             cfg.stream = s;
             cudaLaunchAttribute attr[1];
@@ -532,7 +507,7 @@ static int launch_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUt
             attr[0].val.clusterDim.z = 1;
             cfg.attrs = attr;
             cfg.numAttrs = 1;
-            e = cudaLaunchKernelEx(&cfg, kern, a_hi, a_lo, b_hi, b_lo, zmap, a);
+            e = cudaLaunchKernelEx(&cfg, kern, a_hi, a_lo, b_hi, b_lo, a);
             if (e != cudaSuccess) {
                 set_error("conv_tc(cluster): launch: %s", cudaGetErrorString(e));
                 return (int)e;
@@ -540,24 +515,24 @@ static int launch_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUt
             return launch_status("conv_tc(cluster)");
         }
     }
-    auto kern = conv_tc_kernel<BN, BK, NH, TERMS, PERSIST, MINB>;
+    auto kern = conv_tc_kernel<BN, BK, TERMS, PERSIST, FOLD>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
     if (e != cudaSuccess) {
         set_error("conv_tc: cudaFuncSetAttribute(%d bytes): %s", Cfg::SMEM_BYTES, cudaGetErrorString(e));
         return (int)e;
     }
-    kern<<<grid, 192, Cfg::SMEM_BYTES, s>>>(a_hi, a_lo, b_hi, b_lo, zmap, a);
+    kern<<<grid, TC_THREADS, Cfg::SMEM_BYTES, s>>>(a_hi, a_lo, b_hi, b_lo, a);
     return launch_status(PERSIST ? "conv_tc(persistent)" : "conv_tc");
 }
 
-template <int BN, int BK, int NH, bool PERSIST, int MINB>
+template <int BN, int BK, bool PERSIST, bool FOLD>
 static int launch_tc_terms(int terms, const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi,
-                           const CUtensorMap& b_lo, const CUtensorMap& zmap, const TcArgs& a, int grid, bool cluster, cudaStream_t s) {
+                           const CUtensorMap& b_lo, const TcArgs& a, int grid, bool cluster, cudaStream_t s) {
     switch (terms) {
-        case 0: return launch_tc<BN, BK, 1, 0, PERSIST, MINB>(a_hi, a_lo, b_hi, b_lo, zmap, a, grid, cluster, s);
-        case 1: return launch_tc<BN, BK, 1, 1, PERSIST, MINB>(a_hi, a_lo, b_hi, b_lo, zmap, a, grid, cluster, s);
-        case 2: return launch_tc<BN, BK, 1, 2, PERSIST, MINB>(a_hi, a_lo, b_hi, b_lo, zmap, a, grid, cluster, s);
-        default: return launch_tc<BN, BK, NH, 3, PERSIST, MINB>(a_hi, a_lo, b_hi, b_lo, zmap, a, grid, cluster, s);
+        case 0: return launch_tc<BN, BK, 0, PERSIST, FOLD>(a_hi, a_lo, b_hi, b_lo, a, grid, cluster, s);
+        case 1: return launch_tc<BN, BK, 1, PERSIST, FOLD>(a_hi, a_lo, b_hi, b_lo, a, grid, cluster, s);
+        case 2: return launch_tc<BN, BK, 2, PERSIST, FOLD>(a_hi, a_lo, b_hi, b_lo, a, grid, cluster, s);
+        default: return launch_tc<BN, BK, 3, PERSIST, FOLD>(a_hi, a_lo, b_hi, b_lo, a, grid, cluster, s);
     }
 }
 
@@ -578,25 +553,9 @@ static int make_halo_act_map(CUtensorMap* map, const void* base, int B, int H, i
     return 0;
 }
 
-// fp32 output [B][H][W][ldz] (first Cout channels): boxes of (32 channels, 8 x, 4 y), 128-byte swizzle
-static int make_halo_out_map(CUtensorMap* map, float* z, int B, int H, int W, int Cout, int ldz) {
-    cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)ldz * 4, (cuuint64_t)W * ldz * 4, (cuuint64_t)H * W * ldz * 4};
-    cuuint32_t box[4] = {32, (cuuint32_t)HALO_TW, 4, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = driver_fns().encodeTiled(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, z, dims, strides, box, estr,
-                                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        set_error("conv_halo: output tensor map failed (%d) B=%d H=%d W=%d Cout=%d ldz=%d", (int)r, B, H, W, Cout, ldz);
-        return -3;
-    }
-    return 0;
-}
-
 template <int BN, int NCH>
 static int launch_halo(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi, const CUtensorMap& b_lo,
-                       const CUtensorMap& zmap, const HaloArgs& a, int grid, cudaStream_t s) {
+                       const HaloArgs& a, int grid, cudaStream_t s) {
     constexpr bool BRES = NCH * BN <= 64;          // the whole weight operand (9 * NCH blocks of BN x 64 B x 2 planes) stays in shared memory
     using Cfg = HaloCfg<BN, NCH, BRES>;
     auto kern = conv_halo_kernel<BN, NCH, BRES>;
@@ -605,23 +564,23 @@ static int launch_halo(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const C
         set_error("conv_halo: cudaFuncSetAttribute(%d bytes): %s", Cfg::SMEM_BYTES, cudaGetErrorString(e));
         return (int)e;
     }
-    kern<<<grid, 352, Cfg::SMEM_BYTES, s>>>(a_hi, a_lo, b_hi, b_lo, zmap, a);
+    kern<<<grid, HALO_THREADS, Cfg::SMEM_BYTES, s>>>(a_hi, a_lo, b_hi, b_lo, a);
     return launch_status("conv_halo");
 }
 
 template <int BN>
 static int launch_halo_nch(int nch, const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi, const CUtensorMap& b_lo,
-                           const CUtensorMap& zmap, const HaloArgs& a, int grid, cudaStream_t s) {
+                           const HaloArgs& a, int grid, cudaStream_t s) {
     switch (nch) {
-        case 1: return launch_halo<BN, 1>(a_hi, a_lo, b_hi, b_lo, zmap, a, grid, s);
-        case 2: return launch_halo<BN, 2>(a_hi, a_lo, b_hi, b_lo, zmap, a, grid, s);
-        default: return launch_halo<BN, 4>(a_hi, a_lo, b_hi, b_lo, zmap, a, grid, s);
+        case 1: return launch_halo<BN, 1>(a_hi, a_lo, b_hi, b_lo, a, grid, s);
+        case 2: return launch_halo<BN, 2>(a_hi, a_lo, b_hi, b_lo, a, grid, s);
+        default: return launch_halo<BN, 4>(a_hi, a_lo, b_hi, b_lo, a, grid, s);
     }
 }
 
 static int run_halo(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, int B, const TcArgs& a, const TcPlan& pl,
                     cudaStream_t s) {
-    CUtensorMap a_hi, a_lo, b_hi, b_lo, zmap;
+    CUtensorMap a_hi, a_lo, b_hi, b_lo;
     int rc = make_halo_act_map(&a_hi, x_hi, B, a.H, a.W, a.Cin, a.cpitch);
     if (rc) return rc;
     rc = make_halo_act_map(&a_lo, x_lo, B, a.H, a.W, a.Cin, a.cpitch);
@@ -631,17 +590,15 @@ static int run_halo(const void* x_hi, const void* x_lo, const void* w_hi, const 
     if (rc) return rc;
     rc = make_tiled_map(&b_lo, w_lo, a.Cout, K, pl.bn, 32);
     if (rc) return rc;
-    rc = make_halo_out_map(&zmap, a.z, B, a.H, a.W, a.Cout, a.ldz);
-    if (rc) return rc;
     HaloArgs h;
-    h.amax_a = a.amax_a; h.amax_b = a.amax_b; h.stats = a.stats; h.H = a.H; h.W = a.W; h.Cout = a.Cout; h.cpitch = a.cpitch;
+    h.amax_a = a.amax_a; h.amax_b = a.amax_b; h.z = a.z; h.ldz = a.ldz; h.stats = a.stats; h.H = a.H; h.W = a.W; h.Cout = a.Cout; h.cpitch = a.cpitch;
     h.tiles_x = pl.tiles_x; h.tiles_y = pl.tiles_y; h.tiles_total = pl.tiles_m; h.accumulate = a.accumulate;
     const char* dbg = getenv("FSDET_HALO_FLAGS");      // developer knob (tools/halo_bench.py): see HaloArgs::flags
     h.flags = (dbg ? atoi(dbg) : 0) | (a.nofuse ? 4 : 0);
     const int nch = a.Cin / 32;
-    if (pl.bn == 32) return launch_halo_nch<32>(nch, a_hi, a_lo, b_hi, b_lo, zmap, h, pl.grid, s);
-    if (pl.bn == 64) return launch_halo_nch<64>(nch, a_hi, a_lo, b_hi, b_lo, zmap, h, pl.grid, s);
-    return launch_halo_nch<128>(nch, a_hi, a_lo, b_hi, b_lo, zmap, h, pl.grid, s);
+    if (pl.bn == 32) return launch_halo_nch<32>(nch, a_hi, a_lo, b_hi, b_lo, h, pl.grid, s);
+    if (pl.bn == 64) return launch_halo_nch<64>(nch, a_hi, a_lo, b_hi, b_lo, h, pl.grid, s);
+    return launch_halo_nch<128>(nch, a_hi, a_lo, b_hi, b_lo, h, pl.grid, s);
 }
 
 static int run_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, int B, TcArgs a, int mode, cudaStream_t s) {
@@ -664,34 +621,20 @@ static int run_tc(const void* x_hi, const void* x_lo, const void* w_hi, const vo
         rc = make_tiled_map(&b_lo, w_lo, a.Cout, K, b_rows, pl.bk);
         if (rc) return rc;
     }
-    CUtensorMap zmap;   // fp32 output [M][ldz] (first Cout columns): 32 x 32 boxes, 128-byte swizzle
-    {
-        cuuint64_t dims[2] = {(cuuint64_t)a.Cout, (cuuint64_t)a.M};
-        cuuint64_t strides[1] = {(cuuint64_t)a.ldz * 4};
-        cuuint32_t box[2] = {32, 32};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult r = driver_fns().encodeTiled(&zmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, a.z, dims, strides, box, estr,
-                                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                              CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) {
-            set_error("conv_tc: output tensor map failed (%d) M=%lld Cout=%d ldz=%d", (int)r, a.M, a.Cout, a.ldz);
-            return -3;
-        }
-    }
     a.tiles_n = pl.tiles_n;
     a.tiles_total = pl.tiles_n * pl.tiles_m;
     const int t = pl.terms;
     const bool cl = pl.cluster;
     if (pl.bk == 32) {
         if (pl.persist) {
-            if (pl.bn == 128) return launch_tc_terms<128, 32, 1, true, 1>(t, a_hi, a_lo, b_hi, b_lo, zmap, a, pl.grid, false, s);
-            return launch_tc_terms<64, 32, 1, true, 1>(t, a_hi, a_lo, b_hi, b_lo, zmap, a, pl.grid, false, s);
+            if (pl.bn == 128) return launch_tc_terms<128, 32, true, false>(t, a_hi, a_lo, b_hi, b_lo, a, pl.grid, false, s);
+            return launch_tc_terms<64, 32, true, false>(t, a_hi, a_lo, b_hi, b_lo, a, pl.grid, false, s);
         }
-        if (pl.bn == 128) return launch_tc_terms<128, 32, 1, false, 2>(t, a_hi, a_lo, b_hi, b_lo, zmap, a, pl.grid, cl, s);
-        return launch_tc_terms<64, 32, 1, false, 2>(t, a_hi, a_lo, b_hi, b_lo, zmap, a, pl.grid, cl, s);
+        if (pl.bn == 128) return launch_tc_terms<128, 32, false, false>(t, a_hi, a_lo, b_hi, b_lo, a, pl.grid, cl, s);
+        return launch_tc_terms<64, 32, false, false>(t, a_hi, a_lo, b_hi, b_lo, a, pl.grid, cl, s);
     }
-    if (pl.bn == 128) return launch_tc_terms<128, 64, NHI, false, 1>(t, a_hi, a_lo, b_hi, b_lo, zmap, a, pl.grid, cl, s);
-    return launch_tc_terms<64, 64, NHI, false, 1>(t, a_hi, a_lo, b_hi, b_lo, zmap, a, pl.grid, cl, s);
+    if (pl.bn == 128) return launch_tc_terms<128, 64, false, true>(t, a_hi, a_lo, b_hi, b_lo, a, pl.grid, cl, s);
+    return launch_tc_terms<64, 64, false, true>(t, a_hi, a_lo, b_hi, b_lo, a, pl.grid, cl, s);
 }
 
 }  // namespace fsdet
@@ -791,19 +734,17 @@ extern "C" int fsdet_conv_tc_fwd(const void* x_hi, const void* x_lo, const void*
     return run_tc(x_hi, x_lo, w_hi, w_lo, B, a, mode, (cudaStream_t)stream);
 }
 
-// tile shape of the weight-gradient kernel: Cin <= 64 packs two filter taps into one 128-wide N tile; the plain
-// fp16 x fp16 mode (terms == 0) uses 256-wide N tiles where the layer has the channels (operand bytes per FLOP halve)
-// (a tcgen05.mma narrower than 256 columns does not run faster than ~100 clocks - the 128 x 16 A tile it reads from shared
-// memory paces it - so the fp16 x fp16 mode always uses 256-wide tiles: 1, 2 or 4 filter taps side by side)
-static inline int wg_bn(int Cin, int terms) { return terms == 0 ? 256 : 128; }
-static inline int wg_taps(int Cin, int terms) { return terms == 0 ? (Cin >= 256 ? 1 : (Cin >= 128 ? 2 : 4)) : (Cin >= 128 ? 1 : 2); }
-static inline int wg_cib(int Cin, int terms) { return wg_bn(Cin, terms) / wg_taps(Cin, terms); }
+// tile shape of the weight-gradient kernel: 128-wide N tiles (two MMA warpgroups of 64 co x 128 keep a [hi | lo]
+// accumulator and the hi total in registers); Cin <= 64 packs two filter taps into one tile
+static inline int wg_taps(int Cin) { return Cin >= 128 ? 1 : 2; }
+static inline int wg_cib(int Cin) { return WG_BN / wg_taps(Cin); }
 
 // split-K factor of the weight gradient: every CTA is the same size (one CTA per SM), so the kernel takes
 // ceil(tiles * splits / SMs) rounds of 1 / splits of the pixels each - pick the smallest split count within 3 % of the best
-// rounds / splits ratio (297 CTAs on 148 SMs are three rounds, 294 are two; fewer splits = fewer partials to reduce)
+// rounds / splits ratio (265 CTAs on 132 SMs are three rounds, 264 are two; fewer splits = fewer partials to reduce)
 static int wg_splits(long long M, int Cin, int Cout, int ks, int terms) {
-    const int cib = wg_cib(Cin, terms), taps = wg_taps(Cin, terms);
+    (void)terms;
+    const int cib = wg_cib(Cin), taps = wg_taps(Cin);
     const long long tiles = (long long)((Cin + cib - 1) / cib) * ((ks * ks + taps - 1) / taps) * ((Cout + 127) / 128);
     long long maxs = (M + 511) / 512;  // at least 512 pixels (8 stages) per split
     if (maxs < 1) maxs = 1;
@@ -831,19 +772,19 @@ extern "C" size_t fsdet_conv_tc_wgrad_workspace_floats(int B, int H, int W, int 
     return splits > 1 ? (size_t)splits * Cout * ksize * ksize * Cin : 0;
 }
 
-template <int BN, int TAPS, int TERMS, int NH>
+template <int TAPS, int TERMS>
 static int launch_wg(const CUtensorMap& dhi, const CUtensorMap& dlo, const CUtensorMap& xhi, const CUtensorMap& xlo,
                      const TcWgArgs& a, int splits, cudaStream_t s) {
-    using Cfg = WgCfg<BN, TERMS, NH>;
-    auto kern = wgrad_tc_kernel<BN, TAPS, TERMS, NH>;
+    using Cfg = WgCfg<TERMS>;
+    auto kern = wgrad_tc_kernel<TAPS, TERMS>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
     if (e != cudaSuccess) {
         set_error("conv_tc_wgrad: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
         return (int)e;
     }
-    constexpr int CIB = BN / TAPS;
+    constexpr int CIB = WG_BN / TAPS;
     dim3 grid(((a.Cin + CIB - 1) / CIB) * ((a.ks * a.ks + TAPS - 1) / TAPS), (a.Cout + 127) / 128, splits);
-    kern<<<grid, 192, Cfg::SMEM_BYTES, s>>>(dhi, dlo, xhi, xlo, a);
+    kern<<<grid, 384, Cfg::SMEM_BYTES, s>>>(dhi, dlo, xhi, xlo, a);
     return launch_status("conv_tc_wgrad");
 }
 
@@ -851,10 +792,10 @@ template <int TAPS>
 static int launch_wg_terms(int terms, const CUtensorMap& dhi, const CUtensorMap& dlo, const CUtensorMap& xhi,
                            const CUtensorMap& xlo, const TcWgArgs& a, int splits, cudaStream_t s) {
     switch (terms) {
-        case 0: return launch_wg<128, TAPS, 0, 1>(dhi, dlo, xhi, xlo, a, splits, s);
-        case 1: return launch_wg<128, TAPS, 1, 1>(dhi, dlo, xhi, xlo, a, splits, s);
-        case 2: return launch_wg<128, TAPS, 2, 1>(dhi, dlo, xhi, xlo, a, splits, s);
-        default: return launch_wg<128, TAPS, 3, NHI>(dhi, dlo, xhi, xlo, a, splits, s);
+        case 0: return launch_wg<TAPS, 0>(dhi, dlo, xhi, xlo, a, splits, s);
+        case 1: return launch_wg<TAPS, 1>(dhi, dlo, xhi, xlo, a, splits, s);
+        case 2: return launch_wg<TAPS, 2>(dhi, dlo, xhi, xlo, a, splits, s);
+        default: return launch_wg<TAPS, 3>(dhi, dlo, xhi, xlo, a, splits, s);
     }
 }
 
@@ -907,12 +848,7 @@ extern "C" int fsdet_conv_tc_wgrad(const void* x_hi, const void* x_lo, const voi
         if (rc) return rc;
     }
     cudaStream_t s = (cudaStream_t)stream;
-    if (terms == 0) {
-        const int taps = wg_taps(Cin, 0);
-        if (taps == 1) rc = launch_wg<256, 1, 0, 2>(dhi, dlo, xhi, xlo, a, splits, s);
-        else if (taps == 2) rc = launch_wg<256, 2, 0, 2>(dhi, dlo, xhi, xlo, a, splits, s);
-        else rc = launch_wg<256, 4, 0, 2>(dhi, dlo, xhi, xlo, a, splits, s);
-    } else if (Cin < 128) {
+    if (wg_taps(Cin) == 2) {
         rc = launch_wg_terms<2>(terms, dhi, dlo, xhi, xlo, a, splits, s);
     } else {
         rc = launch_wg_terms<1>(terms, dhi, dlo, xhi, xlo, a, splits, s);

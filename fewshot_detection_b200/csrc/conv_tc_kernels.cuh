@@ -1,34 +1,32 @@
-// The tcgen05 implicit-GEMM convolution kernel (forward and input gradient) - included by conv_tc.cu after the PTX
+// The wgmma implicit-GEMM convolution kernel (forward and input gradient) - included by conv_tc.cu after the PTX
 // wrappers, and by tools/host_emul/conv_tc_emul.cpp after FUNCTIONAL MODELS of the same wrappers (mbarrier, TMA,
-// UMMA, TMEM, named barriers as host code), which is how its control flow - barrier phases, tile sequencing,
-// accumulator double buffering, operand-term selection, epilogue staging, the fused BatchNorm statistics - is
-// tested on the CPU (tests/test_conv_tc_host_emul.py).
+// wgmma, named barriers as host code), which is how its control flow - barrier phases, tile sequencing, operand-term
+// selection, the epilogue and the fused BatchNorm statistics - is tested on the CPU (tests/test_conv_tc_host_emul.py).
 //
 //   z[p][n] = sum_{tap,ci} x[p+tap][ci] * w[n][tap][ci]      (stride 1, "same" padding, k in {1,3})
 //
-// One CTA = 192 threads:
-//   warp 0   : TMA producer.  A tiles (128 output pixels x BK channels of one filter tap, zero-filled halo) come
-//              straight from the NHWC activation planes through an im2col tensor map, B tiles (BN output channels x
-//              BK) from the [Cout][K] weight planes; both land swizzled K-major in shared memory.
-//   warp 1   : allocates TMEM, issues tcgen05.mma (one elected thread), commits to mbarriers.
-//   warps 2-5: epilogue.  tcgen05.ld (lane = pixel) -> registers -> swizzled shared-memory staging -> TMA tensor
-//              store (reduce-add when accumulating), plus - for BatchNorm layers - the per-channel
-//              sum / sum of squares / min / max of z taken from the staged tile (fsdet_bn_finalize reads them), so
-//              that no separate statistics pass over z exists.
+// One CTA = three warpgroups (384 threads):
+//   warpgroup 0   : TMA producer (one warp).  A tiles (128 output pixels x BK channels of one filter tap, zero-filled
+//                   halo) come straight from the NHWC activation planes through an im2col tensor map, B tiles (BN output
+//                   channels x BK) from the [Cout][K] weight planes; both land swizzled K-major in shared memory.
+//   warpgroups 1-2: MMA + epilogue, 64 tile rows each.  wgmma reads both operands from shared memory and accumulates in
+//                   registers; the epilogue scales the accumulators, stores z rows (adds to them when accumulating) and -
+//                   for BatchNorm layers - folds the per-channel sum / sum of squares / min / max of z into one partial
+//                   row per CTA (fsdet_bn_finalize reads them), so that no separate statistics pass over z exists.
+//   Producer registers are handed to the MMA warpgroups (setmaxnreg).
 //
 // Operand precision (template parameter TERMS): every operand exists as two fp16 planes (hi, lo) of the tensor
 // scaled by a power of two; hi*hi is always issued, bit 0 of TERMS adds A_lo*B_hi, bit 1 adds A_hi*B_lo.  TERMS = 3
 // is fp32-grade (22 mantissa bits per operand), TERMS = 1 / 2 keep one operand exact and round the other to fp16
 // (relative rounding 2^-12 per element), TERMS = 0 is plain fp16 x fp16 -> fp32.  Only the planes that are used are
-// loaded.  With hi*hi products of successive k-blocks rotating over NH accumulators (the tensor core's fp32
-// accumulation truncates; NH > 1 only matters for TERMS = 3 and long K).
+// loaded.  FOLD (long K): the tensor core's fp32 accumulation truncates, so the hi*hi products of every k-block are
+// summed in a fresh accumulator and added to a register total with round-to-nearest; the small lo terms accumulate
+// over the whole K.
 //
-// PERSIST = false: one output tile per CTA (grid = number of tiles), the epilogue staging aliases the operand stages.
-// PERSIST = true : one CTA per SM walks tiles blockIdx.x, blockIdx.x + gridDim.x, ...; producer and MMA issuer run
-//              ahead across tile boundaries and the accumulators are double buffered in TMEM so that the epilogue of
-//              tile i overlaps the MMAs of tile i+1 (short-K layers, where the epilogue is a large share of a tile).
-//              gridDim.x must be a multiple of tiles_n (then every CTA keeps one channel range: the statistics are
-//              carried in registers across its tiles and written once).
+// PERSIST = false: one output tile per CTA (grid = number of tiles).
+// PERSIST = true : CTAs walk tiles blockIdx.x, blockIdx.x + gridDim.x, ...; the producer runs ahead across tile
+//              boundaries.  gridDim.x must be a multiple of tiles_n (then every CTA keeps one channel range: the
+//              statistics are carried in registers across its tiles and written once).
 #pragma once
 
 #ifdef FSDET_HOST_EMULATION
@@ -52,11 +50,11 @@ struct TcArgs {
 };
 
 constexpr int TC_BM = 128;
+constexpr int TC_THREADS = 384;   // producer warpgroup + two MMA warpgroups
 
-constexpr int tmem_cols(int n) { return n <= 32 ? 32 : (n <= 64 ? 64 : (n <= 128 ? 128 : (n <= 256 ? 256 : 512))); }
 constexpr int tc_max(int a, int b) { return a > b ? a : b; }
 
-template <int BN, int BK, int NH, int TERMS, bool PERSIST, int MINB>
+template <int BN, int BK, int TERMS, bool PERSIST>
 struct TcCfg {
     static constexpr int ROW_BYTES = BK * 2;
     static constexpr int A_BYTES = TC_BM * ROW_BYTES;
@@ -67,21 +65,13 @@ struct TcCfg {
     static constexpr int OFF_ALO = A_BYTES;
     static constexpr int OFF_BHI = NA * A_BYTES;
     static constexpr int OFF_BLO = OFF_BHI + B_BYTES;
-    static constexpr int EPI_BYTES = 4 * 2 * 4096;                  // 4 epilogue warps x two 32x32 fp32 staging tiles
-    static constexpr int STAT_BYTES = 4 * BN * 16;                  // 4 warps x BN channels x float4
-    static constexpr int TAIL_BYTES = EPI_BYTES + STAT_BYTES;
-    static constexpr int TOTAL_BUDGET = (MINB == 2 ? 113 : 227) * 1024 - 1024 /*align*/ - 256 /*barriers*/;
-    static constexpr int STAGE_BUDGET = PERSIST ? TOTAL_BUDGET - TAIL_BYTES : TOTAL_BUDGET;
-    static constexpr int STAGES = (STAGE_BUDGET / STAGE_BYTES) > 8 ? 8 : (STAGE_BUDGET / STAGE_BYTES);
-    static constexpr int EPI_OFF = PERSIST ? STAGES * STAGE_BYTES : 0;
-    static constexpr int BAR_OFF = PERSIST ? EPI_OFF + TAIL_BYTES : tc_max(STAGES * STAGE_BYTES, TAIL_BYTES);
-    static constexpr int NACC = NH + (TERMS ? 1 : 0);
-    static constexpr int ACC_COLS = NACC * BN;                      // one accumulator set
-    static constexpr int NSETS = PERSIST ? 2 : 1;
-    static constexpr int TMEM_COLS = tmem_cols(NSETS * ACC_COLS);
+    static constexpr int STAT_BYTES = 8 * BN * 16;                  // 8 MMA warps x BN channels x float4
+    static constexpr int BUDGET = 227 * 1024 - 1024 /*align*/ - 256 /*barriers*/;
+    static constexpr int STAGES = ((BUDGET - STAT_BYTES) / STAGE_BYTES) > 8 ? 8 : ((BUDGET - STAT_BYTES) / STAGE_BYTES);
+    static constexpr int STAT_OFF = STAGES * STAGE_BYTES;
+    static constexpr int BAR_OFF = STAT_OFF + STAT_BYTES;
     static constexpr int SMEM_BYTES = BAR_OFF + 1024 + 256;
     static_assert(STAGES >= 2, "at least two pipeline stages");
-    static_assert(NSETS * ACC_COLS <= 512, "accumulators must fit in TMEM");
     static_assert(STAGE_BYTES % 1024 == 0 && A_BYTES % 1024 == 0 && B_BYTES % 1024 == 0, "swizzle atoms need 1 KB alignment");
 };
 
@@ -93,84 +83,104 @@ __device__ __forceinline__ void tc_kahan_add(float& s, float& e, float x) {
     s = t;
 }
 
-// ---- epilogue building blocks (shared with conv_halo_kernels.cuh).  One epilogue warp handles 32 tile rows (its TMEM lane
-// quarter) x 32 columns at a time: TMEM -> registers -> 128-byte-swizzled 4 KB staging block -> TMA store, and - for
-// BatchNorm layers - the column statistics read back from the staged block.  Kept lean on purpose: at 128 x 64 tiles the
-// epilogue's instruction count, not the tensor pipe, paced the short-K kernels (profiles/ncu_r02b.md).
-
 // dynamic shared memory aligned to 1 KB WITHOUT leaving the shared address space (a round trip through uintptr_t makes
 // every later access a generic LD / ST)
 __device__ __forceinline__ uint8_t* tc_align_smem(uint8_t* raw) { return raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u); }
 
-// acc[j] = (hi[j] + lo[j]) * inv for the 32 columns at taddr_hi / taddr_lo (both loads in flight, one wait)
-template <bool HAS_LO>
-__device__ __forceinline__ void epi_load_scaled(uint32_t taddr_hi, uint32_t taddr_lo, float inv, float (&acc)[32]) {
-    uint32_t rh[32], rl[32];
-    if (HAS_LO) tmem_ld32_nowait(taddr_lo, rl);
-    tmem_ld32_nowait(taddr_hi, rh);
-    tmem_ld_wait();
-    if (HAS_LO) tmem_ld_use(rl);
-    tmem_ld_use(rh);
+// ---- epilogue (shared with conv_halo_kernels.cuh).  One MMA warp holds 16 rows x N columns of the accumulator in the
+// wgmma fragment layout: lane l has rows l / 4 and l / 4 + 8, columns 8j + 2 (l % 4) + {0, 1}.  z0 / z1 point at the
+// output rows of those two rows (nullptr: the row lies outside the tensor), cvalid = output channels left in this tile.
+// The values are scaled, stored as float2 (added to z when accumulating) and - with `wstat` - the column statistics of
+// the warp's valid rows go to wstat[0..N) (lanes with the same l % 4 combined by shuffles).
+template <int N, bool HAS_LO>
+__device__ __forceinline__ void epi_tile(const float* hi, const float* lo, float inv, float* z0, float* z1, int cvalid, int accumulate,
+                                         float4* wstat) {
+    const int lane = threadIdx.x & 31;
+    const bool ok0 = z0 != nullptr, ok1 = z1 != nullptr;
 #pragma unroll
-    for (int j = 0; j < 32; ++j) acc[j] = HAS_LO ? (__uint_as_float(rl[j]) + __uint_as_float(rh[j])) * inv : __uint_as_float(rh[j]) * inv;
-}
-
-// row `lane` of the 32 x 32 fp32 block into the staging buffer (16-byte chunk j of row r lives at chunk j ^ (r & 7))
-__device__ __forceinline__ void epi_stage_row(uint8_t* buf, int lane, const float (&acc)[32]) {
+    for (int j = 0; j < N / 8; ++j) {
+        const int c = 8 * j + 2 * (lane & 3);
+        float v[4];
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<float4*>(buf + lane * 128 + ((j ^ (lane & 7)) << 4)) = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
-}
-
-// statistics of column `lane` of a staged block over the rows whose bit is set in `vmask` (conflict-free: the 16-byte
-// chunks of a row are a permutation); four independent partial chains
-__device__ __forceinline__ void epi_col_stats(const uint8_t* buf, int lane, uint32_t vmask, float& s, float& q, float& mn, float& mx) {
-    const uint8_t* col = buf + (lane & 3) * 4;
-    const int cj = lane >> 2;
-    float ps[4] = {0.f, 0.f, 0.f, 0.f}, pq[4] = {0.f, 0.f, 0.f, 0.f};
-    float pmn[4] = {INFINITY, INFINITY, INFINITY, INFINITY}, pmx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-    if (vmask == 0xffffffffu) {
-#pragma unroll
-        for (int rr = 0; rr < 32; ++rr) {
-            const float v = *reinterpret_cast<const float*>(col + rr * 128 + ((cj ^ (rr & 7)) << 4));
-            ps[rr & 3] += v; pq[rr & 3] = fmaf(v, v, pq[rr & 3]); pmn[rr & 3] = fminf(pmn[rr & 3], v); pmx[rr & 3] = fmaxf(pmx[rr & 3], v);
+        for (int e = 0; e < 4; ++e) v[e] = HAS_LO ? (lo[4 * j + e] + hi[4 * j + e]) * inv : hi[4 * j + e] * inv;
+        if (c < cvalid) {
+            if (ok0) {
+                float2* o = reinterpret_cast<float2*>(z0 + c);
+                float2 w = make_float2(v[0], v[1]);
+                if (accumulate) { const float2 u = *o; w.x += u.x; w.y += u.y; }
+                *o = w;
+            }
+            if (ok1) {
+                float2* o = reinterpret_cast<float2*>(z1 + c);
+                float2 w = make_float2(v[2], v[3]);
+                if (accumulate) { const float2 u = *o; w.x += u.x; w.y += u.y; }
+                *o = w;
+            }
         }
-    } else {
+        if (wstat) {
+            float t[8];
 #pragma unroll
-        for (int rr = 0; rr < 32; ++rr) {
-            const float v = *reinterpret_cast<const float*>(col + rr * 128 + ((cj ^ (rr & 7)) << 4));
-            const bool ok = (vmask >> rr) & 1u;
-            ps[rr & 3] += ok ? v : 0.f; pq[rr & 3] = fmaf(ok ? v : 0.f, v, pq[rr & 3]);
-            pmn[rr & 3] = fminf(pmn[rr & 3], ok ? v : INFINITY); pmx[rr & 3] = fmaxf(pmx[rr & 3], ok ? v : -INFINITY);
+            for (int e = 0; e < 2; ++e) {
+                const float a = v[e], b = v[2 + e];
+                t[4 * e + 0] = (ok0 ? a : 0.f) + (ok1 ? b : 0.f);
+                t[4 * e + 1] = (ok0 ? a * a : 0.f) + (ok1 ? b * b : 0.f);
+                t[4 * e + 2] = fminf(ok0 ? a : INFINITY, ok1 ? b : INFINITY);
+                t[4 * e + 3] = fmaxf(ok0 ? a : -INFINITY, ok1 ? b : -INFINITY);
+            }
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    t[4 * e + 0] += __shfl_xor_sync(0xffffffffu, t[4 * e + 0], o);
+                    t[4 * e + 1] += __shfl_xor_sync(0xffffffffu, t[4 * e + 1], o);
+                    t[4 * e + 2] = fminf(t[4 * e + 2], __shfl_xor_sync(0xffffffffu, t[4 * e + 2], o));
+                    t[4 * e + 3] = fmaxf(t[4 * e + 3], __shfl_xor_sync(0xffffffffu, t[4 * e + 3], o));
+                }
+            }
+            if (lane < 4) {
+                wstat[c] = make_float4(t[0], t[1], t[2], t[3]);
+                wstat[c + 1] = make_float4(t[4], t[5], t[6], t[7]);
+            }
         }
     }
-    s = (ps[0] + ps[1]) + (ps[2] + ps[3]);
-    q = (pq[0] + pq[1]) + (pq[2] + pq[3]);
-    mn = fminf(fminf(pmn[0], pmn[1]), fminf(pmn[2], pmn[3]));
-    mx = fmaxf(fmaxf(pmx[0], pmx[1]), fmaxf(pmx[2], pmx[3]));
+}
+
+// statistics of one tile: the 8 MMA warps' column partials (sstat[warp][BN], written by epi_tile) folded in a fixed order
+// by consumer thread `ct` (< BN) into its compensated running sums; barrier 1 spans the 256 MMA threads
+template <int BN>
+__device__ __forceinline__ void epi_fold_stats(const float4* sstat, int ct, float& ssum, float& esum, float& ssq, float& esq,
+                                               float& smin, float& smax) {
+    named_bar_sync(1, 256);
+    if (ct < BN) {
+        float4 tt = sstat[ct];
+#pragma unroll
+        for (int w = 1; w < 8; ++w) {
+            const float4 o = sstat[w * BN + ct];
+            tt.x += o.x; tt.y += o.y; tt.z = fminf(tt.z, o.z); tt.w = fmaxf(tt.w, o.w);
+        }
+        tc_kahan_add(ssum, esum, tt.x);
+        tc_kahan_add(ssq, esq, tt.y);
+        smin = fminf(smin, tt.z);
+        smax = fmaxf(smax, tt.w);
+    }
+    named_bar_sync(1, 256);     // sstat is rewritten by the next tile
 }
 
 // CLUSTER = 2 (one-tile-per-CTA flavours only): two CTAs of a thread-block cluster work on two M tiles of the SAME
 // channel range; each loads its own activation tiles and only HALF of the weight tile, multicast into both CTAs'
-// shared memory - the weight operand crosses the L2 -> SM fabric once per pair instead of once per CTA (the 128 x 128
-// tiles of the 3-term scheme run at the L2 bandwidth limit on the mid-resolution layers).  A stage may be refilled
-// once BOTH CTAs' MMAs have consumed it (its empty barrier counts the two multicast commits).
-template <int BN, int BK, int NH, int TERMS, bool PERSIST, int MINB, int CLUSTER = 1>
-__global__ void __launch_bounds__(192, MINB)
+// shared memory - the weight operand crosses the L2 -> SM fabric once per pair instead of once per CTA.  A stage may be
+// refilled once BOTH CTAs' MMA warps have consumed it (its empty barrier counts the arrivals of both CTAs).
+template <int BN, int BK, int TERMS, bool PERSIST, bool FOLD, int CLUSTER = 1>
+__global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__ CUtensorMap tmAlo,
-               const __grid_constant__ CUtensorMap tmBhi, const __grid_constant__ CUtensorMap tmBlo,
-               const __grid_constant__ CUtensorMap tmZ, const TcArgs p) {
-    using Cfg = TcCfg<BN, BK, NH, TERMS, PERSIST, MINB>;
+               const __grid_constant__ CUtensorMap tmBhi, const __grid_constant__ CUtensorMap tmBlo, const TcArgs p) {
+    using Cfg = TcCfg<BN, BK, TERMS, PERSIST>;
     constexpr int STAGES = Cfg::STAGES;
-    constexpr int NSETS = Cfg::NSETS;
     FSDET_TC_DYN_SMEM(smem_raw);
     uint8_t* smem = tc_align_smem(smem_raw);
-    uint8_t* epi = smem + Cfg::EPI_OFF;
+    float4* sstat = reinterpret_cast<float4*>(smem + Cfg::STAT_OFF);   // [8 MMA warps][BN]
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::BAR_OFF);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* acc_full = empty_bar + STAGES;      // [NSETS] MMA issuer -> epilogue
-    uint64_t* acc_empty = acc_full + 2;           // [NSETS] epilogue (4 warps) -> MMA issuer
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -185,243 +195,164 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant_
     const int first_tile = CLUSTER == 2 ? (((int)(blockIdx.x >> 1) / tiles_n) * 2 + (int)crank) * tiles_n + (int)(blockIdx.x >> 1) % tiles_n
                                         : (int)blockIdx.x;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmAhi);
         if (TERMS & 1) tma_prefetch_desc(&tmAlo);
         tma_prefetch_desc(&tmBhi);
         if (TERMS & 2) tma_prefetch_desc(&tmBlo);
-        tma_prefetch_desc(&tmZ);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], CLUSTER);
-        }
-        for (int a = 0; a < NSETS; ++a) {
-            mbar_init(&acc_full[a], 1);
-            mbar_init(&acc_empty[a], 4);
+            mbar_init(&empty_bar[s], 8 * CLUSTER);     // every MMA warp of every CTA that reads the stage
         }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, (uint32_t)Cfg::TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
     if (CLUSTER == 2) cluster_sync_all();                      // the peer's barriers exist before anything remote touches them
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    // Both issuing roles run with their whole warp converged and issue under elect_one() (tc_ptx.cuh: no serialising loops
-    // around the TMA / MMA instructions, descriptors advance by one 32-bit add).
-    if (warp == 0) {
-        const int HW = p.H * p.W;
-        unsigned it = 0;                                   // k-blocks issued so far (all tiles)
+    if (warp < 4) {
+        regs_dec<40>();
+        if (warp == 0) {
+            // the producer warp runs converged and issues under elect_one() (tc_ptx.cuh)
+            const int HW = p.H * p.W;
+            unsigned it = 0;                                   // k-blocks issued so far (all tiles)
+            for (int tile = first_tile; tile < tiles_total; tile += tile_step) {
+                const int n_tile = tile % tiles_n;
+                const long long m0 = (long long)(tile / tiles_n) * TC_BM;
+                const int img = (int)(m0 / HW);
+                const int rem = (int)(m0 - (long long)img * HW);
+                const int ph = rem / p.W, pw = rem - ph * p.W;
+#pragma unroll 1
+                for (int kb = 0; kb < nk; ++kb, ++it) {
+                    const int s = it % STAGES;
+                    mbar_wait_warp(&empty_bar[s], ((it / STAGES) & 1) ^ 1);
+                    if (elect_one()) {
+                        uint8_t* st = smem + s * Cfg::STAGE_BYTES;
+                        mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
+                        const int tap = kb / kchunks;
+                        const int c0 = (kb - tap * kchunks) * BK;
+                        const int r = tap / p.ks, sx = tap - r * p.ks;
+                        tma_load_im2col_4d(st, &tmAhi, &full_bar[s], c0, pw - p.pad, ph - p.pad, img, (uint16_t)sx, (uint16_t)r);
+                        if (TERMS & 1)
+                            tma_load_im2col_4d(st + Cfg::OFF_ALO, &tmAlo, &full_bar[s], c0, pw - p.pad, ph - p.pad, img, (uint16_t)sx,
+                                               (uint16_t)r);
+                        if (CLUSTER == 2) {       // my half of the weight rows, delivered to both CTAs of the pair
+                            const int half = (int)crank * (BN / 2);
+                            tma_load_2d_mc(st + Cfg::OFF_BHI + half * Cfg::ROW_BYTES, &tmBhi, &full_bar[s], tap * p.cpitch + c0,
+                                           n_tile * BN + half, (uint16_t)3);
+                            if (TERMS & 2)
+                                tma_load_2d_mc(st + Cfg::OFF_BLO + half * Cfg::ROW_BYTES, &tmBlo, &full_bar[s], tap * p.cpitch + c0,
+                                               n_tile * BN + half, (uint16_t)3);
+                        } else {
+                            tma_load_2d(st + Cfg::OFF_BHI, &tmBhi, &full_bar[s], tap * p.cpitch + c0, n_tile * BN);
+                            if (TERMS & 2) tma_load_2d(st + Cfg::OFF_BLO, &tmBlo, &full_bar[s], tap * p.cpitch + c0, n_tile * BN);
+                        }
+                    }
+                    __syncwarp();
+                }
+            }
+        }
+    } else {
+        regs_inc<232>();
+        const int cw = (warp >> 2) - 1;                        // MMA warpgroup: tile rows 64 cw .. 64 cw + 63
+        const int wq = warp & 3;
+        const int ct = (int)threadIdx.x - 128;                 // 0 .. 255
+        constexpr int NR = BN / 2;                             // accumulator registers per thread and term
+        // TERMS = 3 with one hi accumulator: A_hi * [B_hi | B_lo] is ONE MMA of width 2*BN - the lo plane follows the hi
+        // plane in the stage and the lo accumulator follows the hi accumulator in registers (A_hi is read once)
+        constexpr bool CAN_FUSE = TERMS == 3 && !FOLD && 2 * BN <= 256;
+        const bool fused = CAN_FUSE && !p.nofuse;
+        constexpr uint32_t SWZ = BK == 64 ? GMMA_SW128 : GMMA_SW64;
+        constexpr uint32_t SBO = 8 * Cfg::ROW_BYTES;
+        const float inv = 1.f / (scale_from_amax(p.amax_a ? ldg_f32(p.amax_a) : 0.f) * scale_from_amax(p.amax_b ? ldg_f32(p.amax_b) : 0.f));
+        const bool want_stats = p.stats != nullptr;
+        float ssum = 0.f, esum = 0.f, ssq = 0.f, esq = 0.f, smin = INFINITY, smax = -INFINITY;
+        float acc[TERMS ? 2 * NR : NR];                        // [hi | lo]
+        float tot[FOLD ? NR : 1];                              // FOLD: round-to-nearest total of the hi*hi k-blocks
+        const uint32_t smem_base = smem_u32(smem);
+        // this warp has read stage `st` (its wgmma group is complete): one arrival per MMA warp of every CTA that reads it
+        auto release = [&](int st) {
+            __syncwarp();
+            if (lane == 0) {
+                if (CLUSTER == 2) {
+                    mbar_arrive_cluster(&empty_bar[st], 0u);
+                    mbar_arrive_cluster(&empty_bar[st], 1u);
+                } else {
+                    mbar_arrive(&empty_bar[st]);
+                }
+            }
+        };
+        int pend = -1;                                         // stage whose k-block group may still be in flight
+        unsigned it = 0;
         for (int tile = first_tile; tile < tiles_total; tile += tile_step) {
             const int n_tile = tile % tiles_n;
             const long long m0 = (long long)(tile / tiles_n) * TC_BM;
-            const int img = (int)(m0 / HW);
-            const int rem = (int)(m0 - (long long)img * HW);
-            const int ph = rem / p.W, pw = rem - ph * p.W;
+            if (FOLD) {
+#pragma unroll
+                for (int i = 0; i < NR; ++i) tot[i] = 0.f;
+            }
 #pragma unroll 1
             for (int kb = 0; kb < nk; ++kb, ++it) {
                 const int s = it % STAGES;
-                mbar_wait_warp(&empty_bar[s], ((it / STAGES) & 1) ^ 1);
-                if (elect_one()) {
-                    uint8_t* st = smem + s * Cfg::STAGE_BYTES;
-                    mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
-                    const int tap = kb / kchunks;
-                    const int c0 = (kb - tap * kchunks) * BK;
-                    const int r = tap / p.ks, sx = tap - r * p.ks;
-                    tma_load_im2col_4d(st, &tmAhi, &full_bar[s], c0, pw - p.pad, ph - p.pad, img, (uint16_t)sx, (uint16_t)r);
-                    if (TERMS & 1)
-                        tma_load_im2col_4d(st + Cfg::OFF_ALO, &tmAlo, &full_bar[s], c0, pw - p.pad, ph - p.pad, img, (uint16_t)sx,
-                                           (uint16_t)r);
-                    if (CLUSTER == 2) {       // my half of the weight rows, delivered to both CTAs of the pair
-                        const int half = (int)crank * (BN / 2);
-                        tma_load_2d_mc(st + Cfg::OFF_BHI + half * Cfg::ROW_BYTES, &tmBhi, &full_bar[s], tap * p.cpitch + c0,
-                                       n_tile * BN + half, (uint16_t)3);
-                        if (TERMS & 2)
-                            tma_load_2d_mc(st + Cfg::OFF_BLO + half * Cfg::ROW_BYTES, &tmBlo, &full_bar[s], tap * p.cpitch + c0,
-                                           n_tile * BN + half, (uint16_t)3);
+                mbar_wait(&full_bar[s], (it / STAGES) & 1);
+                const uint32_t st = smem_base + s * Cfg::STAGE_BYTES;
+                const uint64_t ah = gmma_desc(st + cw * 64 * Cfg::ROW_BYTES, 0, SBO, SWZ);
+                const uint64_t al = ah + (uint64_t)(Cfg::OFF_ALO >> 4);
+                const uint64_t bh = gmma_desc(st + Cfg::OFF_BHI, 0, SBO, SWZ);
+                const uint64_t bl = bh + (uint64_t)(Cfg::B_BYTES >> 4);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k) {            // 16 halves = 32 B along K inside the swizzle atom: + 2 in the descriptor
+                    const uint32_t first_hi = (FOLD ? k > 0 : (kb > 0 || k > 0)) ? 1u : 0u;
+                    const uint32_t first_lo = (kb > 0 || k > 0) ? 1u : 0u;
+                    const uint64_t adv = (uint64_t)(2 * k);
+                    if (CAN_FUSE && fused) {
+                        wgmma<CAN_FUSE ? 2 * BN : BN>(acc, ah + adv, bh + adv, first_hi);
+                        wgmma<BN>(acc + NR, al + adv, bh + adv, 1u);
                     } else {
-                        tma_load_2d(st + Cfg::OFF_BHI, &tmBhi, &full_bar[s], tap * p.cpitch + c0, n_tile * BN);
-                        if (TERMS & 2) tma_load_2d(st + Cfg::OFF_BLO, &tmBlo, &full_bar[s], tap * p.cpitch + c0, n_tile * BN);
+                        wgmma<BN>(acc, ah + adv, bh + adv, first_hi);
+                        if (TERMS & 1) wgmma<BN>(acc + NR, al + adv, bh + adv, first_lo);
+                        if (TERMS & 2) wgmma<BN>(acc + NR, ah + adv, bl + adv, (TERMS & 1) ? 1u : first_lo);
                     }
                 }
-                __syncwarp();
-            }
-        }
-    } else if (warp == 1) {
-        // instruction descriptors: D=f32, A=B=f16, both K-major, M=128, N=BN (and N=2*BN for the fused hi|lo MMA)
-        const uint32_t idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-        const uint32_t idesc2 = (1u << 4) | ((uint32_t)(2 * BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-        constexpr uint32_t HI = BK == 64 ? UMMA_DESC_HI_K_SW128 : UMMA_DESC_HI_K_SW64;
-        // TERMS = 3 with one hi accumulator: A_hi * [B_hi | B_lo] is ONE MMA of width 2*BN - the lo plane follows the hi
-        // plane in the stage and the lo accumulator follows the hi accumulator in TMEM (A_hi is read once, two MMAs per K step)
-        // With rotating hi accumulators (NH > 1, long K) the fused form keeps TWO (hi | lo) pairs [hi0 | lo0 | hi1 | lo1] -
-        // the same 4 * BN TMEM columns as [hi0 | hi1 | hi2 | lo] - and k-block kb accumulates into pair kb % 2.
-        constexpr bool CAN_FUSE = TERMS == 3 && 2 * BN <= 256 && (NH == 1 || NH == 3);
-        const bool fused = CAN_FUSE && !p.nofuse;
-        const uint32_t smem_base = smem_u32(smem);
-        unsigned it = 0;
-        unsigned t = 0;                                    // tiles done by this CTA
-        for (int tile = first_tile; tile < tiles_total; tile += tile_step, ++t) {
-            const unsigned a = t % NSETS;
-            mbar_wait_warp(&acc_empty[a], ((t / NSETS) & 1u) ^ 1u);    // the epilogue has drained this accumulator set
-            tc_fence_after();
-            const uint32_t acc = tmem_base + a * (uint32_t)Cfg::ACC_COLS;
-#pragma unroll 1
-            for (int kb = 0; kb < nk; ++kb, ++it) {
-                const int s = it % STAGES;
-                mbar_wait_warp(&full_bar[s], (it / STAGES) & 1);
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint32_t ah = umma_desc_lo(smem_base + s * Cfg::STAGE_BYTES);
-                    const uint32_t al = ah + (uint32_t)(Cfg::OFF_ALO >> 4);
-                    const uint32_t bh = ah + (uint32_t)(Cfg::OFF_BHI >> 4);
-                    const uint32_t bl = ah + (uint32_t)(Cfg::OFF_BLO >> 4);
-                    const uint32_t dhi = acc + (uint32_t)((kb % NH) * BN);
-                    const uint32_t dlo = acc + (uint32_t)(NH * BN);
-                    constexpr int NP = NH == 1 ? 1 : 2;            // (hi | lo) accumulator pairs of the fused form
-                    const uint32_t dpair = acc + (uint32_t)((kb % NP) * 2 * BN);
+                wgmma_commit();
+                if (FOLD) {                                    // the k-block's hi sum is read now: wait for all of it
+                    wgmma_wait<0>();
+                    wgmma_use<TERMS ? 2 * NR : NR>(acc);
+                    release(s);
 #pragma unroll
-                    for (uint32_t k = 0; k < BK / 16; ++k) {       // 16 halves = 32 B along K inside the swizzle atom: + 2 in the descriptor
-                        const uint32_t first_hi = (kb >= NH || k > 0) ? 1u : 0u;
-                        const uint32_t first_lo = (kb > 0 || k > 0) ? 1u : 0u;
-                        if (fused) {
-                            umma_f16_lohi(dpair, ah + 2 * k, HI, bh + 2 * k, HI, idesc2, (kb >= NP || k > 0) ? 1u : 0u);
-                            umma_f16_lohi(dpair + BN, al + 2 * k, HI, bh + 2 * k, HI, idesc, 1u);
-                        } else {
-                            umma_f16_lohi(dhi, ah + 2 * k, HI, bh + 2 * k, HI, idesc, first_hi);
-                            if (TERMS & 1) umma_f16_lohi(dlo, al + 2 * k, HI, bh + 2 * k, HI, idesc, first_lo);
-                            if (TERMS & 2) umma_f16_lohi(dlo, ah + 2 * k, HI, bl + 2 * k, HI, idesc, (TERMS & 1) ? 1u : first_lo);
-                        }
-                    }
-                    if (CLUSTER == 2) umma_commit_mc(&empty_bar[s], (uint16_t)3);   // both producers write into this CTA's slot
-                    else umma_commit(&empty_bar[s]);   // frees the smem slot when these MMAs have read it
-                }
-                __syncwarp();
-            }
-            if (elect_one()) umma_commit(&acc_full[a]);        // accumulator set complete
-            __syncwarp();
-        }
-    } else {
-        // epilogue warps 2..5 -> TMEM lane quarters (warp % 4); each warp owns 32 output pixels of the tile
-        const int quarter = warp & 3;
-        const bool leader = elect_one();                       // issues (and later waits for) this warp's TMA stores
-        const float inv = 1.f / (scale_from_amax(p.amax_a ? ldg_f32(p.amax_a) : 0.f) * scale_from_amax(p.amax_b ? ldg_f32(p.amax_b) : 0.f));
-        const int nhi = nk < NH ? nk : NH;
-        uint8_t* stage_buf = epi + quarter * 8192;             // two 4 KB buffers per warp
-        const bool want_stats = p.stats != nullptr;
-        float ssum[BN / 32], esum[BN / 32], ssq[BN / 32], esq[BN / 32], smin[BN / 32], smax[BN / 32];
-#pragma unroll
-        for (int c = 0; c < BN / 32; ++c) { ssum[c] = esum[c] = ssq[c] = esq[c] = 0.f; smin[c] = INFINITY; smax[c] = -INFINITY; }
-        unsigned t = 0, stores = 0;                            // tiles done, TMA stores issued by this warp
-        for (int tile = first_tile; tile < tiles_total; tile += tile_step, ++t) {
-            const unsigned a = t % NSETS;
-            const int n_tile = tile % tiles_n;
-            const long long m0 = (long long)(tile / tiles_n) * TC_BM;
-            const long long mrow = m0 + quarter * 32;
-            mbar_wait(&acc_full[a], (t / NSETS) & 1u);
-            tc_fence_after();
-            const long long left = p.M - mrow;                 // rows beyond the tensor's last pixel are excluded from the statistics
-            const uint32_t vmask = left >= 32 ? 0xffffffffu : (left > 0 ? ((1u << (int)left) - 1u) : 0u);
-#pragma unroll
-            for (int ch = 0; ch < BN / 32; ++ch) {
-                const int n0 = n_tile * BN + ch * 32;
-                if (n0 < p.Cout && mrow < p.M) {               // warp-uniform
-                    float acc[32];
-                    const uint32_t taddr = tmem_base + a * (uint32_t)Cfg::ACC_COLS + ((uint32_t)(quarter * 32) << 16) + ch * 32;
-                    if constexpr (NH == 1) {
-                        epi_load_scaled<TERMS != 0>(taddr, taddr + NH * BN, inv, acc);
-                    } else if (TERMS == 3 && NH == 3 && 2 * BN <= 256 && !p.nofuse) {
-                        // fused pairs [hi0 | lo0 | hi1 | lo1]: lo terms first (small), then the two hi*hi partial sums
-                        float t2[32];
-                        if (nk > 1) {
-                            epi_load_scaled<true>(taddr + BN, taddr + 3 * BN, 1.f, acc);        // lo0 + lo1
-                            epi_load_scaled<true>(taddr, taddr + 2 * BN, 1.f, t2);              // hi0 + hi1
-                        } else {                                                            // a single k-block never touches pair 1
-                            epi_load_scaled<false>(taddr + BN, 0u, 1.f, acc);
-                            epi_load_scaled<false>(taddr, 0u, 1.f, t2);
-                        }
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) acc[j] = (acc[j] + t2[j]) * inv;
-                    } else {                                   // lo terms first (small), then the rotating hi*hi partial sums
-                        uint32_t r[32];
-                        if constexpr (TERMS != 0) {
-                            tmem_ld32(taddr + NH * BN, r);
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) acc[j] = __uint_as_float(r[j]);
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-                        }
-                        for (int h = nhi - 1; h >= 0; --h) {
-                            tmem_ld32(taddr + h * BN, r);
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) acc[j] += __uint_as_float(r[j]);
-                        }
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) acc[j] *= inv;
-                    }
-                    uint8_t* buf = stage_buf + (stores & 1u) * 4096;
-                    if (stores >= 2) {                         // the store that last read this buffer must have drained
-                        if (leader) tma_store_wait_read<1>();
-                        __syncwarp();
-                    }
-                    epi_stage_row(buf, lane, acc);
-                    fence_proxy_async();
-                    __syncwarp();
-                    if (leader) {
-                        if (p.accumulate) tma_reduce_add_2d(&tmZ, buf, n0, (int)mrow);
-                        else tma_store_2d(&tmZ, buf, n0, (int)mrow);
-                        tma_store_commit();
-                    }
-                    ++stores;
-                    if (want_stats) {
-                        float s, q, mn, mx;
-                        epi_col_stats(buf, lane, vmask, s, q, mn, mx);
-                        tc_kahan_add(ssum[ch], esum[ch], s);
-                        tc_kahan_add(ssq[ch], esq[ch], q);
-                        smin[ch] = fminf(smin[ch], mn);
-                        smax[ch] = fmaxf(smax[ch], mx);
-                    }
+                    for (int i = 0; i < NR; ++i) tot[i] += acc[i];
+                } else {                                       // one k-block stays in flight: the previous one has read its stage
+                    wgmma_wait<1>();
+                    if (pend >= 0) release(pend);
+                    pend = s;
                 }
             }
-            // this warp's TMEM reads of set `a` are complete (tcgen05.wait::ld in tmem_ld32): hand the set back
-            tc_fence_before();
-            __syncwarp();
-            if (leader) mbar_arrive(&acc_empty[a]);
+            if (!FOLD) {
+                wgmma_wait<0>();
+                wgmma_use<TERMS ? 2 * NR : NR>(acc);
+                if (pend >= 0) release(pend);
+                pend = -1;
+            }
+            if (nk == 0) {
+#pragma unroll
+                for (int i = 0; i < (TERMS ? 2 * NR : NR); ++i) acc[i] = 0.f;
+            }
+            const long long r0 = m0 + 64 * cw + 16 * wq + (lane >> 2), r1 = r0 + 8;
+            float* z0 = r0 < p.M ? p.z + r0 * p.ldz + n_tile * BN : nullptr;
+            float* z1 = r1 < p.M ? p.z + r1 * p.ldz + n_tile * BN : nullptr;
+            epi_tile<BN, TERMS != 0>(FOLD ? tot : acc, acc + NR, inv, z0, z1, p.Cout - n_tile * BN, p.accumulate,
+                                     want_stats ? sstat + (warp - 4) * BN : nullptr);
+            if (want_stats) epi_fold_stats<BN>(sstat, ct, ssum, esum, ssq, esq, smin, smax);
         }
-        if (leader) tma_store_wait_read<0>();               // shared memory must outlive the bulk reads
-        __syncwarp();
-        if (want_stats) {
-            // fold the four warps (pixel quarters) in a fixed order and write this CTA's partial row
-            float4* sbuf = reinterpret_cast<float4*>(epi + Cfg::EPI_BYTES);   // [4][BN]
-#pragma unroll
-            for (int ch = 0; ch < BN / 32; ++ch)
-                sbuf[quarter * BN + ch * 32 + lane] = make_float4(ssum[ch] - esum[ch], ssq[ch] - esq[ch], smin[ch], smax[ch]);
-            named_bar_sync(1, 128);
-            const int e = (warp - 2) * 32 + lane;
-            const int n_tile = CLUSTER == 2 ? first_tile % tiles_n : (int)(blockIdx.x % (unsigned)tiles_n);
-            const long long row = CLUSTER == 2 ? (long long)(first_tile / tiles_n) : (long long)(blockIdx.x / (unsigned)tiles_n);
-            for (int c = e; c < BN; c += 128) {
-                float4 tt = sbuf[c];
-#pragma unroll
-                for (int qq = 1; qq < 4; ++qq) {
-                    const float4 o = sbuf[qq * BN + c];
-                    tt.x += o.x; tt.y += o.y; tt.z = fminf(tt.z, o.z); tt.w = fmaxf(tt.w, o.w);
-                }
-                const int n = n_tile * BN + c;
-                if (n < p.Cout) {
-                    float* dst = p.stats + row * 4 * p.Cout + n;
-                    dst[0] = tt.x; dst[p.Cout] = tt.y; dst[2 * p.Cout] = tt.z; dst[3 * p.Cout] = tt.w;
-                }
+        if (want_stats && ct < BN) {
+            // this CTA's partial row (one channel range: persistent grids are a multiple of tiles_n)
+            const int n = (first_tile % tiles_n) * BN + ct;
+            const long long row = PERSIST ? (long long)(blockIdx.x / (unsigned)tiles_n) : (long long)(first_tile / tiles_n);
+            if (n < p.Cout) {
+                float* dst = p.stats + row * 4 * p.Cout + n;
+                dst[0] = ssum - esum; dst[p.Cout] = ssq - esq; dst[2 * p.Cout] = smin; dst[3 * p.Cout] = smax;
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
     if (CLUSTER == 2) cluster_sync_all();                      // no CTA leaves while its peer may still signal its barriers
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, (uint32_t)Cfg::TMEM_COLS);
-    }
 }

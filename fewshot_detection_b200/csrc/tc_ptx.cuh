@@ -1,4 +1,4 @@
-// PTX wrappers of the tcgen05 / TMA / mbarrier instructions used by the tensor-core kernels (conv_tc.cu,
+// PTX wrappers of the wgmma / TMA / mbarrier instructions used by the tensor-core kernels (conv_tc.cu,
 // conv_first_tc.cu).  Device code only; included inside namespace fsdet.  The host-emulation builds
 // (tools/host_emul/*_emul.cpp) provide functional models with the same names instead of this file.
 #pragma once
@@ -39,9 +39,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void mbar_wait_warp(uint64_t* bar, uint32_t parity) { mbar_wait(bar, parity); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
 __device__ __forceinline__ void tma_load_im2col_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c, int w, int h,
                                                    int n, uint16_t off_w, uint16_t off_h) {
     asm volatile(
@@ -57,19 +54,8 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
         "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* smem_src, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(map)),
-                 "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-                 : "memory");
-}
-__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* map, const void* smem_src, int c0, int c1) {
-    asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                     reinterpret_cast<uint64_t>(map)),
-                 "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-                 : "memory");
-}
 // ---- tiled 4-D (channel, x, y, image) boxes of an NHWC tensor: the halo-tile kernels (conv_halo_kernels.cuh).
-// Coordinates are signed; elements outside the tensor are zero-filled on loads and dropped on stores.
+// Coordinates are signed; elements outside the tensor are zero-filled.
 __device__ __forceinline__ void tma_load_tiled_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c, int w, int h, int n) {
     asm volatile(
         "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
@@ -77,31 +63,13 @@ __device__ __forceinline__ void tma_load_tiled_4d(void* smem_dst, const CUtensor
         "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c), "r"(w), "r"(h), "r"(n)
         : "memory");
 }
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* smem_src, int c, int w, int h, int n) {
-    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
-                     reinterpret_cast<uint64_t>(map)),
-                 "r"(smem_u32(smem_src)), "r"(c), "r"(w), "r"(h), "r"(n)
-                 : "memory");
-}
-__device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap* map, const void* smem_src, int c, int w, int h, int n) {
-    asm volatile("cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
-                     reinterpret_cast<uint64_t>(map)),
-                 "r"(smem_u32(smem_src)), "r"(c), "r"(w), "r"(h), "r"(n)
-                 : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
 
-// One lane of a CONVERGED warp (elect.sync).  The issuing roles run their loops with the whole warp and put only the
-// TMA / MMA / commit instructions under `if (elect_one())`: the compiler then knows that a single thread executes them
-// and takes their operands from uniform registers directly.  Under `if (lane == 0)` it cannot know, and wraps every such
-// instruction in a serialising ELECT / R2UR / BRA.U.ANY loop - measured at ~100 clocks per tcgen05.mma issued
-// (profiles/ncu_r02b.md), i.e. issue-bound for every tile narrower than 256 columns.
+// One lane of a CONVERGED warp (elect.sync).  The producer warps run their loops with the whole warp and put only the
+// TMA instructions under `if (elect_one())`: the compiler then knows that a single thread executes them and takes their
+// operands from uniform registers directly, instead of wrapping each in a serialising loop as under `if (lane == 0)`.
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile(
@@ -114,122 +82,81 @@ __device__ __forceinline__ bool elect_one() {
     return pred != 0;
 }
 
-// shared-memory matrix descriptors as (lo, hi) words: hi is constant per layout, lo = ((address >> 4) & 0x3fff) | LBO << 16 -
-// advancing inside a tile is one 32-bit add of (bytes >> 4) to lo (addresses < 256 KB never carry into the LBO field)
-__device__ __forceinline__ uint32_t umma_desc_lo(uint32_t saddr) { return ((saddr & 0x3FFFF) >> 4) | (1u << 16); }
-constexpr uint32_t UMMA_DESC_HI_K_SW64 = (512u >> 4) | (1u << 14) | (4u << 29);      // SBO 512 B, version 1, SWIZZLE_64B
-constexpr uint32_t UMMA_DESC_HI_K_SW128 = (1024u >> 4) | (1u << 14) | (2u << 29);    // SBO 1024 B, version 1, SWIZZLE_128B
-__device__ __forceinline__ void umma_f16_lohi(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                              uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t"
-        "}" ::"r"(tmem_d),
-        "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// K-major, 128-byte swizzle shared-memory matrix descriptor (tile rows of 128 B, 8-row groups 1024 B apart)
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);       // start address  [0,14)
-    d |= (uint64_t)1 << 16;                        // leading byte offset (ignored for swizzled K-major) [16,30)
-    d |= (uint64_t)(1024 >> 4) << 32;              // stride byte offset: 8 rows x 128 B            [32,46)
-    d |= (uint64_t)1 << 46;                        // descriptor version (Blackwell)               [46,48)
-    d |= (uint64_t)2 << 61;                        // SWIZZLE_128B                                  [61,64)
-    return d;
-}
-
-// K-major, 64-byte swizzle (tile rows of 64 B = 32 halves, 8-row groups 512 B apart)
-__device__ __forceinline__ uint64_t umma_desc_k_sw64(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(512 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)4 << 61;                        // SWIZZLE_64B
-    return d;
-}
-
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32"
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, "
-        "%25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// the same load without the wait: several loads in flight, then ONE tmem_ld_wait(), then tmem_ld_use(r) on every
-// register array before its values are read (a zero-cost volatile dependency: keeps the compiler from scheduling
-// consumers above the wait)
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32"
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, "
-        "%25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_use(uint32_t (&r)[32]) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) asm volatile("" : "+r"(r[j]));
-}
-
-// ------------------------------------------------------------------ wrappers used by conv_tc_kernels.cuh
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot, uint32_t cols) {   // whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "r"(cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t base, uint32_t cols) {   // whole warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(base), "r"(cols));
-}
 __device__ __forceinline__ float ldg_f32(const float* p) { return __ldg(p); }
-// barrier over `nthreads` threads of the CTA (the epilogue warps), id 1..15
+// barrier over `nthreads` threads of the CTA (the MMA warpgroups), id 1..15
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// MN-major, 128-byte swizzle shared-memory matrix descriptor: a row = one K index (pixel), 64 M/N elements = 128 B;
-// `lbo_bytes` = distance to the next 64-element block along M/N, 8-row groups 1024 B apart along K
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t saddr, uint32_t lbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-    d |= (uint64_t)(lbo_bytes >> 4) << 16;         // next 64-channel block along M/N
-    d |= (uint64_t)(1024 >> 4) << 32;              // next group of 8 pixels along K
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;                        // SWIZZLE_128B
-    return d;
+// ------------------------------------------------------------------ wgmma (sm_90a warpgroup MMA)
+// Shared-memory matrix descriptor: start address, leading / stride byte offsets, swizzle mode (1 = 128 B, 2 = 64 B).
+//   K-major, swizzled: rows of 128 B (or 64 B) along K, 8-row groups SBO apart (LBO unused).
+//   MN-major, swizzled: a row = one K index holding 64 M/N elements (128 B), 8-row groups SBO apart along K, the next
+//   64-element block along M/N LBO bytes further.
+// Advancing inside a tile is an add of (bytes >> 4) to the descriptor (addresses < 256 KB never carry out of the field).
+constexpr uint32_t GMMA_SW128 = 1, GMMA_SW64 = 2;
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo, uint32_t swz) {
+    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32) | ((uint64_t)swz << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving reads of the accumulators above the wait that completes them
+template <int R>
+__device__ __forceinline__ void wgmma_use(float* d) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// register budget of a warpgroup (producer warpgroups give registers to the MMA warpgroups)
+template <int R> __device__ __forceinline__ void regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], fp16 operands from shared memory, fp32 accumulators in registers (N / 2 per
+// thread of the warpgroup: d[4j + {0,1}] = row 16 * warp + lane / 4, columns 8j + 2 * (lane % 4) + {0, 1}; d[4j + {2,3}] =
+// the same columns 8 rows further down).  TA / TB = 1: that operand is MN-major.  accumulate = 0 overwrites D.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n32(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n64(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n128(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n256(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %131, %132;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+}
+template <int N, int TA = 0, int TB = 0>
+__device__ __forceinline__ void wgmma(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    static_assert(N == 32 || N == 64 || N == 128 || N == 256, "wgmma width");
+    if constexpr (N == 32) wgmma_n32<TA, TB>(d, da, db, accumulate);
+    else if constexpr (N == 64) wgmma_n64<TA, TB>(d, da, db, accumulate);
+    else if constexpr (N == 128) wgmma_n128<TA, TB>(d, da, db, accumulate);
+    else wgmma_n256<TA, TB>(d, da, db, accumulate);
 }
 
 // ---- thread-block clusters (2 CTAs sharing the weight tile through TMA multicast)
@@ -251,9 +178,12 @@ __device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap
         "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
         : "memory");
 }
-// tcgen05.commit arriving on the mbarrier at the same offset of every CTA in `cta_mask`
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-                 "h"(cta_mask)
-                 : "memory");
+// arrive on the mbarrier at the same shared-memory offset of CTA `cta` of the cluster (possibly this one)
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+    asm volatile(
+        "{\n\t.reg .b32 ra;\n\t"
+        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
+        "r"(cta)
+        : "memory");
 }

@@ -1,6 +1,6 @@
 // Per-step preparation of ALL convolution weights of a network for the tensor-core kernels, in two launches.
 //
-// The tcgen05 convolutions read their weight operand as scaled fp16 (hi, lo) planes, the forward GEMM in OHWI order
+// The tensor-core convolutions read their weight operand as scaled fp16 (hi, lo) planes, the forward GEMM in OHWI order
 // [Cout][tap][Cin], the input-gradient GEMM flip-transposed [Cin][kk-1-tap][Cout] (the weights of the transposed
 // convolution; nn.Conv2d's autograd does the same inside cuDNN, darknet_meta.py:236-252).  Round 1 produced them per
 // use with four small launches per layer (amax, split, flip-transpose, split: ~120 launches per step); here one

@@ -1,5 +1,5 @@
 """`Darknet(cfgfile)`: the plain YOLOv2 cfg interpreter of the reference
-(darknet.py:61-341) on the B200-native engine (BASELINE config #1,
+(darknet.py:61-341) on the H100-native engine (BASELINE config #1,
 cfg/tiny-yolo-voc.cfg).  Same surface: `.blocks .models .loss .width .height
 .anchors .num_anchors .anchor_step .num_classes .header .seen`, `forward(x)`,
 `load_weights`, `save_weights`, `print_network`.  CUDA only."""

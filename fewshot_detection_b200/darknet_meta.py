@@ -1,5 +1,5 @@
 """`Darknet(darknet_file, learnet_file)`: the meta-detector of the reference
-(darknet_meta.py:86-482) on the B200-native engine.
+(darknet_meta.py:86-482) on the H100-native engine.
 
 Kept from the reference so that train_meta.py / valid_ensemble.py drop in:
 constructor arguments (cfg path or parsed block list, darknet_meta.py:87-90),
@@ -13,7 +13,7 @@ same), and `nn.Module` behaviour (.cuda(), .train(), .eval()).
 
 New underneath: nn.Conv2d / nn.BatchNorm2d are only parameter containers here;
 the forward and backward passes are executed by engine.NetRunner with
-hand-written sm_100a kernels (libfsdet.so).  CUDA only - no CPU fallback.
+hand-written sm_90a kernels (libfsdet.so).  CUDA only - no CPU fallback.
 """
 import numpy as np
 import torch

@@ -3,9 +3,9 @@ buckets, overlapped with the backward pass.
 
 The reference's only multi-GPU path is single-process `nn.DataParallel`
 (train_meta.py:137-141): replicate parameters, scatter inputs, gather outputs,
-reduce gradients onto GPU 0 every step.  The B200-native equivalent is one
+reduce gradients onto GPU 0 every step.  The H100-native equivalent is one
 process per GPU with identical replicas and a single sum-all-reduce of the 66 M
-fp32 gradients over NVLink 5 / NVSwitch: no broadcast, no scatter, no gather.
+fp32 gradients over NVLink / NVSwitch: no broadcast, no scatter, no gather.
 Gradients are *summed* (the reference's losses are sums, region_loss.py:340-345,
 and the driver divides lr by the global batch, train_meta.py:143-147).
 

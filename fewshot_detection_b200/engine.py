@@ -3,7 +3,7 @@
 The reference interprets its block list with one torch module per block
 (darknet_meta.py:130-195, darknet.py:80-129) and lets autograd + cuDNN do the
 rest.  Here the same block list is walked, but every block launches hand-written
-sm_100a kernels through the C ABI (include/fsdet.h) on NHWC fp32 buffers, and a
+sm_90a kernels through the C ABI (include/fsdet.h) on NHWC fp32 buffers, and a
 small tape replays the blocks in reverse for the backward pass.
 
 Memory comes from torch's caching allocator (`torch.empty`): torch is used for
@@ -17,21 +17,21 @@ from ._lib import call, ptr
 
 import os
 
-# tensor-core (tcgen05) convolution path for layers with Cin % 64 == 0; FSDET_TC=0 selects the exact-fp32 SIMT kernels
+# tensor-core (wgmma) convolution path for layers with Cin % 64 == 0; FSDET_TC=0 selects the exact-fp32 SIMT kernels
 USE_TC = os.environ.get('FSDET_TC', '1') != '0'
-# 'first' = the recomputing first-block kernels (csrc/conv_first_tc.cuh): correct but, as measured on a B200, slower than the
-# store-z path they were meant to replace (instruction-bound epilogues, DESIGN.md section 3) - opt-in only
+# 'first' = the recomputing first-block kernels (csrc/conv_first_tc.cuh): correct but slower than the store-z path they were
+# meant to replace (instruction-bound epilogues, DESIGN.md section 3) - opt-in only
 TC_PARTS = set(os.environ.get('FSDET_TC_PARTS', 'fwd,dgrad,wgrad,head').split(','))  # debugging: which GEMMs may use it
 
 
 def _parse_terms(spec):
     """'fwd=3,dgrad=3,wgrad=0,head=3' -> dict.  Operand-term mode of each GEMM class (include/fsdet.h,
     fsdet_conv_tc_fwd `mode` bits 0-1): 3 = hi*hi + lo*hi + hi*lo (fp32 grade), 1 / 2 = one operand exact and the
-    other rounded to fp16, 0 = fp16 x fp16.  The defaults are the measured per-class decision (DESIGN.md section 3,
-    profiles/precision_budget_r02.*): the forward chain amplifies per-layer rounding ~1000x through 23 train-mode BN
-    layers (2-term forward: 9e-3 at the head output) and the input-gradient chain accumulates it towards the first
-    layers (2-term: 1.4e-3), so both keep the fp32-grade 3-term scheme; the weight gradient feeds SGD only, does not
-    compound, and its plain fp16 x fp16 form stays within 2.3e-4 ... 5.7e-4 of the fp32-grade value on every tensor."""
+    other rounded to fp16, 0 = fp16 x fp16.  The defaults are the per-class decision of the precision budget (DESIGN.md
+    section 3, tools/precision_budget.py): the forward chain amplifies per-layer rounding through 23 train-mode BN layers
+    (2-term forward: ~1e-2 at the head output) and the input-gradient chain accumulates it towards the first layers, so
+    both keep the fp32-grade 3-term scheme; the weight gradient feeds SGD only, does not compound, and its plain
+    fp16 x fp16 form stays within a few 1e-4 of the fp32-grade value on every tensor."""
     d = {'fwd': 3, 'dgrad': 3, 'wgrad': 0, 'head': 3}
     for item in filter(None, (spec or '').split(',')):
         k, v = item.split('=')
@@ -42,7 +42,7 @@ def _parse_terms(spec):
 
 
 TC_TERMS = _parse_terms(os.environ.get('FSDET_TC_TERMS'))
-# persistent tile loop (one CTA per SM, double-buffered TMEM accumulators) for the short-K layers
+# persistent tile loop (one CTA per SM walks the tiles) for the short-K layers
 TC_PERSIST = os.environ.get('FSDET_TC_PERSIST', '0') == '1'
 
 
@@ -658,7 +658,7 @@ class NetRunner(object):
             assert cout_p == s.cout, 'BatchNorm conv with Cout % 4 != 0 is unsupported'
             z = Act.new(B, H, W, s.cout, dev)
             use_batch_stats = training or not bn.track_running_stats
-            rows_cap = max(_lib.lib.fsdet_conv_stat_rows(npix), _lib.lib.fsdet_colstats_rows(npix), (npix + 127) // 128 + 1, 3 * 148)
+            rows_cap = max(_lib.lib.fsdet_conv_stat_rows(npix), _lib.lib.fsdet_colstats_rows(npix), (npix + 127) // 128 + 1, 3 * _lib.lib.fsdet_num_sms())
             stat = _empty(rows_cap + _lib.lib.fsdet_bn_stat_scratch_rows(), 4 * s.cout, device=dev) if use_batch_stats else None
             wp = getattr(self, '_wp', {}).get(id(wuse))
             rows = self._conv('fwd', x, wuse, None, z, stat, cin_p, s.cout, s.k, 0, st, wplanes=wp['fwd'] if wp else None)

@@ -2,8 +2,8 @@
 
 The reference's `Darknet(darknet_file, learnet_file)` accepts either a path to a
 Darknet `.cfg` file or an already parsed list of block dicts
-(darknet_meta.py:87-90).  `/root/reference/cfg/*.cfg` does not travel to the GPU
-box, so the benchmark and the tests build the same architectures from the
+(darknet_meta.py:87-90).  The reference's `cfg/*.cfg` files are not part of this
+repository, so the benchmark and the tests build the same architectures from the
 compact specs below (architecture facts taken from cfg/darknet_dynamic.cfg,
 cfg/reweighting_net.cfg and cfg/tiny-yolo-voc.cfg) in the exact dict format
 `cfg.parse_cfg` produces (all values are strings, `type=` keys renamed

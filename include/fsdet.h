@@ -1,5 +1,5 @@
 /*
- * libfsdet.so — C ABI of the B200-native few-shot-detection training hot path.
+ * libfsdet.so — C ABI of the H100-native few-shot-detection training hot path.
  *
  * Drop-in boundary.  The reference (bingykang/Fewshot_Detection) reaches its
  * device code through torch-0.3.1 library calls made from
@@ -28,7 +28,7 @@
  * exactly as darknet_meta.Darknet.forward / RegionLossV2.forward exchange them.
  *
  * Each entry point cites the reference code it replaces (paths relative to
- * /root/reference).
+ * the reference repository).
  */
 #ifndef FSDET_H_
 #define FSDET_H_
@@ -44,8 +44,10 @@ extern "C" {
 int fsdet_version(void);
 /* thread-local description of the last non-zero return value */
 const char* fsdet_last_error(void);
-/* compute capability the kernels were compiled for (100 = sm_100a) */
+/* compute capability the kernels were compiled for (90 = sm_90a) */
 int fsdet_compiled_arch(void);
+/* streaming multiprocessors the launch plans assume (persistent grids, split-K rounds): 132 = H100 SXM */
+int fsdet_num_sms(void);
 
 /* ---- layout conversion at the reference-facing boundary ---------------- */
 /* [B,C0,H,W] (+ optional second tensor [B,C1,H,W], the support branch's
@@ -88,7 +90,7 @@ int fsdet_conv_first_wgrad(const float* in0, int C0, const float* in1, int C1, c
                            float* workspace, size_t workspace_floats, int B, int H, int W, int Cout, void* stream);
 size_t fsdet_conv_first_wgrad_workspace_floats(int B, int H, int W, int Cout);
 /* The same first block (conv 3x3 from <= 4 NCHW input channels into Cout <= 32 + train-mode BatchNorm + LeakyReLU +
- * MaxPool 2/2) WITHOUT storing its pre-BN output: every pass recomputes it from the input images with a tcgen05 GEMM
+ * MaxPool 2/2) WITHOUT storing its pre-BN output: every pass recomputes it from the input images with a wgmma GEMM
  * per 128-pixel tile (csrc/conv_first_tc.cuh).  Needs H % 8 == 0, W % 16 == 0 (fsdet_conv_first_tc_supported).
  * amax_x: device scalar >= max |input| (fsdet_amax over the input tensors).  w_pad4 as above.
  *   _stats      -> BatchNorm partial rows float [fsdet_conv_first_tc_rows(B,H,W)][4*Cout] for fsdet_bn_finalize
@@ -119,7 +121,7 @@ int fsdet_weight_flip_transpose(const float* w, float* wt, int Cout, int kk, int
 /* copy [rows][cin] -> [rows][cout] channel-padded / -cropped (zero fill) */
 int fsdet_pad_channels(const float* in, int cin, float* out, int cout, size_t rows, void* stream);
 
-/* ---- tensor-core convolution (tcgen05 + TMA im2col), csrc/conv_tc.cu ---- */
+/* ---- tensor-core convolution (wgmma + TMA im2col), csrc/conv_tc.cu ---- */
 /* Same contraction as fsdet_conv_fwd for layers with Cin % 32 == 0, Cout % 4 == 0
  * (fsdet_conv_tc_supported); `cpitch` >= Cin is the channel pitch of the planes
  * (activation rows and the weights' [tap][channel] axis), so 32-channel tensors
@@ -133,7 +135,7 @@ int fsdet_pad_channels(const float* in, int cin, float* out, int cout, size_t ro
  *     3 = fp32-grade (reproduces the fp32 reference incl. its max-pool arg-max
  *     decisions), 0 = plain fp16 x fp16 -> fp32.  Planes that are not used may be
  *     NULL.  Bit 4 (16): persistent tile loop for short-K layers (one CTA per
- *     SM, double-buffered TMEM accumulators).  Bit 5 (32): thread-block clusters
+ *     SM, the producer runs ahead across tiles).  Bit 5 (32): thread-block clusters
  *     of two CTAs that share the weight tile through TMA multicast (ignored in
  *     persistent mode and for single-tile problems).  Bit 6 (64): never take the
  *     halo-tile kernel.  By default (bits 4-6 clear, mode 3) the 3x3 layers with
@@ -144,8 +146,8 @@ int fsdet_pad_channels(const float* in, int cin, float* out, int cout, size_t ro
  *     Bit 7 (128): issue x_hi*w_hi and x_hi*w_lo as two MMAs.  By default the
  *     mode-3 kernels with one hi accumulator issue them as ONE MMA of width
  *     2*BN (the lo weight plane follows the hi plane in shared memory, the lo
- *     accumulator follows the hi accumulator in TMEM): same products, two
- *     tcgen05.mma per K step instead of three.
+ *     accumulator follows the hi accumulator in registers): same products, two
+ *     wgmma per K step instead of three.
  * x_hi/x_lo dense NHWC [B*H*W][cpitch] fp16, w_hi/w_lo [Cout][k*k*cpitch] fp16,
  * amax_x / amax_w: device floats holding the tensors' absolute maxima (NULL =
  * planes are unscaled).  Output fp32 z[p][n] (+ previous z when accumulate

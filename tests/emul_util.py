@@ -18,7 +18,8 @@ def build_emul(name, kernel_src, opt='-O2'):
     ksrc = os.path.join(ROOT, 'fewshot_detection_b200', 'csrc', kernel_src)
     lib = os.path.join(ROOT, 'build', 'lib%s_emul.so' % name)
     os.makedirs(os.path.dirname(lib), exist_ok=True)
-    if not os.path.exists(lib) or os.path.getmtime(lib) < max(os.path.getmtime(p) for p in (src, HDR, ksrc)):
+    deps = [src, HDR, ksrc] + [os.path.join(os.path.dirname(HDR), f) for f in os.listdir(os.path.dirname(HDR))]
+    if not os.path.exists(lib) or os.path.getmtime(lib) < max(os.path.getmtime(p) for p in deps):
         cmd = ['g++', opt, '-std=c++17', '-ffp-contract=off', '-fPIC', '-shared', '-pthread', '-w',
                '-DFSDET_HOST_EMULATION', '-I' + inc, '-include', HDR, '-x', 'c++', src, '-o', lib]
         r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)

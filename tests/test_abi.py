@@ -62,13 +62,14 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, name), name
     lib.fsdet_version.restype = ctypes.c_int
     assert lib.fsdet_version() >= 100
-    assert lib.fsdet_compiled_arch() == 100
+    assert lib.fsdet_compiled_arch() == 90
+    assert lib.fsdet_num_sms() == 132
 
 
-def test_library_is_sm100a_native():
+def test_library_is_sm90a_native():
     _build_if_needed()
     out = subprocess.run(['cuobjdump', '-lelf', LIB], capture_output=True, text=True).stdout
-    assert 'sm_100a' in out, out
+    assert 'sm_90a' in out, out
 
 
 def test_product_package_never_imports_the_oracle():
@@ -89,7 +90,7 @@ def test_product_package_never_imports_the_oracle():
 def test_tile_plans_of_the_benchmarked_layers():
     """Host-side planning of the tensor-core kernels at configs[1] (64 query + 20 support images, 416x416) - pure C
     functions of the library, no GPU: which layers the halo-tile kernel takes, how many BatchNorm partial rows the
-    kernels emit, and that the weight gradient's split-K fills whole rounds of the 148 SMs."""
+    kernels emit, and that the weight gradient's split-K fills whole rounds of the 132 SMs."""
     _build_if_needed()
     from fewshot_detection_b200 import _lib
     L = _lib.lib
@@ -104,17 +105,17 @@ def test_tile_plans_of_the_benchmarked_layers():
         assert L.fsdet_conv_tc_uses_halo(B, H, H, Cin, Cout, 3, 3) == want, (B, H, Cin, Cout)
         assert L.fsdet_conv_tc_uses_halo(B, H, H, Cin, Cout, 3, 3 | 64) == 0          # mode bit 6: never
         rows = L.fsdet_conv_tc_stat_rows(B, H, H, Cin, Cout, 3, 3)
-        assert rows == (148 if want else -(-B * H * H // 128)), (B, H, Cin, Cout, rows)
+        assert rows == (132 if want else -(-B * H * H // 128)), (B, H, Cin, Cout, rows)
     assert L.fsdet_conv_tc_uses_halo(64, 208, 208, 32, 64, 1, 3) == 0                 # 1x1
     assert L.fsdet_conv_tc_uses_halo(64, 208, 208, 32, 64, 3, 0) == 0                 # only the 3-term mode
-    # weight gradient (fp16 x fp16 mode, 256-wide tiles): CTAs = tiles * splits never spill a few CTAs into an extra round
+    # weight gradient (fp16 x fp16 mode, 128-wide tiles): CTAs = tiles * splits never spill a few CTAs into an extra round
     for B, H, Cin, Cout in [(64, 208, 64, 64), (64, 104, 64, 128), (64, 52, 128, 256), (64, 26, 256, 512), (64, 13, 512, 1024),
                             (64, 13, 1024, 1024), (64, 13, 1280, 1024), (20, 208, 64, 64), (20, 13, 512, 1024)]:
-        taps = 1 if Cin >= 256 else (2 if Cin >= 128 else 4)
-        cib = 256 // taps
+        taps = 1 if Cin >= 128 else 2
+        cib = 128 // taps
         tiles = -(-Cin // cib) * -(-9 // taps) * -(-Cout // 128)
         ws = L.fsdet_conv_tc_wgrad_workspace_floats(B, H, H, Cin, Cout, 3, 0)
         splits = max(1, ws // (Cout * 9 * Cin))
         ctas = tiles * splits
-        rounds = -(-ctas // 148)
-        assert ctas > 0.8 * rounds * 148 or splits == 1, (B, H, Cin, Cout, tiles, splits, ctas)
+        rounds = -(-ctas // 132)
+        assert ctas > 0.8 * rounds * 132 or splits == 1, (B, H, Cin, Cout, tiles, splits, ctas)

@@ -1,6 +1,6 @@
 """The recomputing first-layer kernels (csrc/conv_first_tc.cuh: conv 3x3 + BatchNorm + LeakyReLU + max-pool in four
 passes that never store the pre-BN tensor) on the CPU: the kernel source compiled against functional models of its
-PTX wrappers (tools/host_emul/conv_first_tc_emul.cpp; the tcgen05.mma model reads the 128-byte-swizzled operand tiles the
+PTX wrappers (tools/host_emul/conv_first_tc_emul.cpp; the wgmma model reads the 128-byte-swizzled operand tiles the
 kernel itself writes, K-major for the forward GEMM and MN-major for the weight-gradient GEMM) against numpy."""
 import ctypes
 

@@ -1,4 +1,4 @@
-"""Control flow of the halo-tile tcgen05 convolution (csrc/conv_halo_kernels.cuh) on the CPU: the kernel source compiled
+"""Control flow of the halo-tile wgmma convolution (csrc/conv_halo_kernels.cuh) on the CPU: the kernel source compiled
 against functional models of its PTX wrappers (tools/host_emul/conv_halo_emul.cpp) must reproduce the 3x3 convolution of
 the operand planes - persistent grids smaller than / equal to the tile count, resident and streamed weight operands
 (both producer warps), one to four 32-channel chunks, tiles that overhang the image (clipped stores, masked statistics),
@@ -64,7 +64,7 @@ def test_halo_kernel_control_flow(emul, B, H, W, Cin, cpitch, Cout, ctas, acc, s
 
 
 def test_slow_epilogue(emul):
-    """The MMA issuer runs ahead of a slow epilogue: it must wait for the accumulator set to be handed back."""
+    """The producers run ahead of slow MMA warpgroups: they must wait for every MMA warp to release a stage."""
     emul.emul_set_ld_delay_us(20000)
     try:
         test_halo_kernel_control_flow(emul, *CASES[3])

@@ -1,11 +1,11 @@
-"""Control flow of the tcgen05 convolution kernel (csrc/conv_tc_kernels.cuh) on the CPU: the kernel source is compiled
+"""Control flow of the wgmma convolution kernel (csrc/conv_tc_kernels.cuh) on the CPU: the kernel source is compiled
 against functional models of its PTX wrappers (tools/host_emul/conv_tc_emul.cpp: mbarrier phases and transaction counts,
-im2col / tiled TMA loads, tcgen05.mma into a TMEM array, commit, tcgen05.ld, swizzled TMA store, named barriers) and
+im2col / tiled TMA loads into swizzled shared memory, wgmma with the device descriptor encoding, named barriers) and
 must reproduce the convolution - for one-tile-per-CTA grids and for persistent grids smaller than, equal to and larger
 than the tile count, for every operand-term mode (which planes are loaded and multiplied), with and without the fused
 BatchNorm statistics.  A wrong barrier phase deadlocks (reported as -100 after a timeout) or corrupts the result.
-Descriptors, swizzle modes and the instruction descriptor are NOT what is tested here - those are exercised by the
-GPU tests (tests/test_gpu_tc.py)."""
+The shared-memory descriptors and swizzle modes are checked too: the modelled TMA stores its boxes swizzled and the wgmma
+model reads them back through the device descriptor encoding (tools/host_emul/wgmma_emul.h)."""
 import ctypes
 
 import numpy as np
@@ -76,10 +76,10 @@ CASES = [
     (2, 12, 12, 64, 200, 1, 128, 32, 3, 1, 2, 0, 1),    # 1x1, BN = 128, two N tiles (the second one partial), 2 k-blocks per tile
     (1, 20, 20, 32, 64, 3, 64, 32, 3, 1, 2, 1, 0),      # accumulate into z (TMA reduce-add)
     (3, 8, 8, 96, 64, 3, 64, 32, 3, 1, 2, 0, 1),        # 27 k-blocks per tile, 3 channel chunks per tap
-    (2, 16, 16, 32, 64, 3, 64, 32, 3, 0, 0, 0, 1),      # one tile per CTA (2 CTAs / SM flavour): staging aliases the stages
+    (2, 16, 16, 32, 64, 3, 64, 32, 3, 0, 0, 0, 1),      # one tile per CTA
     (1, 13, 13, 64, 136, 3, 128, 32, 3, 0, 0, 0, 1),    # two N tiles, partial second one, clipped rows, statistics per M tile
     (1, 20, 20, 32, 64, 3, 64, 32, 3, 0, 0, 1, 0),      # accumulate, one tile per CTA
-    (2, 10, 10, 128, 128, 3, 128, 64, 3, 0, 0, 0, 1),   # long-K flavour: 3 rotating hi accumulators + lo accumulator
+    (2, 10, 10, 128, 128, 3, 128, 64, 3, 0, 0, 0, 1),   # long-K flavour: hi*hi k-blocks folded into a register total + lo accumulator
     (2, 10, 10, 128, 64, 3, 64, 64, 3, 0, 0, 0, 1),     # long-K, BN = 64
     (2, 16, 16, 32, 64, 3, 64, 32, 0, 1, 2, 0, 1),      # terms = 0: only the hi planes exist (lo maps are poisoned)
     (2, 16, 16, 32, 64, 3, 64, 32, 1, 1, 2, 0, 1),      # terms = 1: x_lo * w_hi added
@@ -124,8 +124,8 @@ def test_kernel_control_flow(emul, B, H, W, Cin, Cout, k, bn, bk, terms, persist
 
 
 def test_slow_epilogue_does_not_lose_accumulators(emul):
-    """With a slow epilogue the MMA issuer runs ahead: it must wait until the epilogue has handed an accumulator set
-    back (acc_empty) before overwriting it - one CTA, four tiles, two sets."""
+    """With slow MMA warpgroups the producer runs ahead across tile boundaries: it must wait until every MMA warp has
+    released a stage before refilling it - one CTA, four tiles."""
     emul.emul_set_ld_delay_us(30000)
     try:
         test_kernel_control_flow(emul, *CASES[1])

@@ -1,5 +1,5 @@
 """Per-kernel parity of the C-ABI entry points against torch fp32 / the oracle.
-All tests need a B200 (`-m gpu`)."""
+All tests need an H100 (`-m gpu`)."""
 import os
 
 import numpy as np

@@ -10,10 +10,10 @@ pytestmark = pytest.mark.gpu
 
 # Two arithmetic paths are tested (engine.USE_TC):
 #   'fp32' : exact-fp32 SIMT kernels (per-op rounding ~1e-7)  -> the strict bars below
-#   'tc'   : tcgen05 tensor-core kernels, the shipped precision policy (engine.TC_TERMS): forward and input-gradient
+#   'tc'   : wgmma tensor-core kernels, the shipped precision policy (engine.TC_TERMS): forward and input-gradient
 #            GEMMs with scaled fp16 hi/lo operand splitting (per-op rounding 1e-7..4e-6, like fp32 FMA kernels),
-#            weight-gradient GEMMs in plain fp16 x fp16 (measured 2e-4..6e-4 per tensor against the 3-term value at
-#            the real layer shapes, profiles/precision_budget_r02.log; it feeds SGD only and does not compound).
+#            weight-gradient GEMMs in plain fp16 x fp16 (a few 1e-4 per tensor against the 3-term value at the real
+#            layer shapes, tools/precision_budget.py; it feeds SGD only and does not compound).
 #            Every mini-model tensor - output, loss, all 60 parameter gradients - meets the north star's 1e-3 on
 #            both paths.  Gradients of the FULL architecture on tiny batches are ill-conditioned in float32
 #            (DESIGN.md "Parity": torch's own cuDNN fp32 sits 1e-2 from float64), so there both paths are held to

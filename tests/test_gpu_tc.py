@@ -1,11 +1,11 @@
-"""tcgen05 / TMA-im2col convolution path (csrc/conv_tc.cu) against torch fp32."""
+"""wgmma / TMA-im2col convolution path (csrc/conv_tc.cu) against torch fp32."""
 import pytest
 import torch
 import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
-TOL_TC = 1e-5  # vs float64: scaled fp16 hi/lo split (22 bits), hi*hi products spread over 3 fp32 TMEM accumulators
+TOL_TC = 1e-5  # vs float64: scaled fp16 hi/lo split (22 bits), hi*hi k-blocks added to an fp32 register total
 
 
 def rel(a, b):

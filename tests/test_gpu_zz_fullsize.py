@@ -1,7 +1,7 @@
 """Size-independent properties of the conv stack at the BASELINE configs[1] size (64 query images, 20 classes,
 416x416), where the CPU oracle would take minutes: permuting the query images permutes the (image, class) row blocks
 of the head output and nothing else (training-mode BatchNorm statistics, the tensor-wide operand scales of the
-tcgen05 path and the class reweighting are all permutation invariant up to summation order).
+tensor-core path and the class reweighting are all permutation invariant up to summation order).
 (File name sorts last on purpose: newest GPU tests run last.)"""
 import pytest
 import torch

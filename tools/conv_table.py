@@ -31,7 +31,7 @@ def main():
     lines = [l for l in open(sys.argv[1]) if not l.startswith('==')]
     rows = [r for r in csv.DictReader(lines) if r['Metric Name'] == 'gpu__time_duration.sum']
     pk = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json'))) if os.path.exists(os.path.join(ROOT, 'MEASURED_PEAKS.json')) else {}
-    peak_tf, peak_gb = pk.get('bf16_tflops_sustained', 1441.5), pk.get('hbm_gbs', 6577.7)
+    peak_tf, peak_gb = pk.get('bf16_tflops_sustained', 989.4), pk.get('hbm_gbs', 3350.0)   # H100 SXM data sheet
     seq = [(short(r['Kernel Name']), float(r['Metric Value']) / 1e3) for r in rows]
     # the halo-tile flavour (conv_halo_kernel) is a conv_tc dispatch: same role in the sequence
     seq = [('conv_tc_kernel' if n == 'conv_halo_kernel' else n, t) for n, t in seq]

@@ -32,7 +32,7 @@ def main():
     path = sys.argv[1]
     lines = [l for l in open(path) if not l.startswith('==')]
     rows = [r for r in csv.DictReader(lines) if r['Metric Name'] == 'gpu__time_duration.sum']
-    peak = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['hbm_gbs'] if os.path.exists(os.path.join(ROOT, 'MEASURED_PEAKS.json')) else 6577.7
+    peak = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['hbm_gbs'] if os.path.exists(os.path.join(ROOT, 'MEASURED_PEAKS.json')) else 3350.0   # H100 SXM HBM3 data sheet
     # one full step: from the first colstats of the support branch of the second step to the end, plus the tail of the first
     names = [short(r['Kernel Name']) for r in rows]
     us = [float(r['Metric Value']) / 1e3 for r in rows]

@@ -1,12 +1,10 @@
 // Host build of csrc/conv_first_tc.cuh (the recomputing first-layer kernels) against FUNCTIONAL MODELS of its PTX
-// wrappers (see cuda_host_emul.h for the thread model).  Unlike conv_tc_emul.cpp - whose operand tiles are written by
-// (modelled) TMA loads - this kernel writes its operand tiles ITSELF, byte by byte, in the 128-byte-swizzled layout, so
-// the tcgen05.mma model here reads shared memory the way the hardware does: logical address of element (row, k) from
-// the descriptor (K-major: start + row*128 + k*2; MN-major: start + block*LBO + k*128 + m*2), then the swizzle
-// XOR of address bits [4,7) with bits [7,10).  What this validates: the im2col row construction and its chunk
-// placement, operand-term bookkeeping, the lane <-> pixel map and the shuffle-based pooling / arg-max routing, the
-// transposition reductions, the persistent dW accumulator and its read-out, barrier phases (deadlock = -100).
-// The descriptor bit layouts themselves are shared, unchanged, with the GPU-verified kernels of conv_tc.cu.
+// wrappers (see cuda_host_emul.h for the thread model).  This kernel writes its operand tiles ITSELF, byte by byte, in
+// the 128-byte-swizzled layout; the wgmma model (wgmma_emul.h) reads shared memory the way the hardware does, through
+// the device descriptor encoding and the swizzle.  What this validates: the im2col row construction and its chunk
+// placement, operand-term bookkeeping, the descriptors (K-major forward, MN-major weight gradient), the fragment ->
+// pixel transposition, the shuffle-based pooling / arg-max routing, the transposition reductions, the persistent dW
+// accumulators and their read-out, barrier phases (deadlock = -100).
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -44,7 +42,6 @@ static std::atomic<bool> g_deadlock{false};
 static std::mutex g_mu;
 struct Bar { int count, pending; int phase; };
 static std::map<const void*, Bar> g_bars;
-static float g_tmem[128][512];
 
 static inline uint32_t smem_u32(const void* p) { return (uint32_t)((const unsigned char*)p - emul::g_dyn_smem); }
 static inline void mbar_init(uint64_t* bar, uint32_t count) {
@@ -70,51 +67,13 @@ static inline void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 static inline void fence_barrier_init() {}
 static inline void fence_proxy_async() {}
-static inline void tc_fence_before() {}
-static inline void tc_fence_after() {}
-static inline void tmem_alloc(uint32_t* slot, uint32_t) { *slot = 0; }
-static inline void tmem_dealloc(uint32_t, uint32_t) {}
 static inline void cp_async4_zfill(void* dst, const float* src, bool valid) {
     const float v = valid ? *src : 0.f;
     memcpy(dst, &v, 4);
 }
 static inline void cp_async_wait_all() {}
 
-// descriptors of the model: bits [0,32) start offset >> 4, [32,56) LBO bytes, bit 62 = MN-major
-static inline uint64_t umma_desc_k_sw128(uint32_t saddr) { return (uint64_t)(saddr >> 4); }
-static inline uint64_t umma_desc_mn_sw128(uint32_t saddr, uint32_t lbo) { return (uint64_t)(saddr >> 4) | ((uint64_t)lbo << 32) | (1ull << 62); }
-static inline float h2f(uint16_t b) { __half_raw r; r.x = b; return __half2float(__half(r)); }
-static inline float smem_half_swz(uint32_t addr) {
-    const uint32_t a = addr ^ (((addr >> 7) & 7u) << 4);      // 128-byte swizzle: address bits [4,7) ^= bits [7,10)
-    uint16_t v;
-    memcpy(&v, emul::g_dyn_smem + a, 2);
-    return h2f(v);
-}
-static inline float operand(uint64_t desc, int idx, int k) {   // idx = M or N index, k = 0..15
-    const uint32_t start = (uint32_t)(desc & 0xffffffffu) << 4;
-    if (desc >> 62 & 1) {
-        const uint32_t lbo = (uint32_t)((desc >> 32) & 0xffffff);
-        return smem_half_swz(start + (uint32_t)(idx / 64) * lbo + (uint32_t)k * 128 + (uint32_t)(idx % 64) * 2);
-    }
-    return smem_half_swz(start + (uint32_t)idx * 128 + (uint32_t)k * 2);
-}
-static inline void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    const int N = (int)((idesc >> 17) & 0x3f) << 3, M = (int)((idesc >> 24) & 0x1f) << 4;
-    const bool a_mn = (idesc >> 15) & 1, b_mn = (idesc >> 16) & 1;
-    if (a_mn != (bool)(adesc >> 62 & 1) || b_mn != (bool)(bdesc >> 62 & 1)) { g_deadlock.store(true); return; }   // descriptor / instruction mismatch
-    const int col0 = (int)(tmem_d & 0xffff);
-    for (int m = 0; m < M; ++m)
-        for (int n = 0; n < N; ++n) {
-            float acc = accumulate ? g_tmem[m][col0 + n] : 0.f;
-            for (int k = 0; k < 16; ++k) acc += operand(adesc, m, k) * operand(bdesc, n, k);
-            g_tmem[m][col0 + n] = acc;
-        }
-}
-static inline void umma_commit(uint64_t* bar) { mbar_arrive(bar); }
-static inline void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    const int row = (int)(taddr >> 16) + (int)(threadIdx.x & 31), col = (int)(taddr & 0xffff);
-    for (int j = 0; j < 32; ++j) memcpy(&r[j], &g_tmem[row][col + j], 4);
-}
+#include "wgmma_emul.h"
 
 #define FSDET_TC_DYN_SMEM(name) uint8_t* name = emul::g_dyn_smem
 #include "../../fewshot_detection_b200/csrc/conv_first_tc.cuh"
@@ -128,9 +87,9 @@ static int run(FtArgs a, int ctas) {
     g_deadlock.store(false);
     emul::launch(dim3(ctas), dim3(FT_THREADS), FtCfg<MODE>::SMEM_BYTES + 1024, [&]() {
         if (threadIdx.x == 0) {
-            memset(g_tmem, 0, sizeof(g_tmem));
             std::lock_guard<std::mutex> l(g_mu);
             g_bars.clear();
+            for (auto& nb : g_named) nb = NamedBar{};
         }
         // the kernel aligns its dynamic shared memory to 1 KB: make offset 0 of the model 1 KB aligned too
         pthread_barrier_wait(&emul::g_block.bar);

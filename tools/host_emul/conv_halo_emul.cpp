@@ -1,10 +1,10 @@
 // Host build of csrc/conv_halo_kernels.cuh (the halo-tile convolution) against the functional models of
-// conv_tc_emul.cpp plus models of the tiled 4-D TMA boxes it adds.  As there, tiles land UNSWIZZLED and the UMMA
-// model reads rows at the descriptor's row pitch from the descriptor's start address - which is exactly what the
+// conv_tc_emul.cpp plus a model of the tiled 4-D TMA box it adds.  As there, boxes land 64-byte swizzled and the wgmma
+// model reads shared memory through the device descriptor encoding and the same swizzle - which is exactly what the
 // halo scheme relies on: filter tap (dy, dx) = the K-major tile starting dy * 8 rows into x-shifted copy dx.  What is
 // validated: tile walk of the persistent grid, the two producer warps (activation stages / weight ring or resident
-// weights), stage and accumulator-set phases, tap addressing inside the halo copies, zero fill at the image border,
-// clipped stores and statistics for tiles that overhang the image.  Test tooling only.
+// weights), stage phases, tap addressing inside the halo copies, zero fill at the image border, clipped stores and
+// statistics for tiles that overhang the image.  Test tooling only.
 #include "conv_tc_emul.cpp"
 
 namespace fsdet {
@@ -12,33 +12,15 @@ namespace fsdet {
 // box (32 channels, 8 x, 18 y) of an NHWC fp16 plane at signed coordinates; zero outside the tensor
 static inline void tma_load_tiled_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c, int w, int h, int n) {
     const MapModel* m = model(map);
-    uint16_t* d = reinterpret_cast<uint16_t*>(dst);
     for (int yy = 0; yy < 18; ++yy)
         for (int xx = 0; xx < 8; ++xx)
             for (int k = 0; k < 32; ++k) {
                 const int y = h + yy, x = w + xx, ch = c + k;
                 const bool ok = n >= 0 && n < m->B && y >= 0 && y < m->H && x >= 0 && x < m->W && ch < m->C;
-                d[((size_t)yy * 8 + xx) * 32 + k] = ok ? m->base[(((size_t)n * m->H + y) * m->W + x) * m->cpitch + ch] : (uint16_t)0;
+                box_store(dst, yy * 8 + xx, k, 64, ok ? m->base[(((size_t)n * m->H + y) * m->W + x) * m->cpitch + ch] : (uint16_t)0);
             }
     bar_complete_tx(bar, 18 * 8 * 32 * 2);
 }
-// box (32 channels, 8 x, 4 y) of the fp32 NHWC output, 128-byte swizzled in shared memory, clipped by the tensor
-static inline void store_box_4d(const CUtensorMap* map, const void* src, int c, int w, int h, int n, bool add) {
-    const MapModel* m = model(map);
-    const unsigned char* s = reinterpret_cast<const unsigned char*>(src);
-    for (int r = 0; r < 32; ++r)
-        for (int j = 0; j < 32; ++j) {
-            const int y = h + (r >> 3), x = w + (r & 7);
-            if (y >= m->H || x >= m->W || c + j >= m->rows || n >= m->B) continue;
-            float v;
-            memcpy(&v, s + r * 128 + ((((j >> 2) ^ (r & 7))) << 4) + (j & 3) * 4, 4);
-            float* o = m->z + (((size_t)n * m->H + y) * m->W + x) * m->ldz + c + j;
-            *o = add ? *o + v : v;
-        }
-}
-static inline void tma_store_4d(const CUtensorMap* map, const void* src, int c, int w, int h, int n) { store_box_4d(map, src, c, w, h, n, false); }
-static inline void tma_reduce_add_4d(const CUtensorMap* map, const void* src, int c, int w, int h, int n) { store_box_4d(map, src, c, w, h, n, true); }
-
 #include "../../fewshot_detection_b200/csrc/conv_halo_kernels.cuh"
 
 }  // namespace fsdet
@@ -48,7 +30,7 @@ static int run_halo(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* 
                     int ldz, int B, int Cin, int ctas) {
     constexpr bool BRES = NCH * BN <= 64;
     using Cfg = HaloCfg<BN, NCH, BRES>;
-    CUtensorMap mAh, mAl, mBh, mBl, mZ;
+    CUtensorMap mAh, mAl, mBh, mBl;
     auto act = [&](CUtensorMap* m, const uint16_t* base) {
         MapModel mm{}; mm.kind = 3; mm.base = base; mm.B = B; mm.H = a.H; mm.W = a.W; mm.C = Cin; mm.cpitch = a.cpitch;
         memset(m, 0, sizeof(*m)); memcpy(m, &mm, sizeof(mm));
@@ -58,17 +40,16 @@ static int run_halo(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* 
         memset(m, 0, sizeof(*m)); memcpy(m, &mm, sizeof(mm));
     };
     act(&mAh, x_hi); act(&mAl, x_lo); wgt(&mBh, w_hi); wgt(&mBl, w_lo);
-    { MapModel mm{}; mm.kind = 4; mm.z = z; mm.rows = a.Cout; mm.B = B; mm.H = a.H; mm.W = a.W; mm.ldz = ldz; memset(&mZ, 0, sizeof(mZ)); memcpy(&mZ, &mm, sizeof(mm)); }
+    a.z = z; a.ldz = ldz;
     g_deadlock.store(false);
-    emul::launch(dim3(ctas), dim3(352), Cfg::SMEM_BYTES, [&]() {
+    emul::launch(dim3(ctas), dim3(HALO_THREADS), Cfg::SMEM_BYTES, [&]() {
         if (threadIdx.x == 0) {
-            memset(g_tmem, 0, sizeof(g_tmem));
             std::lock_guard<std::mutex> l(g_mu);
             g_bars.clear();
             for (auto& nb : g_named) nb = NamedBar{};
         }
         pthread_barrier_wait(&emul::g_block.bar);
-        conv_halo_kernel<BN, NCH, BRES>(mAh, mAl, mBh, mBl, mZ, a);
+        conv_halo_kernel<BN, NCH, BRES>(mAh, mAl, mBh, mBl, a);
     });
     return g_deadlock.load() ? -100 : 0;
 }

@@ -1,11 +1,10 @@
 // Host build of csrc/conv_tc_kernels.cuh against FUNCTIONAL MODELS of the PTX wrappers it uses (see
 // cuda_host_emul.h for the thread model).  What is modelled: mbarriers (arrival counts, transaction bytes, phase
-// parity), the im2col / tiled TMA loads (tiles land unswizzled), tcgen05.mma (fp16 x fp16 -> fp32 into a TMEM array),
-// tcgen05.commit, tcgen05.ld, the swizzled 32x32 TMA store / reduce-add.  What this validates: the kernel's CONTROL
-// FLOW - stage and accumulator-set phases, tile sequencing over a persistent grid, accumulate flags of the three-MMA
-// hi/lo scheme, epilogue staging, edge clipping - i.e. everything that is new relative to the GPU-verified
-// conv_tc_kernel, whose descriptors / swizzle modes / instruction descriptor the persistent kernel reuses unchanged.
-// A wrong phase shows up as a deadlock (reported after a timeout) or as a wrong result.  Test tooling only.
+// parity), the im2col / tiled TMA loads (boxes land 64- / 128-byte swizzled, like the hardware's), wgmma with the device
+// descriptor encoding (wgmma_emul.h), named barriers.  What this validates: the kernel's CONTROL FLOW - stage phases,
+// tile sequencing over a persistent grid, accumulate flags of the three-MMA hi/lo scheme and of the k-block totals,
+// the epilogue's fragment -> row mapping, edge clipping, the fused statistics - and the shared-memory descriptors it
+// builds.  A wrong phase shows up as a deadlock (reported after a timeout) or as a wrong result.  Test tooling only.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -40,7 +39,6 @@ static std::atomic<bool> g_deadlock{false};
 static std::mutex g_mu;
 struct Bar { int count, pending; long long tx; int phase; };
 static std::map<const void*, Bar> g_bars;
-static float g_tmem[128][512];
 
 struct MapModel {   // lives in the first bytes of a CUtensorMap
     int kind;       // 0 = im2col activation plane, 1 = weight plane, 2 = fp32 output
@@ -98,25 +96,25 @@ static inline void mbar_wait_warp(uint64_t* bar, uint32_t parity) {
 }
 static inline void fence_barrier_init() {}
 static inline void fence_proxy_async() {}
-static inline void tc_fence_before() {}
-static inline void tc_fence_after() {}
 static inline void tma_prefetch_desc(const CUtensorMap*) {}
-static inline void tma_store_commit() {}
-template <int N> static inline void tma_store_wait_read() {}
-static inline void tmem_alloc(uint32_t* slot, uint32_t) { *slot = 0; }
-static inline void tmem_dealloc(uint32_t, uint32_t) {}
+
+#include "wgmma_emul.h"
+
+// element k of row r of a TMA box with rows of `row_bytes` bytes, through the shared-memory swizzle of the tensor map
+static inline void box_store(void* dst, int r, int k, int row_bytes, uint16_t v) {
+    const uint32_t a = swizzle_addr(smem_u32(dst) + (uint32_t)(r * row_bytes + k * 2), row_bytes == 128 ? GMMA_SW128 : GMMA_SW64);
+    memcpy(emul::g_dyn_smem + a, &v, 2);
+}
 
 // 128 consecutive output pixels starting at the pixel whose filter window has its corner at (w, h) of image n;
 // one filter tap (off_w, off_h), channels c .. c+bk-1; zero outside the image / beyond the last pixel
 static inline void tma_load_im2col_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c, int w, int h, int n,
                                       uint16_t off_w, uint16_t off_h) {
     const MapModel* m = model(map);
-    uint16_t* d = reinterpret_cast<uint16_t*>(dst);
     long long pix0 = ((long long)n * m->H + (h + m->pad)) * m->W + (w + m->pad);
     const long long total = (long long)m->B * m->H * m->W;
     for (int i = 0; i < EMUL_BM; ++i) {
         const long long pi = pix0 + i;
-        uint16_t* row = d + (size_t)i * m->bk;
         bool ok = pi < total;
         int img = 0, y = 0, x = 0;
         if (ok) {
@@ -128,105 +126,26 @@ static inline void tma_load_im2col_4d(void* dst, const CUtensorMap* map, uint64_
         }
         for (int k = 0; k < m->bk; ++k) {
             const int ch = c + k;
-            row[k] = (ok && ch < m->C) ? m->base[(((size_t)img * m->H + y) * m->W + x) * m->cpitch + ch] : (uint16_t)0;
+            box_store(dst, i, k, m->bk * 2, (ok && ch < m->C) ? m->base[(((size_t)img * m->H + y) * m->W + x) * m->cpitch + ch] : (uint16_t)0);
         }
     }
     bar_complete_tx(bar, (uint32_t)(EMUL_BM * m->bk * 2));
 }
 static inline void tma_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
     const MapModel* m = model(map);
-    uint16_t* d = reinterpret_cast<uint16_t*>(dst);
     for (int r = 0; r < m->box_rows; ++r)
         for (int k = 0; k < m->bk; ++k) {
             const long long row = c1 + r, col = c0 + k;
-            d[(size_t)r * m->bk + k] = (row < m->rows && col < m->K) ? m->base[(size_t)row * m->K + col] : (uint16_t)0;
+            box_store(dst, r, k, m->bk * 2, (row < m->rows && col < m->K) ? m->base[(size_t)row * m->K + col] : (uint16_t)0);
         }
     bar_complete_tx(bar, (uint32_t)(m->box_rows * m->bk * 2));
 }
-static inline void store_box(const CUtensorMap* map, const void* src, int c0, int c1, bool add) {
-    const MapModel* m = model(map);
-    const unsigned char* s = reinterpret_cast<const unsigned char*>(src);
-    for (int r = 0; r < 32; ++r)
-        for (int j = 0; j < 32; ++j) {
-            if (c1 + r >= m->M || c0 + j >= m->rows) continue;      // clipped by the tensor map
-            float v;
-            memcpy(&v, s + r * 128 + ((((j >> 2) ^ (r & 7))) << 4) + (j & 3) * 4, 4);   // 128-byte swizzle
-            float* o = m->z + (size_t)(c1 + r) * m->ldz + c0 + j;
-            *o = add ? *o + v : v;
-        }
-}
-static inline void tma_store_2d(const CUtensorMap* map, const void* src, int c0, int c1) { store_box(map, src, c0, c1, false); }
-static inline void tma_reduce_add_2d(const CUtensorMap* map, const void* src, int c0, int c1) { store_box(map, src, c0, c1, true); }
-
-// model descriptors: [0,32) = byte offset >> 4 (so that the kernel's `+ adv` in 16-byte units works), [32,48) = row bytes
-static inline uint64_t umma_desc_k_sw128(uint32_t saddr) { return (uint64_t)(saddr >> 4) | ((uint64_t)128 << 32); }
-static inline uint64_t umma_desc_k_sw64(uint32_t saddr) { return (uint64_t)(saddr >> 4) | ((uint64_t)64 << 32); }
-static inline float h2f(uint16_t b) { __half_raw r; r.x = b; return __half2float(__half(r)); }
-static inline void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    const int N = (int)((idesc >> 17) & 0x3f) << 3, M = (int)((idesc >> 24) & 0x1f) << 4;
-    const unsigned char* A = emul::g_dyn_smem + ((adesc & 0xffffffffu) << 4);
-    const unsigned char* Bm = emul::g_dyn_smem + ((bdesc & 0xffffffffu) << 4);
-    const int ra = (int)(adesc >> 32), rb = (int)(bdesc >> 32);
-    const int col0 = (int)(tmem_d & 0xffff);
-    for (int m = 0; m < M; ++m)
-        for (int n = 0; n < N; ++n) {
-            float acc = accumulate ? g_tmem[m][col0 + n] : 0.f;
-            for (int k = 0; k < 16; ++k) {
-                uint16_t a, b;
-                memcpy(&a, A + (size_t)m * ra + k * 2, 2);
-                memcpy(&b, Bm + (size_t)n * rb + k * 2, 2);
-                acc += h2f(a) * h2f(b);
-            }
-            g_tmem[m][col0 + n] = acc;
-        }
-}
-static inline void umma_commit(uint64_t* bar) { mbar_arrive(bar); }
-// (lo, hi) descriptor words: lo = byte offset >> 4, hi = one of the layout constants (only the row pitch matters to the model)
-static inline bool elect_one() { return (threadIdx.x & 31) == 0; }
-static inline uint32_t umma_desc_lo(uint32_t saddr) { return saddr >> 4; }
-constexpr uint32_t UMMA_DESC_HI_K_SW64 = 64, UMMA_DESC_HI_K_SW128 = 128;
-static inline void umma_f16_lohi(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t idesc, uint32_t accumulate) {
-    umma_f16(tmem_d, (uint64_t)a_lo | ((uint64_t)a_hi << 32), (uint64_t)b_lo | ((uint64_t)b_hi << 32), idesc, accumulate);
-}
-static std::atomic<int> g_ld_delay_us{0};   // slows the epilogue down so that a missing accumulator hand-back shows
-static inline void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    if (g_ld_delay_us.load() > 0) std::this_thread::sleep_for(std::chrono::microseconds(g_ld_delay_us.load()));
-    const int row = (int)(taddr >> 16) + (int)(threadIdx.x & 31), col = (int)(taddr & 0xffff);
-    for (int j = 0; j < 32; ++j) memcpy(&r[j], &g_tmem[row][col + j], 4);
-}
-
-static inline void tmem_ld32_nowait(uint32_t taddr, uint32_t (&r)[32]) { tmem_ld32(taddr, r); }
-static inline void tmem_ld_wait() {}
-static inline void tmem_ld_use(uint32_t (&)[32]) {}
-
-// barrier over a subset of the block's threads (bar.sync id, n): generation counter per id
-struct NamedBar { int waiting = 0; long long gen = 0; };
-static NamedBar g_named[16];
-static inline void named_bar_sync(int id, int nthreads) {
-    long long my;
-    {
-        std::lock_guard<std::mutex> l(g_mu);
-        NamedBar& b = g_named[id];
-        my = b.gen;
-        if (++b.waiting == nthreads) { b.waiting = 0; ++b.gen; return; }
-    }
-    const auto t0 = std::chrono::steady_clock::now();
-    for (;;) {
-        {
-            std::lock_guard<std::mutex> l(g_mu);
-            if (g_named[id].gen != my) return;
-        }
-        if (g_deadlock.load()) return;
-        if (std::chrono::steady_clock::now() - t0 > std::chrono::seconds(20)) { g_deadlock.store(true); return; }
-        std::this_thread::yield();
-    }
-}
-
 // thread-block clusters are not modelled (blocks run one after another): the cluster flavour is never instantiated here
 static inline uint32_t cluster_ctarank() { return 0; }
 static inline void cluster_sync_all() {}
 static inline void tma_load_2d_mc(void*, const CUtensorMap*, uint64_t*, int, int, uint16_t) { g_deadlock.store(true); }
-static inline void umma_commit_mc(uint64_t*, uint16_t) { g_deadlock.store(true); }
+static inline void mbar_arrive_cluster(uint64_t*, uint32_t) { g_deadlock.store(true); }
+static inline bool elect_one() { return (threadIdx.x & 31) == 0; }
 
 #include "../../fewshot_detection_b200/csrc/conv_tc_kernels.cuh"
 static_assert(EMUL_BM == TC_BM, "tile height of the models");
@@ -235,11 +154,11 @@ static_assert(EMUL_BM == TC_BM, "tile height of the models");
 
 using namespace fsdet;
 
-template <int BN, int BK, int NH, int TERMS, bool PERSIST, int MINB>
+template <int BN, int BK, int TERMS, bool PERSIST, bool FOLD>
 static int run(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* w_hi, const uint16_t* w_lo, TcArgs a, int B,
                int ctas) {
-    using Cfg = TcCfg<BN, BK, NH, TERMS, PERSIST, MINB>;
-    CUtensorMap mAh, mAl, mBh, mBl, mZ;
+    using Cfg = TcCfg<BN, BK, TERMS, PERSIST>;
+    CUtensorMap mAh, mAl, mBh, mBl;
     const long long K = (long long)a.ks * a.ks * a.cpitch;
     auto act = [&](CUtensorMap* m, const uint16_t* base) {
         MapModel mm{}; mm.kind = 0; mm.base = base; mm.B = B; mm.H = a.H; mm.W = a.W; mm.C = a.Cin; mm.cpitch = a.cpitch;
@@ -253,38 +172,36 @@ static int run(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* w_hi,
     static_assert(sizeof(MapModel) <= sizeof(CUtensorMap), "model must fit in the tensor map");
     // planes a term does not use must never be touched: their maps get a null base (a load would crash)
     act(&mAh, x_hi); act(&mAl, (TERMS & 1) ? x_lo : nullptr); wgt(&mBh, w_hi); wgt(&mBl, (TERMS & 2) ? w_lo : nullptr);
-    { MapModel mm{}; mm.kind = 2; mm.z = a.z; mm.rows = a.Cout; mm.M = a.M; mm.ldz = a.ldz; memset(&mZ, 0, sizeof(mZ)); memcpy(&mZ, &mm, sizeof(mm)); }
     a.tiles_n = ceil_div(a.Cout, BN);
     a.tiles_total = a.tiles_n * ceil_div(a.M, TC_BM);
     const int grid = PERSIST ? ctas : a.tiles_total;
     g_deadlock.store(false);
-    emul::launch(dim3(grid), dim3(192), Cfg::SMEM_BYTES, [&]() {
+    emul::launch(dim3(grid), dim3(TC_THREADS), Cfg::SMEM_BYTES, [&]() {
         if (threadIdx.x == 0) {
-            memset(g_tmem, 0, sizeof(g_tmem));
             std::lock_guard<std::mutex> l(g_mu);
             g_bars.clear();
             for (auto& nb : g_named) nb = NamedBar{};
         }
         pthread_barrier_wait(&emul::g_block.bar);
-        conv_tc_kernel<BN, BK, NH, TERMS, PERSIST, MINB>(mAh, mAl, mBh, mBl, mZ, a);
+        conv_tc_kernel<BN, BK, TERMS, PERSIST, FOLD>(mAh, mAl, mBh, mBl, a);
     });
     return g_deadlock.load() ? -100 : 0;
 }
 
-template <int BN, int BK, int NH, bool PERSIST, int MINB>
+template <int BN, int BK, bool PERSIST, bool FOLD>
 static int run_terms(int terms, const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* w_hi, const uint16_t* w_lo,
                      const TcArgs& a, int B, int ctas) {
     switch (terms) {
-        case 0: return run<BN, BK, 1, 0, PERSIST, MINB>(x_hi, x_lo, w_hi, w_lo, a, B, ctas);
-        case 1: return run<BN, BK, 1, 1, PERSIST, MINB>(x_hi, x_lo, w_hi, w_lo, a, B, ctas);
-        case 2: return run<BN, BK, 1, 2, PERSIST, MINB>(x_hi, x_lo, w_hi, w_lo, a, B, ctas);
-        default: return run<BN, BK, NH, 3, PERSIST, MINB>(x_hi, x_lo, w_hi, w_lo, a, B, ctas);
+        case 0: return run<BN, BK, 0, PERSIST, FOLD>(x_hi, x_lo, w_hi, w_lo, a, B, ctas);
+        case 1: return run<BN, BK, 1, PERSIST, FOLD>(x_hi, x_lo, w_hi, w_lo, a, B, ctas);
+        case 2: return run<BN, BK, 2, PERSIST, FOLD>(x_hi, x_lo, w_hi, w_lo, a, B, ctas);
+        default: return run<BN, BK, 3, PERSIST, FOLD>(x_hi, x_lo, w_hi, w_lo, a, B, ctas);
     }
 }
 
 // returns 0, or -100 when a barrier wait timed out (deadlock: wrong phase / arrival count).
 //   bk = 32: short-K flavour (persist = 0: one tile per CTA, `ctas` ignored; persist = 1: `ctas` CTAs walk the tiles,
-//            ctas must be a multiple of ceil(Cout / bn));  bk = 64: long-K flavour (3 rotating hi accumulators for terms = 3)
+//            ctas must be a multiple of ceil(Cout / bn));  bk = 64: long-K flavour (hi*hi k-blocks folded into a total)
 //   stats: optional [rows][4*Cout] partial rows (rows = persist ? ctas / tiles_n : number of 128-pixel tiles)
 extern "C" int emul_conv_tc(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* w_hi, const uint16_t* w_lo,
                             const float* amax_x, const float* amax_w, float* z, int ldz, int B, int H, int W, int Cin,
@@ -295,17 +212,17 @@ extern "C" int emul_conv_tc(const uint16_t* x_hi, const uint16_t* x_lo, const ui
     a.ks = ks; a.pad = (ks - 1) / 2; a.cpitch = cpitch; a.M = (long long)B * H * W; a.accumulate = accumulate;
     a.tiles_n = a.tiles_total = 0; a.nofuse = 0;
     if (bk == 32 && persist) {
-        if (bn == 64) return run_terms<64, 32, 1, true, 1>(terms, x_hi, x_lo, w_hi, w_lo, a, B, ctas);
-        if (bn == 128) return run_terms<128, 32, 1, true, 1>(terms, x_hi, x_lo, w_hi, w_lo, a, B, ctas);
+        if (bn == 64) return run_terms<64, 32, true, false>(terms, x_hi, x_lo, w_hi, w_lo, a, B, ctas);
+        if (bn == 128) return run_terms<128, 32, true, false>(terms, x_hi, x_lo, w_hi, w_lo, a, B, ctas);
     } else if (bk == 32) {
-        if (bn == 64) return run_terms<64, 32, 1, false, 2>(terms, x_hi, x_lo, w_hi, w_lo, a, B, ctas);
-        if (bn == 128) return run_terms<128, 32, 1, false, 2>(terms, x_hi, x_lo, w_hi, w_lo, a, B, ctas);
+        if (bn == 64) return run_terms<64, 32, false, false>(terms, x_hi, x_lo, w_hi, w_lo, a, B, ctas);
+        if (bn == 128) return run_terms<128, 32, false, false>(terms, x_hi, x_lo, w_hi, w_lo, a, B, ctas);
     } else if (bk == 64 && !persist) {
-        if (bn == 64) return run_terms<64, 64, 3, false, 1>(terms, x_hi, x_lo, w_hi, w_lo, a, B, ctas);
-        if (bn == 128) return run_terms<128, 64, 3, false, 1>(terms, x_hi, x_lo, w_hi, w_lo, a, B, ctas);
+        if (bn == 64) return run_terms<64, 64, false, true>(terms, x_hi, x_lo, w_hi, w_lo, a, B, ctas);
+        if (bn == 128) return run_terms<128, 64, false, true>(terms, x_hi, x_lo, w_hi, w_lo, a, B, ctas);
     }
     return -1;
 }
 
-// test knob: every tcgen05.ld of the model sleeps this long (0 = off)
-extern "C" void emul_set_ld_delay_us(int us) { fsdet::g_ld_delay_us.store(us); }
+// test knob: every wgmma wait of the model sleeps this long (0 = off)
+extern "C" void emul_set_ld_delay_us(int us) { fsdet::g_mma_delay_us.store(us); }

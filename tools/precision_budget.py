@@ -1,7 +1,7 @@
 """Precision budget of the tensor-core GEMM classes (VERDICT r1 item 3): what does each operand-term mode of the
 forward / input-gradient / weight-gradient GEMMs cost in accuracy on the REAL layer shapes, and what does it buy?
 
-    python tools/precision_budget.py [B] [n_cls] [out.json]       (on a B200; default B = 16, n_cls = 20)
+    python tools/precision_budget.py [B] [n_cls] [out.json]       (on an H100; default B = 16, n_cls = 20)
 
 One seeded meta-training step (full darknet_dynamic + reweighting_net at 416x416) is evaluated
   * with torch's own float64 kernels on the device (the oracle module in float64) = ground truth,

@@ -1,4 +1,4 @@
-"""Developer tool: measured precision of the 3xBF16 tcgen05 convolution vs float64."""
+"""Developer tool: measured precision of the 3xBF16 tensor-core convolution vs float64."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
