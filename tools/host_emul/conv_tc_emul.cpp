@@ -1,154 +1,14 @@
-// Host build of csrc/conv_tc_kernels.cuh against FUNCTIONAL MODELS of the PTX wrappers it uses (see
+// Host build of csrc/conv_tc_kernels.cuh against FUNCTIONAL MODELS of the PTX wrappers it uses (tc_models_emul.h; see
 // cuda_host_emul.h for the thread model).  What is modelled: mbarriers (arrival counts, transaction bytes, phase
 // parity), the im2col / tiled TMA loads (boxes land 64- / 128-byte swizzled, like the hardware's), wgmma with the device
 // descriptor encoding (wgmma_emul.h), named barriers.  What this validates: the kernel's CONTROL FLOW - stage phases,
 // tile sequencing over a persistent grid, accumulate flags of the three-MMA hi/lo scheme and of the k-block totals,
 // the epilogue's fragment -> row mapping, edge clipping, the fused statistics - and the shared-memory descriptors it
 // builds.  A wrong phase shows up as a deadlock (reported after a timeout) or as a wrong result.  Test tooling only.
-#include <cuda.h>
-#include <cuda_fp16.h>
-
-#include <atomic>
-#include <chrono>
-#include <map>
-#include <mutex>
-
-#include "../../fewshot_detection_b200/csrc/common.cuh"
-
-namespace emul {
-Block g_block;
-unsigned char* g_dyn_smem = nullptr;
-}  // namespace emul
+#include "tc_models_emul.h"
 
 namespace fsdet {
-void set_error(const char*, ...) {}
-
-// ---- helpers conv_tc.cu defines before including the kernel header
-constexpr int EMUL_BM = 128;   // == TC_BM (checked below)
-static inline float scale_from_amax(float a) {   // conv_tc.cu: power of two mapping amax into [512, 1024)
-    if (!(a > 0.f) || !std::isfinite(a)) return 1.f;
-    int ex = (int)((__float_as_uint(a) >> 23) & 0xff) - 126;
-    int e = 10 - ex;
-    e = e < -60 ? -60 : (e > 60 ? 60 : e);
-    return __uint_as_float((uint32_t)(e + 127) << 23);
-}
-static inline float ldg_f32(const float* p) { return *p; }
-
-// ---- models
-static std::atomic<bool> g_deadlock{false};
-static std::mutex g_mu;
-struct Bar { int count, pending; long long tx; int phase; };
-static std::map<const void*, Bar> g_bars;
-
-struct MapModel {   // lives in the first bytes of a CUtensorMap
-    int kind;       // 0 = im2col activation plane, 1 = weight plane, 2 = fp32 output
-    const uint16_t* base;
-    float* z;
-    int B, H, W, C, cpitch, ks, pad, bk, box_rows, rows, ldz;
-    long long K, M;
-};
-static inline const MapModel* model(const CUtensorMap* m) { return reinterpret_cast<const MapModel*>(m); }
-
-static inline uint32_t smem_u32(const void* p) { return (uint32_t)((const unsigned char*)p - emul::g_dyn_smem); }
-
-static void bar_check(Bar& b) {
-    if (b.pending == 0 && b.tx == 0) { b.phase ^= 1; b.pending = b.count; }
-}
-static inline void mbar_init(uint64_t* bar, uint32_t count) {
-    std::lock_guard<std::mutex> l(g_mu);
-    g_bars[bar] = Bar{(int)count, (int)count, 0, 0};
-}
-static inline void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    std::lock_guard<std::mutex> l(g_mu);
-    Bar& b = g_bars[bar];
-    b.tx += bytes; b.pending -= 1;
-    bar_check(b);
-}
-static inline void bar_complete_tx(uint64_t* bar, uint32_t bytes) {
-    std::lock_guard<std::mutex> l(g_mu);
-    Bar& b = g_bars[bar];
-    b.tx -= bytes;
-    bar_check(b);
-}
-static inline void mbar_arrive(uint64_t* bar) {
-    std::lock_guard<std::mutex> l(g_mu);
-    Bar& b = g_bars[bar];
-    b.pending -= 1;
-    bar_check(b);
-}
-static inline void mbar_wait(uint64_t* bar, uint32_t parity) {
-    const auto t0 = std::chrono::steady_clock::now();
-    for (;;) {
-        {
-            std::lock_guard<std::mutex> l(g_mu);
-            if ((uint32_t)g_bars[bar].phase != parity) return;   // the phase with this parity has completed
-        }
-        if (g_deadlock.load()) return;
-        if (std::chrono::steady_clock::now() - t0 > std::chrono::seconds(60)) { g_deadlock.store(true); return; }
-        std::this_thread::sleep_for(std::chrono::microseconds(20));   // whole warps poll (elect_one pattern): keep the lock free
-    }
-}
-// whole-warp wait: OS threads are not lock-step, a slow lane could miss a complete phase flip that lane 0 already acted
-// on - so lane 0 polls and the warp converges behind it
-static inline void mbar_wait_warp(uint64_t* bar, uint32_t parity) {
-    if ((threadIdx.x & 31) == 0) mbar_wait(bar, parity);
-    __syncwarp();
-}
-static inline void fence_barrier_init() {}
-static inline void fence_proxy_async() {}
-static inline void tma_prefetch_desc(const CUtensorMap*) {}
-
-#include "wgmma_emul.h"
-
-// element k of row r of a TMA box with rows of `row_bytes` bytes, through the shared-memory swizzle of the tensor map
-static inline void box_store(void* dst, int r, int k, int row_bytes, uint16_t v) {
-    const uint32_t a = swizzle_addr(smem_u32(dst) + (uint32_t)(r * row_bytes + k * 2), row_bytes == 128 ? GMMA_SW128 : GMMA_SW64);
-    memcpy(emul::g_dyn_smem + a, &v, 2);
-}
-
-// 128 consecutive output pixels starting at the pixel whose filter window has its corner at (w, h) of image n;
-// one filter tap (off_w, off_h), channels c .. c+bk-1; zero outside the image / beyond the last pixel
-static inline void tma_load_im2col_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c, int w, int h, int n,
-                                      uint16_t off_w, uint16_t off_h) {
-    const MapModel* m = model(map);
-    long long pix0 = ((long long)n * m->H + (h + m->pad)) * m->W + (w + m->pad);
-    const long long total = (long long)m->B * m->H * m->W;
-    for (int i = 0; i < EMUL_BM; ++i) {
-        const long long pi = pix0 + i;
-        bool ok = pi < total;
-        int img = 0, y = 0, x = 0;
-        if (ok) {
-            img = (int)(pi / ((long long)m->H * m->W));
-            const int rem = (int)(pi - (long long)img * m->H * m->W);
-            y = rem / m->W - m->pad + off_h;
-            x = rem % m->W - m->pad + off_w;
-            ok = y >= 0 && y < m->H && x >= 0 && x < m->W;
-        }
-        for (int k = 0; k < m->bk; ++k) {
-            const int ch = c + k;
-            box_store(dst, i, k, m->bk * 2, (ok && ch < m->C) ? m->base[(((size_t)img * m->H + y) * m->W + x) * m->cpitch + ch] : (uint16_t)0);
-        }
-    }
-    bar_complete_tx(bar, (uint32_t)(EMUL_BM * m->bk * 2));
-}
-static inline void tma_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
-    const MapModel* m = model(map);
-    for (int r = 0; r < m->box_rows; ++r)
-        for (int k = 0; k < m->bk; ++k) {
-            const long long row = c1 + r, col = c0 + k;
-            box_store(dst, r, k, m->bk * 2, (row < m->rows && col < m->K) ? m->base[(size_t)row * m->K + col] : (uint16_t)0);
-        }
-    bar_complete_tx(bar, (uint32_t)(m->box_rows * m->bk * 2));
-}
-// thread-block clusters are not modelled (blocks run one after another): the cluster flavour is never instantiated here
-static inline uint32_t cluster_ctarank() { return 0; }
-static inline void cluster_sync_all() {}
-static inline void tma_load_2d_mc(void*, const CUtensorMap*, uint64_t*, int, int, uint16_t) { g_deadlock.store(true); }
-static inline void mbar_arrive_cluster(uint64_t*, uint32_t) { g_deadlock.store(true); }
-static inline bool elect_one() { return (threadIdx.x & 31) == 0; }
-
 #include "../../fewshot_detection_b200/csrc/conv_tc_kernels.cuh"
-static_assert(EMUL_BM == TC_BM, "tile height of the models");
 
 }  // namespace fsdet
 
@@ -162,7 +22,7 @@ static int run(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* w_hi,
     const long long K = (long long)a.ks * a.ks * a.cpitch;
     auto act = [&](CUtensorMap* m, const uint16_t* base) {
         MapModel mm{}; mm.kind = 0; mm.base = base; mm.B = B; mm.H = a.H; mm.W = a.W; mm.C = a.Cin; mm.cpitch = a.cpitch;
-        mm.ks = a.ks; mm.pad = a.pad; mm.bk = BK;
+        mm.ks = a.ks; mm.pad = a.pad; mm.bk = BK; mm.box_rows = TC_BM;
         memset(m, 0, sizeof(*m)); memcpy(m, &mm, sizeof(mm));
     };
     auto wgt = [&](CUtensorMap* m, const uint16_t* base) {
@@ -176,6 +36,7 @@ static int run(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* w_hi,
     a.tiles_total = a.tiles_n * ceil_div(a.M, TC_BM);
     const int grid = PERSIST ? ctas : a.tiles_total;
     g_deadlock.store(false);
+    g_fault.store(false);
     emul::launch(dim3(grid), dim3(TC_THREADS), Cfg::SMEM_BYTES, [&]() {
         if (threadIdx.x == 0) {
             std::lock_guard<std::mutex> l(g_mu);
@@ -185,7 +46,7 @@ static int run(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* w_hi,
         pthread_barrier_wait(&emul::g_block.bar);
         conv_tc_kernel<BN, BK, TERMS, PERSIST, FOLD>(mAh, mAl, mBh, mBl, a);
     });
-    return g_deadlock.load() ? -100 : 0;
+    return g_deadlock.load() ? -100 : (g_fault.load() ? -101 : 0);
 }
 
 template <int BN, int BK, bool PERSIST, bool FOLD>
@@ -199,7 +60,8 @@ static int run_terms(int terms, const uint16_t* x_hi, const uint16_t* x_lo, cons
     }
 }
 
-// returns 0, or -100 when a barrier wait timed out (deadlock: wrong phase / arrival count).
+// returns 0, -100 when a barrier wait timed out (deadlock: wrong phase / arrival count), or -101 when a TMA load used a
+// filter offset outside the map's window.
 //   bk = 32: short-K flavour (persist = 0: one tile per CTA, `ctas` ignored; persist = 1: `ctas` CTAs walk the tiles,
 //            ctas must be a multiple of ceil(Cout / bn));  bk = 64: long-K flavour (hi*hi k-blocks folded into a total)
 //   stats: optional [rows][4*Cout] partial rows (rows = persist ? ctas / tiles_n : number of 128-pixel tiles)
