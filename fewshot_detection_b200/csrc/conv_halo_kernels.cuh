@@ -18,8 +18,9 @@
 //     gradient, 72 KB) it is loaded ONCE per CTA and stays resident, otherwise it streams through a ring of (tap, chunk)
 //     stages filled by a second producer warp.
 //
-// Arithmetic: 3-term fp16 hi/lo scheme (conv_tc_kernels.cuh, TERMS = 3) - D_hi += A_hi * B_hi, D_lo += A_lo * B_hi +
-// A_hi * B_lo, summed in the epilogue.  K <= 1152 here, so one hi accumulator (the im2col short-K flavour's choice).
+// Arithmetic: 3-term fp16 hi/lo scheme (conv_tc_kernels.cuh, TERMS = 3) - D_hi += A_hi * B_hi, D_lo += A_hi * B_lo +
+// A_lo * B_hi (three MMAs of width BN per K step), summed in the epilogue.  K <= 1152 here, so one hi accumulator (the
+// im2col short-K flavour's choice).
 //
 // Warps (384 threads): 0 = activation producer (+ resident weights), 1 = weight-ring producer (idle when the weights
 // are resident), 2-3 idle (the producer warpgroup hands its registers to the MMA warpgroups); warpgroups 1 and 2 =
@@ -37,9 +38,8 @@ struct HaloArgs {
     int tiles_x, tiles_y;
     int tiles_total;     // B * tiles_x * tiles_y
     int accumulate;
-    int flags;           // developer knob FSDET_HALO_FLAGS.  bit 2: three MMAs per K step instead of the fused pair (same products).
-                         // Timing experiments only (results invalid): bit 0 = fetch one halo copy instead of three,
-                         // bit 1 = no output stores, bit 3 = hi*hi term only
+    int flags;           // developer knob FSDET_HALO_FLAGS, timing experiments only (results invalid): bit 0 = fetch one
+                         // halo copy instead of three, bit 1 = no output stores.  Other bits are ignored.
 };
 
 constexpr int HALO_TW = 8, HALO_TH = 16;
@@ -166,8 +166,6 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constan
         const int wq = warp & 3;
         const int ct = (int)threadIdx.x - 128;
         constexpr int NR = BN / 2;
-        const bool fused = !(p.flags & 4);                     // flags bit 2 selects the three-MMA form (A / B experiments)
-        const bool hi_only = (p.flags & 8) != 0;
         const float inv = 1.f / (scale_from_amax(p.amax_a ? ldg_f32(p.amax_a) : 0.f) * scale_from_amax(p.amax_b ? ldg_f32(p.amax_b) : 0.f));
         const bool want_stats = p.stats != nullptr;
         float ssum = 0.f, esum = 0.f, ssq = 0.f, esq = 0.f, smin = INFINITY, smax = -INFINITY;
@@ -186,10 +184,6 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constan
         unsigned ita = 0, itb = 0;
         for (int tile = (int)blockIdx.x; tile < tiles_total; tile += (int)gridDim.x) {
             uint32_t started = 0;
-            if (hi_only) {
-#pragma unroll
-                for (int i = NR; i < 2 * NR; ++i) acc[i] = 0.f;
-            }
 #pragma unroll 1
             for (int chunk = 0; chunk < NCH; ++chunk, ++ita) {
                 const int sa = ita % SA;
@@ -214,18 +208,9 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constan
 #pragma unroll
                         for (int k = 0; k < 2; ++k) {          // 16 halves = 32 B along K inside the swizzle atom: + 2 in the descriptor
                             const uint64_t adv = (uint64_t)(2 * k);
-                            if (hi_only) {
-                                wgmma<BN>(acc, ah + adv, bh + adv, started);
-                            } else if (fused) {
-                                // [D_hi | D_lo] (+)= A_hi * [B_hi | B_lo]: ONE MMA of width 2*BN (the lo block follows the hi block
-                                // in shared memory, the lo accumulator follows the hi accumulator in registers); D_lo += A_lo * B_hi
-                                wgmma<2 * BN>(acc, ah + adv, bh + adv, started);
-                                wgmma<BN>(acc + NR, al + adv, bh + adv, 1u);
-                            } else {
-                                wgmma<BN>(acc, ah + adv, bh + adv, started);
-                                wgmma<BN>(acc + NR, al + adv, bh + adv, started);
-                                wgmma<BN>(acc + NR, ah + adv, bl + adv, 1u);
-                            }
+                            wgmma<BN>(acc, ah + adv, bh + adv, started);
+                            wgmma<BN>(acc + NR, ah + adv, bl + adv, started);
+                            wgmma<BN>(acc + NR, al + adv, bh + adv, 1u);
                             started = 1u;
                         }
                         wgmma_commit();

@@ -264,7 +264,7 @@ struct TcPlan {
 // 128 input and output channels (short K: the im2col kernel is L2-bound there), a width that tiles by 8, little padding
 // waste in the 16-row direction and enough tiles to fill the persistent grid.  mode bit 6 switches it off.
 static bool halo_ok(int B, int H, int W, int Cin, int Cout, int ksize, int mode) {
-    if (ksize != 3 || (mode & 3) != 3 || (mode & 0x70)) return false;     // bit 7 (no fused MMA) does not change the plan
+    if (ksize != 3 || (mode & 3) != 3 || (mode & 0x70)) return false;
     if (!(Cin == 32 || Cin == 64 || Cin == 128) || Cout > 128) return false;
     if (W % HALO_TW != 0) return false;
     const int ty = ceil_div(H, HALO_TH);
@@ -421,7 +421,7 @@ static int run_halo(const void* x_hi, const void* x_lo, const void* w_hi, const 
     h.amax_a = a.amax_a; h.amax_b = a.amax_b; h.z = a.z; h.ldz = a.ldz; h.stats = a.stats; h.H = a.H; h.W = a.W; h.Cout = a.Cout; h.cpitch = a.cpitch;
     h.tiles_x = pl.tiles_x; h.tiles_y = pl.tiles_y; h.tiles_total = pl.tiles_m; h.accumulate = a.accumulate;
     const char* dbg = getenv("FSDET_HALO_FLAGS");      // developer knob (tools/halo_bench.py): see HaloArgs::flags
-    h.flags = (dbg ? atoi(dbg) : 0) | (a.nofuse ? 4 : 0);
+    h.flags = dbg ? atoi(dbg) : 0;
     const int nch = a.Cin / 32;
     if (pl.bn == 32) return launch_halo_nch<32>(nch, a_hi, a_lo, b_hi, b_lo, h, pl.grid, s);
     if (pl.bn == 64) return launch_halo_nch<64>(nch, a_hi, a_lo, b_hi, b_lo, h, pl.grid, s);
@@ -543,6 +543,7 @@ extern "C" int fsdet_conv_tc_fwd(const void* x_hi, const void* x_lo, const void*
                                  const float* amax_w, float* z, int ldz, int B, int H, int W, int Cin, int cpitch, int Cout,
                                  int ksize, int accumulate, int mode, float* stat_partial, void* stream) {
     const int terms = mode & 3;
+    // bit 7 asks for three MMAs per K step, which every kernel issues: accepted so that callers setting it keep working
     FSDET_CHECK_ARG((mode & ~0xf3) == 0, "conv_tc_fwd: unknown mode bits 0x%x", mode);
     FSDET_CHECK_ARG(x_hi && w_hi && z && (!(terms & 1) || x_lo) && (!(terms & 2) || w_lo), "conv_tc_fwd: null pointer (mode %d)", mode);
     FSDET_CHECK_ARG(fsdet_conv_tc_supported(Cin, Cout, ksize) && cpitch >= Cin && cpitch % 8 == 0,
@@ -555,7 +556,7 @@ extern "C" int fsdet_conv_tc_fwd(const void* x_hi, const void* x_lo, const void*
     TcArgs a;
     a.z = z; a.amax_a = amax_x; a.amax_b = amax_w; a.stats = stat_partial; a.ldz = ldz; a.H = H; a.W = W; a.Cin = Cin;
     a.Cout = Cout; a.ks = ksize; a.pad = (ksize - 1) / 2; a.cpitch = cpitch; a.M = (long long)B * H * W;
-    a.accumulate = accumulate; a.tiles_n = a.tiles_total = 0; a.nofuse = (mode & 128) ? 1 : 0;
+    a.accumulate = accumulate; a.tiles_n = a.tiles_total = 0;
     if (a.M == 0) return 0;
     FSDET_CHECK_ARG(a.M < (1ll << 31) - 256, "conv_tc_fwd: too many pixels");
     return run_tc(x_hi, x_lo, w_hi, w_lo, B, a, mode, (cudaStream_t)stream);

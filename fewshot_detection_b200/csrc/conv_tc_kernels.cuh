@@ -23,6 +23,13 @@
 // summed in a fresh accumulator and added to a register total with round-to-nearest; the small lo terms accumulate
 // over the whole K.
 //
+// Every MMA of a K step has the width BN and writes registers no other MMA of the same group writes at the same time
+// (a wider A_hi * [B_hi | B_lo] followed by A_lo * B_hi into half of its registers makes ptxas serialise every wgmma of
+// the kernel).  One wgmma group stays in flight across k-blocks: the short-K flavour issues one group per k-block and
+// waits for the previous one; the FOLD flavour issues the hi*hi group and then the lo group of a k-block, so that
+// wait<1> completes the hi group and its sum is added to the total while the lo MMAs still run.  A stage is released
+// once every group that read it is complete, i.e. one k-block late.
+//
 // PERSIST = false: one output tile per CTA (grid = number of tiles).
 // PERSIST = true : CTAs walk tiles blockIdx.x, blockIdx.x + gridDim.x, ...; the producer runs ahead across tile
 //              boundaries.  gridDim.x must be a multiple of tiles_n (then every CTA keeps one channel range: the
@@ -46,7 +53,6 @@ struct TcArgs {
     long long M;      // B*H*W
     int accumulate;
     int tiles_n, tiles_total;
-    int nofuse;       // mode bit 7: keep A_hi * B_hi and A_hi * B_lo as two MMAs (A / B comparisons of the fused form)
 };
 
 constexpr int TC_BM = 128;
@@ -257,10 +263,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant_
         const int wq = warp & 3;
         const int ct = (int)threadIdx.x - 128;                 // 0 .. 255
         constexpr int NR = BN / 2;                             // accumulator registers per thread and term
-        // TERMS = 3 with one hi accumulator: A_hi * [B_hi | B_lo] is ONE MMA of width 2*BN - the lo plane follows the hi
-        // plane in the stage and the lo accumulator follows the hi accumulator in registers (A_hi is read once)
-        constexpr bool CAN_FUSE = TERMS == 3 && !FOLD && 2 * BN <= 256;
-        const bool fused = CAN_FUSE && !p.nofuse;
         constexpr uint32_t SWZ = BK == 64 ? GMMA_SW128 : GMMA_SW64;
         constexpr uint32_t SBO = 8 * Cfg::ROW_BYTES;
         const float inv = 1.f / (scale_from_amax(p.amax_a ? ldg_f32(p.amax_a) : 0.f) * scale_from_amax(p.amax_b ? ldg_f32(p.amax_b) : 0.f));
@@ -299,40 +301,45 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant_
                 const uint64_t al = ah + (uint64_t)(Cfg::OFF_ALO >> 4);
                 const uint64_t bh = gmma_desc(st + Cfg::OFF_BHI, 0, SBO, SWZ);
                 const uint64_t bl = bh + (uint64_t)(Cfg::B_BYTES >> 4);
+                // 16 halves = 32 B along K inside the swizzle atom: + 2 in the descriptor
                 wgmma_fence();
+                if (FOLD) {
 #pragma unroll
-                for (int k = 0; k < BK / 16; ++k) {            // 16 halves = 32 B along K inside the swizzle atom: + 2 in the descriptor
-                    const uint32_t first_hi = (FOLD ? k > 0 : (kb > 0 || k > 0)) ? 1u : 0u;
-                    const uint32_t first_lo = (kb > 0 || k > 0) ? 1u : 0u;
-                    const uint64_t adv = (uint64_t)(2 * k);
-                    if (CAN_FUSE && fused) {
-                        wgmma<CAN_FUSE ? 2 * BN : BN>(acc, ah + adv, bh + adv, first_hi);
-                        wgmma<BN>(acc + NR, al + adv, bh + adv, 1u);
-                    } else {
-                        wgmma<BN>(acc, ah + adv, bh + adv, first_hi);
-                        if (TERMS & 1) wgmma<BN>(acc + NR, al + adv, bh + adv, first_lo);
-                        if (TERMS & 2) wgmma<BN>(acc + NR, ah + adv, bl + adv, (TERMS & 1) ? 1u : first_lo);
+                    for (int k = 0; k < BK / 16; ++k) wgmma<BN>(acc, ah + 2 * k, bh + 2 * k, k > 0 ? 1u : 0u);
+                    if (TERMS) {                               // the lo terms as a second group
+                        wgmma_commit();
+#pragma unroll
+                        for (int k = 0; k < BK / 16; ++k) {
+                            const uint32_t first_lo = (kb > 0 || k > 0) ? 1u : 0u;
+                            if (TERMS & 1) wgmma<BN>(acc + NR, al + 2 * k, bh + 2 * k, first_lo);
+                            if (TERMS & 2) wgmma<BN>(acc + NR, ah + 2 * k, bl + 2 * k, (TERMS & 1) ? 1u : first_lo);
+                        }
+                    }
+                } else {
+#pragma unroll
+                    for (int k = 0; k < BK / 16; ++k) {
+                        const uint32_t first = (kb > 0 || k > 0) ? 1u : 0u;
+                        wgmma<BN>(acc, ah + 2 * k, bh + 2 * k, first);
+                        if (TERMS & 2) wgmma<BN>(acc + NR, ah + 2 * k, bl + 2 * k, first);
+                        if (TERMS & 1) wgmma<BN>(acc + NR, al + 2 * k, bh + 2 * k, (TERMS & 2) ? 1u : first);
                     }
                 }
                 wgmma_commit();
-                if (FOLD) {                                    // the k-block's hi sum is read now: wait for all of it
-                    wgmma_wait<0>();
-                    wgmma_use<TERMS ? 2 * NR : NR>(acc);
-                    release(s);
+                // short K: the previous k-block is complete.  FOLD: so is this k-block's hi group (TERMS = 0 has no lo group)
+                if (FOLD && TERMS == 0) wgmma_wait<0>();
+                else wgmma_wait<1>();
+                if (FOLD) {
+                    wgmma_use<NR>(acc);
 #pragma unroll
                     for (int i = 0; i < NR; ++i) tot[i] += acc[i];
-                } else {                                       // one k-block stays in flight: the previous one has read its stage
-                    wgmma_wait<1>();
-                    if (pend >= 0) release(pend);
-                    pend = s;
                 }
-            }
-            if (!FOLD) {
-                wgmma_wait<0>();
-                wgmma_use<TERMS ? 2 * NR : NR>(acc);
                 if (pend >= 0) release(pend);
-                pend = -1;
+                pend = s;
             }
+            wgmma_wait<0>();
+            wgmma_use<TERMS ? 2 * NR : NR>(acc);
+            if (pend >= 0) release(pend);
+            pend = -1;
             if (nk == 0) {
 #pragma unroll
                 for (int i = 0; i < (TERMS ? 2 * NR : NR); ++i) acc[i] = 0.f;

@@ -8,7 +8,10 @@
 // = 128 B), A = dz tile via a 2-D tiled map, B = x tile of ONE filter tap via the im2col map (zero-filled halo).
 // One CTA = 128 co x BN ci x one tap over a range of pixels (split-K across blockIdx.z): a producer warp and two MMA
 // warpgroups of 64 co each.  The hi*hi products of every 64-pixel stage are summed in a fresh accumulator and added to
-// a register total (round-to-nearest: the tensor core's fp32 accumulation truncates, see conv_tc.cu).
+// a register total (round-to-nearest: the tensor core's fp32 accumulation truncates, see conv_tc.cu).  That addition
+// overlaps MMAs still in flight: TERMS = 0 alternates two hi accumulators (stage kb + 1 is issued before stage kb is
+// added), the other modes issue the lo terms as a second wgmma group after the hi*hi group.  A stage is released one
+// k-block late, once every group that read it is complete.
 #pragma once
 
 struct TcWgArgs {
@@ -120,15 +123,18 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDhi, const __grid_constant
         const int cw = (warp >> 2) - 1;                 // MMA warpgroup: output channels co0 + 64 cw .. + 63
         const int wq = warp & 3;
         constexpr int NR = BN / 2;
-        float acc[TERMS ? 2 * NR : NR];                 // [hi | lo]
+        // TERMS != 0: [hi | lo].  TERMS = 0: two hi accumulators used in turn, so that k-block kb + 1 is in flight while
+        // the sum of k-block kb is added to the total
+        float acc[2 * NR];
         float tot[NR];
 #pragma unroll
         for (int i = 0; i < NR; ++i) tot[i] = 0.f;
 #pragma unroll
-        for (int i = 0; i < (TERMS ? 2 * NR : NR); ++i) acc[i] = 0.f;
+        for (int i = 0; i < 2 * NR; ++i) acc[i] = 0.f;
         const uint32_t smem_base = smem_u32(smem);
-#pragma unroll 1
-        for (int kb = 0; kb < nk; ++kb) {
+        // k-block kb: its hi*hi products into the fresh accumulator `hi` as one wgmma group, then (TERMS != 0) the lo terms
+        // into acc[NR..] as a second group
+        auto issue = [&](int kb, float* hi) {
             const int s = kb % STAGES;
             mbar_wait(&full_bar[s], (kb / STAGES) & 1);
             const uint32_t st = smem_base + s * Cfg::STAGE_BYTES;
@@ -139,20 +145,62 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDhi, const __grid_constant
             const uint64_t bl = bh + (uint64_t)(Cfg::B_BYTES >> 4);
             wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < WG_BP / 16; ++k) {
-                const uint64_t adv = (uint64_t)(k * (2048 >> 4));   // 16 pixels = two 8-row groups of 1024 B
-                const uint32_t first_lo = (kb > 0 || k > 0) ? 1u : 0u;
-                wgmma<BN, 1, 1>(acc, ah + adv, bh + adv, k > 0 ? 1u : 0u);
-                if (TERMS & 1) wgmma<BN, 1, 1>(acc + NR, al + adv, bh + adv, first_lo);
-                if (TERMS & 2) wgmma<BN, 1, 1>(acc + NR, ah + adv, bl + adv, (TERMS & 1) ? 1u : first_lo);
-            }
+            for (int k = 0; k < WG_BP / 16; ++k)        // 16 pixels = two 8-row groups of 1024 B
+                wgmma<BN, 1, 1>(hi, ah + k * (2048 >> 4), bh + k * (2048 >> 4), k > 0 ? 1u : 0u);
             wgmma_commit();
-            wgmma_wait<0>();
-            wgmma_use<TERMS ? 2 * NR : NR>(acc);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty_bar[s]);
+            if (TERMS) {
 #pragma unroll
-            for (int i = 0; i < NR; ++i) tot[i] += acc[i];
+                for (int k = 0; k < WG_BP / 16; ++k) {
+                    const uint64_t adv = (uint64_t)(k * (2048 >> 4));
+                    const uint32_t first_lo = (kb > 0 || k > 0) ? 1u : 0u;
+                    if (TERMS & 1) wgmma<BN, 1, 1>(acc + NR, al + adv, bh + adv, first_lo);
+                    if (TERMS & 2) wgmma<BN, 1, 1>(acc + NR, ah + adv, bl + adv, (TERMS & 1) ? 1u : first_lo);
+                }
+                wgmma_commit();
+            }
+        };
+        auto fold = [&](float* hi) {                    // `hi` holds a completed k-block sum
+            wgmma_use<NR>(hi);
+#pragma unroll
+            for (int i = 0; i < NR; ++i) tot[i] += hi[i];
+        };
+        auto release = [&](int kb) {                    // every group that read k-block kb's stage is complete
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[kb % STAGES]);
+        };
+        if (TERMS) {
+#pragma unroll 1
+            for (int kb = 0; kb < nk; ++kb) {
+                issue(kb, acc);
+                wgmma_wait<1>();                        // only this k-block's lo group may still run
+                fold(acc);
+                if (kb > 0) release(kb - 1);
+            }
+        } else {
+#pragma unroll 1
+            for (int kb = 0; kb < nk; kb += 2) {
+                issue(kb, acc);
+                if (kb > 0) {
+                    wgmma_wait<1>();                    // k-block kb - 1 is complete
+                    fold(acc + NR);
+                    release(kb - 1);
+                }
+                if (kb + 1 < nk) {
+                    issue(kb + 1, acc + NR);
+                    wgmma_wait<1>();                    // k-block kb is complete
+                    fold(acc);
+                    release(kb);
+                }
+            }
+        }
+        wgmma_wait<0>();
+        wgmma_use<2 * NR>(acc);
+        if (nk > 0) {
+            if (!TERMS) {                               // the last k-block's sum (even k-blocks use acc, odd ones acc + NR)
+                if (nk & 1) fold(acc);
+                else fold(acc + NR);
+            }
+            release(nk - 1);
         }
         const float inv = 1.f / (scale_from_amax(p.amax_a ? __ldg(p.amax_a) : 0.f) * scale_from_amax(p.amax_b ? __ldg(p.amax_b) : 0.f));
         const long long K = (long long)p.ks * p.ks * p.Cin;

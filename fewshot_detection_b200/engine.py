@@ -54,13 +54,8 @@ TC_CLUSTER = os.environ.get('FSDET_TC_CLUSTER', '0') == '1'
 TC_HALO = os.environ.get('FSDET_TC_HALO', '1') != '0'
 
 
-# A_hi * [B_hi | B_lo] as one MMA of width 2*BN (two MMAs per K step instead of three): on unless FSDET_TC_FUSE=0
-TC_FUSE = os.environ.get('FSDET_TC_FUSE', '1') != '0'
-
-
 def tc_mode(name):
-    return (TC_TERMS[name] | (16 if TC_PERSIST else 0) | (32 if TC_CLUSTER else 0) | (0 if TC_HALO else 64)
-            | (0 if TC_FUSE else 128))
+    return TC_TERMS[name] | (16 if TC_PERSIST else 0) | (32 if TC_CLUSTER else 0) | (0 if TC_HALO else 64)
 
 # Weight gradients on a second stream: after a block's BatchNorm backward, its weight-gradient GEMM (tensor-bound, one
 # CTA per SM) and the rest of the backward chain (input gradient, then the next block's HBM-bound BatchNorm passes) are

@@ -143,11 +143,9 @@ int fsdet_pad_channels(const float* in, int cin, float* out, int cout, size_t ro
  *     run the halo-tile kernel (csrc/conv_halo_kernels.cuh: the input tile is
  *     fetched once with its halo for all nine taps instead of once per tap - those
  *     layers are L2-bandwidth bound otherwise); fsdet_conv_tc_uses_halo tells.
- *     Bit 7 (128): issue x_hi*w_hi and x_hi*w_lo as two MMAs.  By default the
- *     mode-3 kernels with one hi accumulator issue them as ONE MMA of width
- *     2*BN (the lo weight plane follows the hi plane in shared memory, the lo
- *     accumulator follows the hi accumulator in registers): same products, two
- *     wgmma per K step instead of three.
+ *     Bit 7 (128): three MMAs of width BN per K step (x_hi*w_hi, x_hi*w_lo,
+ *     x_lo*w_hi).  Every kernel issues that form, so the bit is accepted and
+ *     changes nothing.
  * x_hi/x_lo dense NHWC [B*H*W][cpitch] fp16, w_hi/w_lo [Cout][k*k*cpitch] fp16,
  * amax_x / amax_w: device floats holding the tensors' absolute maxima (NULL =
  * planes are unscaled).  Output fp32 z[p][n] (+ previous z when accumulate

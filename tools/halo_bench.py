@@ -36,8 +36,8 @@ def main():
     ]
     if ncu:
         shapes = shapes[:4]
-    print('%-22s %10s  halo us by FSDET_HALO_FLAGS %s (4 = fused hi|lo MMA; 1 / 2 / 8 = timing experiments: one halo copy / no '
-          'stores / hi*hi only)' % ('layer', 'im2col us', flag_list))
+    print('%-22s %10s  halo us by FSDET_HALO_FLAGS %s (1 / 2 = timing experiments: one halo copy / no stores)'
+          % ('layer', 'im2col us', flag_list))
     for name, B, H, W, Cin, cp, Cout in shapes:
         npix = B * H * W
         xh, xl, xa = planes(npix, cp, 1)

@@ -1,5 +1,5 @@
 """Developer tool: one halo-tile convolution launch (conv2 forward shape, B images) under FSDET_HALO_FLAGS, compared with
-the im2col kernel - small enough for compute-sanitizer.  Usage: FSDET_HALO_FLAGS=4 python tools/halo_one.py [B]"""
+the im2col kernel - small enough for compute-sanitizer.  Usage: python tools/halo_one.py [B]"""
 import os
 import sys
 

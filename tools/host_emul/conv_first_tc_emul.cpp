@@ -85,6 +85,7 @@ using namespace fsdet;
 template <int MODE>
 static int run(FtArgs a, int ctas) {
     g_deadlock.store(false);
+    g_wgmma_pending_at_exit.store(false);
     emul::launch(dim3(ctas), dim3(FT_THREADS), FtCfg<MODE>::SMEM_BYTES + 1024, [&]() {
         if (threadIdx.x == 0) {
             std::lock_guard<std::mutex> l(g_mu);
@@ -94,8 +95,9 @@ static int run(FtArgs a, int ctas) {
         // the kernel aligns its dynamic shared memory to 1 KB: make offset 0 of the model 1 KB aligned too
         pthread_barrier_wait(&emul::g_block.bar);
         conv_first_tc_kernel<MODE>(a);
+        wgmma_block_exit();
     });
-    return g_deadlock.load() ? -100 : 0;
+    return g_deadlock.load() ? -100 : (g_wgmma_pending_at_exit.load() ? -102 : 0);
 }
 
 extern "C" int emul_conv_first_tc(int mode, int ctas, const float* in0, int C0, const float* in1, int C1, const float* w,

@@ -42,6 +42,7 @@ static int run_halo(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* 
     act(&mAh, x_hi); act(&mAl, x_lo); wgt(&mBh, w_hi); wgt(&mBl, w_lo);
     a.z = z; a.ldz = ldz;
     g_deadlock.store(false);
+    g_wgmma_pending_at_exit.store(false);
     emul::launch(dim3(ctas), dim3(HALO_THREADS), Cfg::SMEM_BYTES, [&]() {
         if (threadIdx.x == 0) {
             std::lock_guard<std::mutex> l(g_mu);
@@ -50,8 +51,9 @@ static int run_halo(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* 
         }
         pthread_barrier_wait(&emul::g_block.bar);
         conv_halo_kernel<BN, NCH, BRES>(mAh, mAl, mBh, mBl, a);
+        wgmma_block_exit();
     });
-    return g_deadlock.load() ? -100 : 0;
+    return g_deadlock.load() ? -100 : (g_wgmma_pending_at_exit.load() ? -102 : 0);
 }
 
 template <int BN>
@@ -65,7 +67,8 @@ static int run_halo_nch(int nch, const uint16_t* x_hi, const uint16_t* x_lo, con
     return -1;
 }
 
-// 3x3 convolution through the halo-tile kernel on `ctas` persistent CTAs; returns 0, -100 on a barrier deadlock.
+// 3x3 convolution through the halo-tile kernel on `ctas` persistent CTAs; returns 0, -100 on a barrier deadlock, -102
+// when a thread ended with wgmma operations not waited for.
 // stats: optional [ctas][4*Cout] partial rows
 extern "C" int emul_conv_halo(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* w_hi, const uint16_t* w_lo,
                               const float* amax_x, const float* amax_w, float* z, int ldz, int B, int H, int W, int Cin, int cpitch,

@@ -37,6 +37,7 @@ static int run(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* w_hi,
     const int grid = PERSIST ? ctas : a.tiles_total;
     g_deadlock.store(false);
     g_fault.store(false);
+    g_wgmma_pending_at_exit.store(false);
     emul::launch(dim3(grid), dim3(TC_THREADS), Cfg::SMEM_BYTES, [&]() {
         if (threadIdx.x == 0) {
             std::lock_guard<std::mutex> l(g_mu);
@@ -45,8 +46,9 @@ static int run(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* w_hi,
         }
         pthread_barrier_wait(&emul::g_block.bar);
         conv_tc_kernel<BN, BK, TERMS, PERSIST, FOLD>(mAh, mAl, mBh, mBl, a);
+        wgmma_block_exit();
     });
-    return g_deadlock.load() ? -100 : (g_fault.load() ? -101 : 0);
+    return g_deadlock.load() ? -100 : (g_fault.load() ? -101 : (g_wgmma_pending_at_exit.load() ? -102 : 0));
 }
 
 template <int BN, int BK, bool PERSIST, bool FOLD>
@@ -60,8 +62,8 @@ static int run_terms(int terms, const uint16_t* x_hi, const uint16_t* x_lo, cons
     }
 }
 
-// returns 0, -100 when a barrier wait timed out (deadlock: wrong phase / arrival count), or -101 when a TMA load used a
-// filter offset outside the map's window.
+// returns 0, -100 when a barrier wait timed out (deadlock: wrong phase / arrival count), -101 when a TMA load used a
+// filter offset outside the map's window, or -102 when a thread ended with wgmma operations not waited for.
 //   bk = 32: short-K flavour (persist = 0: one tile per CTA, `ctas` ignored; persist = 1: `ctas` CTAs walk the tiles,
 //            ctas must be a multiple of ceil(Cout / bn));  bk = 64: long-K flavour (hi*hi k-blocks folded into a total)
 //   stats: optional [rows][4*Cout] partial rows (rows = persist ? ctas / tiles_n : number of 128-pixel tiles)
@@ -72,7 +74,7 @@ extern "C" int emul_conv_tc(const uint16_t* x_hi, const uint16_t* x_lo, const ui
     TcArgs a;
     a.z = z; a.amax_a = amax_x; a.amax_b = amax_w; a.stats = stats; a.ldz = ldz; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout;
     a.ks = ks; a.pad = (ks - 1) / 2; a.cpitch = cpitch; a.M = (long long)B * H * W; a.accumulate = accumulate;
-    a.tiles_n = a.tiles_total = 0; a.nofuse = 0;
+    a.tiles_n = a.tiles_total = 0;
     if (bk == 32 && persist) {
         if (bn == 64) return run_terms<64, 32, true, false>(terms, x_hi, x_lo, w_hi, w_lo, a, B, ctas);
         if (bn == 128) return run_terms<128, 32, true, false>(terms, x_hi, x_lo, w_hi, w_lo, a, B, ctas);

@@ -36,6 +36,7 @@ static int run(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* dz_hi
     const dim3 grid(((a.Cin + CIB - 1) / CIB) * ((a.ks * a.ks + TAPS - 1) / TAPS), (a.Cout + 127) / 128, splits);
     g_deadlock.store(false);
     g_fault.store(false);
+    g_wgmma_pending_at_exit.store(false);
     emul::launch(grid, dim3(384), Cfg::SMEM_BYTES, [&]() {
         if (threadIdx.x == 0) {
             std::lock_guard<std::mutex> l(g_mu);
@@ -43,8 +44,9 @@ static int run(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* dz_hi
         }
         pthread_barrier_wait(&emul::g_block.bar);
         wgrad_tc_kernel<TAPS, TERMS>(mDh, mDl, mXh, mXl, a);
+        wgmma_block_exit();
     });
-    return g_deadlock.load() ? -100 : (g_fault.load() ? -101 : 0);
+    return g_deadlock.load() ? -100 : (g_fault.load() ? -101 : (g_wgmma_pending_at_exit.load() ? -102 : 0));
 }
 
 template <int TAPS>
@@ -61,7 +63,8 @@ static int run_terms(int terms, const uint16_t* x_hi, const uint16_t* x_lo, cons
 // Weight gradient of an NHWC x [B][H][W][Cin] and dz [B*H*W][Cout] (fp16 hi / lo planes) into out [splits][Cout][k*k*Cin]:
 // slice z holds the sum over pixels [z * pix_per_split, min((z + 1) * pix_per_split, M)), unreduced, exactly as
 // fsdet_conv_tc_wgrad's workspace.  Two taps per N tile when Cin < 128 (as wg_taps in conv_tc.cu).
-// Returns 0, -100 on a barrier deadlock, -101 on a TMA load outside the im2col filter window, -1 on bad arguments.
+// Returns 0, -100 on a barrier deadlock, -101 on a TMA load outside the im2col filter window, -102 when a thread ended
+// with wgmma operations not waited for, -1 on bad arguments.
 extern "C" int emul_conv_wgrad(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* dz_hi, const uint16_t* dz_lo,
                                const float* amax_x, const float* amax_dz, float* out, int B, int H, int W, int Cin, int Cout,
                                int ks, int terms, int splits, long long pix_per_split) {

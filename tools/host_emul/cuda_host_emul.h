@@ -12,6 +12,7 @@
 #include <stdint.h>
 #include <string.h>
 
+#include <deque>
 #include <functional>
 #include <thread>
 #include <vector>

@@ -7,7 +7,14 @@
 // aligned) shared-memory offset.  The modelled TMA loads store their boxes through the same swizzle, so descriptor
 // encodings, K advances inside a swizzle atom and the TMA / wgmma layout agreement are all checked on the CPU.
 // Each thread computes its own accumulator fragment (rows 16 * warp + lane / 4 (+ 8), columns 8j + 2 (lane % 4) (+ 1)
-// of the warpgroup's 64 x N tile) at the call - the asynchronous completion is not modelled.
+// of the warpgroup's 64 x N tile).
+//
+// Completion is asynchronous, as on the device: wgmma() only queues the operation in the thread's open group,
+// wgmma_commit() closes that group, and wgmma_wait<N>() executes the oldest committed groups - reading shared memory and
+// writing the accumulators at that moment - until at most N remain.  A stage released to the producer before the group
+// that reads it has been waited for, or an accumulator read before its group is complete, therefore gives a wrong result
+// once the producer runs ahead (g_mma_delay_us).  Operations still queued when a block ends are a kernel bug:
+// wgmma_block_exit() reports them.
 #pragma once
 
 constexpr uint32_t GMMA_SW128 = 1, GMMA_SW64 = 2;
@@ -35,22 +42,50 @@ static inline float gmma_operand(uint64_t desc, bool mn_major, int idx, int k) {
     return emul_h2f(v);
 }
 
-template <int N, int TA = 0, int TB = 0>
-static inline void wgmma(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+struct WgmmaOp {
+    float* d;
+    uint64_t da, db;
+    uint32_t accumulate;
+    int n;
+    bool ta, tb;
+};
+static inline void wgmma_execute(const WgmmaOp& o) {
     const int t = (int)(threadIdx.x & 127), wq = t >> 5, lane = t & 31;
-    for (int j = 0; j < N / 8; ++j)
+    for (int j = 0; j < o.n / 8; ++j)
         for (int e = 0; e < 4; ++e) {
             const int row = 16 * wq + (lane >> 2) + 8 * (e >> 1), col = 8 * j + 2 * (lane & 3) + (e & 1);
-            float acc = accumulate ? d[4 * j + e] : 0.f;
-            for (int k = 0; k < 16; ++k) acc += gmma_operand(da, TA != 0, row, k) * gmma_operand(db, TB != 0, col, k);
-            d[4 * j + e] = acc;
+            float acc = o.accumulate ? o.d[4 * j + e] : 0.f;
+            for (int k = 0; k < 16; ++k) acc += gmma_operand(o.da, o.ta, row, k) * gmma_operand(o.db, o.tb, col, k);
+            o.d[4 * j + e] = acc;
         }
+}
+static thread_local std::vector<WgmmaOp> t_wgmma_open;                 // issued since the last commit
+static thread_local std::deque<std::vector<WgmmaOp>> t_wgmma_groups;   // committed, not yet complete (oldest first)
+
+template <int N, int TA = 0, int TB = 0>
+static inline void wgmma(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    t_wgmma_open.push_back(WgmmaOp{d, da, db, accumulate, N, TA != 0, TB != 0});
 }
 static std::atomic<int> g_mma_delay_us{0};   // slows the MMA warpgroups down so that the producers run far ahead
 static inline void wgmma_fence() {}
-static inline void wgmma_commit() {}
+static inline void wgmma_commit() {
+    t_wgmma_groups.push_back(std::move(t_wgmma_open));
+    t_wgmma_open.clear();
+}
 template <int N> static inline void wgmma_wait() {
     if (g_mma_delay_us.load() > 0) std::this_thread::sleep_for(std::chrono::microseconds(g_mma_delay_us.load()));
+    while (t_wgmma_groups.size() > (size_t)N) {
+        for (const WgmmaOp& o : t_wgmma_groups.front()) wgmma_execute(o);
+        t_wgmma_groups.pop_front();
+    }
+}
+// set when a thread ended a block with wgmma operations still queued (the emulated launches return -102)
+static std::atomic<bool> g_wgmma_pending_at_exit{false};
+// called by every thread when its kernel body returns
+static inline void wgmma_block_exit() {
+    if (!t_wgmma_open.empty() || !t_wgmma_groups.empty()) g_wgmma_pending_at_exit.store(true);
+    t_wgmma_open.clear();
+    t_wgmma_groups.clear();
 }
 template <int R> static inline void wgmma_use(float*) {}
 template <int R> static inline void regs_dec() {}
