@@ -82,6 +82,10 @@ SIGNATURES = {
     'fsdet_nms': ('ppiiiidppp', 'i'),
     'fsdet_nms_boxes64': ('ppiidppp', 'i'),
     'fsdet_rw_running_mean': ('pppppiiip', 'i'),
+    'fsdet_voc_round6': ('pppqp', 'i'),
+    'fsdet_voc_gather': ('pppiiiiiippppqpipp', 'i'),
+    'fsdet_voc_workspace_bytes': ('ii', 'z'),
+    'fsdet_voc_evaluate': ('ppipipppiiidppzppppppppp', 'i'),
     'fsdet_augment_workspace_bytes': ('iiii', 'z'),
     'fsdet_augment_batch': ('pppiiiiipzpppp', 'i'),
     'fsdet_box_masks': ('piiipp', 'i'),

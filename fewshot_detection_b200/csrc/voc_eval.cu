@@ -1,0 +1,634 @@
+// PASCAL VOC detection AP on the device, from the detections that decode + NMS (detect.cu) leave there.
+//
+// Replaces, for evaluation (valid_ensemble.py:153-178 + scripts/voc_eval.py:96-243):
+//   valid.detection_lines / write_detections   one '%f' text line per kept box
+//   voc_eval.voc_eval                          parses the lines back
+//   voc_eval.match_detections                  Python loop over every detection
+//   voc_eval.voc_ap                            precision envelope / VOC07 11-point average
+//
+// Data model.  An accumulator owns a pool of detection records in result-file order (batch, image, survivor order):
+//   rank_key uint32 = class << 20 | (2^20 - 1 - n), n = the '%f' integer of the confidence (prob = n / 1e6)
+//   box      double[4] = the corners after the '%f' -> float() round trip
+// and one group descriptor per (image, class) row: {first record, record count, image index, class}.  A group is a
+// contiguous run of its class's result-file lines.
+//
+// Ranking.  Detections of a class are ranked by a STABLE sort on the confidence, descending: ties keep result-file
+// order.  The host evaluator ranks with np.argsort(-conf), whose order at ties depends on numpy's sort implementation;
+// the stable order is the one deliberate definition here.  Sorting by rank_key ascending, stably, gives exactly this
+// order for every class at once (class-major).
+//
+// Arithmetic follows voc_eval.py in float64 with its operation order and no FMA contraction; see each kernel.
+#include "common.cuh"
+
+namespace fsdet {
+
+constexpr int kVocThreads = 256;
+constexpr int kVocKeyBits = 20;                       // n <= 1e6 < 2^20 for a probability in [0, 1]
+constexpr uint32_t kVocKeyMask = (1u << kVocKeyBits) - 1;
+constexpr int kVocMaxClasses = 1 << (32 - kVocKeyBits);
+constexpr int kVocItems = 8;                          // items per thread of a radix / scan tile
+constexpr int kVocTile = kVocThreads * kVocItems;
+constexpr int kVocFlagIgnored = 0, kVocFlagTP = 1, kVocFlagFP = 2;
+
+struct VocThresholds {
+    double t[11];                                     // the host's np.arange(0., 1.1, 0.1)
+};
+
+// '%f' % x followed by float(): x rounded to a multiple of 1e-6, half to even on the exact binary value, then read
+// back as the correctly rounded n / 1e6.  x * 1e6 = p + e exactly (e from an fma); rint(p) is right unless p sits on
+// a half (decided by the sign of e) or e itself is a half (p integral, p >= 2^52).  For |x| >= 2^33 the spacing of
+// doubles exceeds 2e-6 and float() of the text returns x itself.  NaN and inf pass through.
+__device__ __forceinline__ double voc_round6(double x, double* n_out) {
+    if (!(fabs(x) < 8589934592.0)) {
+        *n_out = x;
+        return x;
+    }
+    const double p = __dmul_rn(x, 1e6);
+    const double e = fma(x, 1e6, -p);
+    double n = rint(p);
+    const double d = __dsub_rn(p, n);                 // exact: |p - n| <= 0.5
+    if (d == 0.5 && e > 0.0) n = __dadd_rn(n, 1.0);
+    else if (d == -0.5 && e < 0.0) n = __dsub_rn(n, 1.0);
+    else if (d == 0.0 && fabs(e) == 0.5 && fmod(n, 2.0) != 0.0) n = e > 0.0 ? __dadd_rn(n, 1.0) : __dsub_rn(n, 1.0);
+    *n_out = n;
+    return __ddiv_rn(n, 1e6);
+}
+
+__global__ void voc_round6_kernel(const double* __restrict__ x, double* __restrict__ y, double* __restrict__ n,
+                                  long long count) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (long long)gridDim.x * blockDim.x) {
+        double k;
+        y[i] = voc_round6(x[i], &k);
+        if (n) n[i] = k;
+    }
+}
+
+// Exclusive prefix sum of one value per thread over a kVocThreads block (Hillis-Steele in shared memory).
+__device__ __forceinline__ unsigned long long voc_block_scan(unsigned long long v, unsigned long long* s,
+                                                            unsigned long long& total) {
+    s[threadIdx.x] = v;
+    __syncthreads();
+    for (int off = 1; off < kVocThreads; off <<= 1) {
+        const unsigned long long t = s[threadIdx.x] + (threadIdx.x >= (unsigned)off ? s[threadIdx.x - off] : 0ull);
+        __syncthreads();
+        s[threadIdx.x] = t;
+        __syncthreads();
+    }
+    const unsigned long long incl = s[threadIdx.x];
+    total = s[kVocThreads - 1];
+    __syncthreads();                                  // s is reused by the caller
+    return incl - v;
+}
+
+// ---- gather: one batch of Detections (after NMS) -> records + group descriptors ---------------------------------
+// counters (int64): [0] records in the pool, [1] groups, [2] first group of the last batch, [3] overflow flag.
+
+// One block: the batch's rows get consecutive groups and record ranges (row order = result-file order per class).
+__global__ void __launch_bounds__(kVocThreads) voc_gather_plan_kernel(const int32_t* __restrict__ keep_count, int N,
+                                                                      int n_cls, const int32_t* __restrict__ image_index,
+                                                                      long long pool_cap, int32_t* __restrict__ groups,
+                                                                      int group_cap, long long* counters) {
+    __shared__ unsigned long long s[kVocThreads];
+    __shared__ int s_ok;
+    const long long pool0 = counters[0], group0 = counters[1];
+    // pass 1: total, to decide whether the batch fits
+    unsigned long long sum = 0;
+    for (int r = threadIdx.x; r < N; r += kVocThreads) sum += (unsigned long long)max(keep_count[r], 0);
+    unsigned long long total;
+    voc_block_scan(sum, s, total);
+    if (threadIdx.x == 0)
+        s_ok = counters[3] == 0 && pool0 + (long long)total <= pool_cap && group0 + N <= (long long)group_cap;
+    __syncthreads();
+    if (!s_ok) {
+        if (threadIdx.x == 0) counters[3] = 1;
+        return;
+    }
+    // pass 2: ordered ranges
+    unsigned long long base = 0;
+    for (int r0 = 0; r0 < N; r0 += kVocThreads) {
+        const int r = r0 + threadIdx.x;
+        const int c = r < N ? max(keep_count[r], 0) : 0;
+        unsigned long long chunk;
+        const unsigned long long pre = voc_block_scan((unsigned long long)c, s, chunk);
+        if (r < N) {
+            int32_t* g = groups + (group0 + r) * 4;
+            g[0] = (int32_t)(pool0 + (long long)(base + pre));
+            g[1] = c;
+            g[2] = image_index[r / n_cls];
+            g[3] = r % n_cls;
+        }
+        base += chunk;
+    }
+    if (threadIdx.x == 0) {
+        counters[0] = pool0 + (long long)total;
+        counters[1] = group0 + N;
+        counters[2] = group0;
+    }
+}
+
+// One block per row: the kept boxes of row r in survivor order, as valid.detection_lines computes and prints them:
+// box = [xs/W, ys/H, ws/W, hs/H, det, cls] (float64 of the float32 candidate), x1 = (box[0] - box[2]/2.0) * width, ...,
+// prob = det * cls; every value through '%f' -> float().
+__global__ void __launch_bounds__(kVocThreads) voc_gather_rows_kernel(const float* __restrict__ cand,
+                                                                      const int32_t* __restrict__ keep, int cap, int H,
+                                                                      int W, int n_cls, const double* __restrict__ image_size,
+                                                                      const int32_t* __restrict__ groups,
+                                                                      const long long* __restrict__ counters,
+                                                                      uint32_t* __restrict__ rank_key,
+                                                                      double* __restrict__ box) {
+    if (counters[3]) return;
+    const int r = blockIdx.x;
+    const int32_t* g = groups + (counters[2] + r) * 4;
+    const long long start = g[0];
+    const int count = g[1];
+    const int cls = r % n_cls;
+    const double width = image_size[(r / n_cls) * 2], height = image_size[(r / n_cls) * 2 + 1];
+    for (int t = threadIdx.x; t < count; t += kVocThreads) {
+        const int slot = keep[(size_t)r * cap + t];
+        const float* v = cand + ((size_t)r * cap + slot) * 8;
+        const double bx = __ddiv_rn((double)v[0], (double)W), by = __ddiv_rn((double)v[1], (double)H);
+        const double bw = __ddiv_rn((double)v[2], (double)W), bh = __ddiv_rn((double)v[3], (double)H);
+        const double hw = __ddiv_rn(bw, 2.0), hh = __ddiv_rn(bh, 2.0);
+        double n;
+        const double x1 = voc_round6(__dmul_rn(__dsub_rn(bx, hw), width), &n);
+        const double y1 = voc_round6(__dmul_rn(__dsub_rn(by, hh), height), &n);
+        const double x2 = voc_round6(__dmul_rn(__dadd_rn(bx, hw), width), &n);
+        const double y2 = voc_round6(__dmul_rn(__dadd_rn(by, hh), height), &n);
+        voc_round6(__dmul_rn((double)v[4], (double)v[5]), &n);
+        const uint32_t key = (uint32_t)fmin(fmax(n, 0.0), (double)kVocKeyMask);
+        const long long d = start + t;
+        rank_key[d] = ((uint32_t)cls << kVocKeyBits) | (kVocKeyMask - key);
+        box[d * 4 + 0] = x1;
+        box[d * 4 + 1] = y1;
+        box[d * 4 + 2] = x2;
+        box[d * 4 + 3] = y2;
+    }
+}
+
+// ---- match: voc_eval.match_detections for one (image, class) group per warp ------------------------------------
+__device__ __forceinline__ double np_minimum(double a, double b) { return a != a ? a : (b != b ? b : (b < a ? b : a)); }
+__device__ __forceinline__ double np_maximum(double a, double b) { return a != a ? a : (b != b ? b : (b > a ? b : a)); }
+
+// The group's detections are ranked (key descending, result-file position ascending: the class-wide stable order
+// restricted to one image) by counting, then lane 0 walks them in rank order: pixel-inclusive IoU with every
+// ground-truth box of the class in the image, the first maximum (np.argmax), a match needs IoU > ovthresh, a match to
+// a difficult box is neither TP nor FP, a match to a claimed box or no match is an FP.
+__global__ void __launch_bounds__(kVocThreads) voc_match_kernel(const uint32_t* __restrict__ rank_key,
+                                                                const double* __restrict__ box,
+                                                                const int32_t* __restrict__ groups, int n_groups,
+                                                                const int32_t* __restrict__ gt_ptr,
+                                                                const int32_t* __restrict__ gt_box,
+                                                                const uint8_t* __restrict__ gt_difficult, int n_images,
+                                                                double ovthresh, int32_t* __restrict__ gperm,
+                                                                uint8_t* __restrict__ claimed,
+                                                                uint8_t* __restrict__ flags) {
+    const int gi = blockIdx.x * (kVocThreads / 32) + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (gi >= n_groups) return;                       // whole warps leave together
+    const int32_t* g = groups + (size_t)gi * 4;
+    const int start = g[0], count = g[1], img = g[2], cls = g[3];
+    for (int j = lane; j < count; j += 32) {
+        const uint32_t kj = rank_key[start + j];
+        int r = 0;
+        for (int m = 0; m < count; ++m) {
+            const uint32_t km = rank_key[start + m];
+            r += (km < kj || (km == kj && m < j)) ? 1 : 0;
+        }
+        gperm[start + r] = j;
+    }
+    __syncwarp();
+    if (lane != 0) return;
+    const int gb = gt_ptr[(size_t)cls * n_images + img], ge = gt_ptr[(size_t)cls * n_images + img + 1];
+    for (int k = gb; k < ge; ++k) claimed[k] = 0;
+    for (int r = 0; r < count; ++r) {
+        const int d = start + gperm[start + r];
+        const double b0 = box[(size_t)d * 4], b1 = box[(size_t)d * 4 + 1], b2 = box[(size_t)d * 4 + 2], b3 = box[(size_t)d * 4 + 3];
+        const double barea = __dmul_rn(__dadd_rn(__dsub_rn(b2, b0), 1.0), __dadd_rn(__dsub_rn(b3, b1), 1.0));
+        double best = -INFINITY;
+        int j = -1;
+        for (int k = gb; k < ge; ++k) {
+            const double g0 = gt_box[k * 4], g1 = gt_box[k * 4 + 1], g2 = gt_box[k * 4 + 2], g3 = gt_box[k * 4 + 3];
+            const double iw = __dadd_rn(__dsub_rn(np_minimum(g2, b2), np_maximum(g0, b0)), 1.0);
+            const double ih = __dadd_rn(__dsub_rn(np_minimum(g3, b3), np_maximum(g1, b1)), 1.0);
+            const double inter = __dmul_rn(np_maximum(iw, 0.0), np_maximum(ih, 0.0));
+            const double garea = __dmul_rn(__dadd_rn(__dsub_rn(g2, g0), 1.0), __dadd_rn(__dsub_rn(g3, g1), 1.0));
+            const double iou = __ddiv_rn(inter, __dsub_rn(__dadd_rn(barea, garea), inter));
+            if (j < 0 || (best == best && (iou != iou || iou > best))) {   // np.argmax: first maximum, a NaN wins
+                best = iou;
+                j = k;
+            }
+        }
+        uint8_t f = kVocFlagFP;
+        if (best > ovthresh) {
+            if (gt_difficult[j]) f = kVocFlagIgnored;
+            else if (!claimed[j]) { f = kVocFlagTP; claimed[j] = 1; }
+        }
+        flags[d] = f;
+    }
+}
+
+// ---- stable LSD radix sort of (rank_key, record index), 8 bits per pass ----------------------------------------
+__global__ void __launch_bounds__(kVocThreads) voc_radix_hist_kernel(const uint32_t* __restrict__ keys, int n, int shift,
+                                                                     int ntiles, unsigned long long* __restrict__ cnt) {
+    __shared__ int h[256];
+    h[threadIdx.x] = 0;
+    __syncthreads();
+    const int tile = blockIdx.x;
+    for (int it = 0; it < kVocItems; ++it) {
+        const int i = tile * kVocTile + it * kVocThreads + threadIdx.x;
+        if (i < n) atomicAdd(&h[(keys[i] >> shift) & 255], 1);
+    }
+    __syncthreads();
+    cnt[(size_t)threadIdx.x * ntiles + tile] = (unsigned long long)h[threadIdx.x];
+}
+
+// cnt_scan[d * ntiles + t] = where tile t's first item of digit d goes.  Items are taken in index order (round, warp,
+// lane), and each one's place among the equal digits before it is counted exactly: the pass is stable.
+__global__ void __launch_bounds__(kVocThreads) voc_radix_scatter_kernel(const uint32_t* __restrict__ keys_in,
+                                                                        const int32_t* __restrict__ vals_in, int n,
+                                                                        int shift, int ntiles,
+                                                                        const unsigned long long* __restrict__ cnt_scan,
+                                                                        uint32_t* __restrict__ keys_out,
+                                                                        int32_t* __restrict__ vals_out) {
+    __shared__ unsigned long long base[256];
+    __shared__ int wc[kVocThreads / 32][256];
+    __shared__ int tot[256];
+    const int tile = blockIdx.x, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    base[threadIdx.x] = cnt_scan[(size_t)threadIdx.x * ntiles + tile];
+    for (int it = 0; it < kVocItems; ++it) {
+        for (int q = 0; q < kVocThreads / 32; ++q) wc[q][threadIdx.x] = 0;
+        __syncthreads();
+        const int i = tile * kVocTile + it * kVocThreads + threadIdx.x;
+        const bool valid = i < n;
+        const uint32_t k = valid ? keys_in[i] : 0u;
+        const int32_t v = valid ? (vals_in ? vals_in[i] : i) : 0;
+        const int dg = (int)((k >> shift) & 255u);
+        unsigned peers = __ballot_sync(0xffffffffu, valid);
+        for (int b = 0; b < 8; ++b) {
+            const bool bit = (dg >> b) & 1;
+            const unsigned m = __ballot_sync(0xffffffffu, bit);
+            peers &= bit ? m : ~m;
+        }
+        const unsigned below = peers & ((1u << lane) - 1u);
+        if (valid && below == 0) wc[w][dg] = __popc(peers);
+        __syncthreads();
+        int run = 0;
+        for (int q = 0; q < kVocThreads / 32; ++q) {
+            const int c = wc[q][threadIdx.x];
+            wc[q][threadIdx.x] = run;
+            run += c;
+        }
+        tot[threadIdx.x] = run;
+        __syncthreads();
+        if (valid) {
+            const unsigned long long dst = base[dg] + (unsigned long long)wc[w][dg] + (unsigned long long)__popc(below);
+            keys_out[dst] = k;
+            vals_out[dst] = v;
+        }
+        __syncthreads();
+        base[threadIdx.x] += (unsigned long long)tot[threadIdx.x];
+    }
+}
+
+// ---- prefix sums over uint64 (three kernels: tile sums, one block over the tile sums, tile scans) -------------------
+__global__ void __launch_bounds__(kVocThreads) voc_scan_partials_kernel(const unsigned long long* __restrict__ a, long long n,
+                                                                        unsigned long long* __restrict__ part) {
+    __shared__ unsigned long long s[kVocThreads];
+    const long long b0 = (long long)blockIdx.x * kVocTile + (long long)threadIdx.x * kVocItems;
+    unsigned long long v = 0;
+    for (int k = 0; k < kVocItems; ++k)
+        if (b0 + k < n) v += a[b0 + k];
+    unsigned long long total;
+    voc_block_scan(v, s, total);
+    if (threadIdx.x == 0) part[blockIdx.x] = total;
+}
+
+__global__ void __launch_bounds__(kVocThreads) voc_scan_top_kernel(unsigned long long* __restrict__ part, int nb) {
+    __shared__ unsigned long long s[kVocThreads];
+    unsigned long long carry = 0;
+    for (int b0 = 0; b0 < nb; b0 += kVocThreads) {
+        const int b = b0 + threadIdx.x;
+        const unsigned long long v = b < nb ? part[b] : 0ull;
+        unsigned long long total;
+        const unsigned long long pre = voc_block_scan(v, s, total);
+        if (b < nb) part[b] = carry + pre;
+        carry += total;
+    }
+}
+
+__global__ void __launch_bounds__(kVocThreads) voc_scan_apply_kernel(unsigned long long* __restrict__ a, long long n,
+                                                                     const unsigned long long* __restrict__ part,
+                                                                     int inclusive) {
+    __shared__ unsigned long long s[kVocThreads];
+    const long long b0 = (long long)blockIdx.x * kVocTile + (long long)threadIdx.x * kVocItems;
+    unsigned long long x[kVocItems], v = 0;
+    for (int k = 0; k < kVocItems; ++k) {
+        x[k] = b0 + k < n ? a[b0 + k] : 0ull;
+        v += x[k];
+    }
+    unsigned long long total;
+    unsigned long long run = part[blockIdx.x] + voc_block_scan(v, s, total);
+    for (int k = 0; k < kVocItems; ++k) {
+        const unsigned long long next = run + x[k];
+        if (b0 + k < n) a[b0 + k] = inclusive ? next : run;
+        run = next;
+    }
+}
+
+// TP count in the high, FP count in the low 32 bits, in rank order: one inclusive scan gives both cumulative sums.
+__global__ void voc_pack_flags_kernel(const int32_t* __restrict__ order, const uint8_t* __restrict__ flags, int n,
+                                      unsigned long long* __restrict__ packed) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const uint8_t f = flags[order[r]];
+    packed[r] = f == kVocFlagTP ? (1ull << 32) : (f == kVocFlagFP ? 1ull : 0ull);
+}
+
+// ---- per-class curves and AP: one block per class ------------------------------------------------------------
+__device__ __forceinline__ int voc_lower_bound(const uint32_t* k, int n, uint32_t v) {
+    int lo = 0, hi = n;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (k[mid] < v) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+__device__ __forceinline__ double voc_rec_at(const unsigned long long* cum, int r, unsigned long long base, double npos) {
+    return __ddiv_rn((double)((cum[r] - base) >> 32), npos);
+}
+
+// rec = tp / float(npos), prec = tp / np.maximum(tp + fp, eps) over the class's ranks; VOC07: ap += max(prec[rec >= t])
+// / 11. for the 11 host thresholds in order (0 where no rank qualifies); area: envelope p[i] = max(prec[i:], 0), summed
+// (r[i+1] - r[i]) * p[i+1] wherever r changes, with r = [0, rec..., 1] (summation order differs from np.sum's).
+__global__ void __launch_bounds__(kVocThreads) voc_ap_kernel(const uint32_t* __restrict__ skeys, int n,
+                                                             const unsigned long long* __restrict__ cum,
+                                                             const int32_t* __restrict__ gt_ptr,
+                                                             const uint8_t* __restrict__ gt_difficult, int n_images,
+                                                             VocThresholds th, double* __restrict__ rec_out,
+                                                             double* __restrict__ prec_out, int32_t* __restrict__ cls_count,
+                                                             int32_t* __restrict__ npos_out, double* __restrict__ ap07,
+                                                             double* __restrict__ ap_area) {
+    __shared__ double s_env[kVocThreads];
+    __shared__ double s_red[kVocThreads / 32][12];
+    __shared__ int s_cnt[kVocThreads / 32];
+    __shared__ double s_carry;
+    const int c = blockIdx.x, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int lo = voc_lower_bound(skeys, n, (uint32_t)c << kVocKeyBits);
+    const int hi = voc_lower_bound(skeys, n, (uint32_t)(c + 1) << kVocKeyBits);
+    // npos = non-difficult ground truths of the class
+    int np_ = 0;
+    for (int k = gt_ptr[(size_t)c * n_images] + threadIdx.x; k < gt_ptr[(size_t)(c + 1) * n_images]; k += kVocThreads)
+        np_ += gt_difficult[k] ? 0 : 1;
+    for (int o = 16; o; o >>= 1) np_ += __shfl_xor_sync(0xffffffffu, np_, o);
+    if (lane == 0) s_cnt[w] = np_;
+    if (threadIdx.x == 0) s_carry = 0.0;
+    __syncthreads();
+    int npos_i = 0;
+    for (int q = 0; q < kVocThreads / 32; ++q) npos_i += s_cnt[q];
+    const double npos = (double)npos_i;
+    const unsigned long long base = lo > 0 ? cum[lo - 1] : 0ull;
+    const double eps = 2.220446049250313e-16;         // np.finfo(np.float64).eps
+    double mx[11];
+    for (int t = 0; t < 11; ++t) mx[t] = -1.0;        // no rank with rec >= t yet (prec >= 0)
+    double area = 0.0;
+    for (int end = hi; end > lo; end -= kVocThreads) {
+        const int i = end - kVocThreads + (int)threadIdx.x;
+        const bool valid = i >= lo;
+        double rec = 0.0, prec = 0.0;
+        if (valid) {
+            const unsigned long long v = cum[i] - base;
+            const double tp = (double)(v >> 32), fp = (double)(v & 0xffffffffull);
+            const double s = __dadd_rn(tp, fp);
+            rec = __ddiv_rn(tp, npos);
+            prec = __ddiv_rn(tp, s > eps ? s : eps);
+            rec_out[i] = rec;
+            prec_out[i] = prec;
+            for (int t = 0; t < 11; ++t)
+                if (rec >= th.t[t] && prec > mx[t]) mx[t] = prec;
+        }
+        // suffix maximum of prec inside the chunk, then with everything after it
+        s_env[threadIdx.x] = valid ? prec : 0.0;
+        __syncthreads();
+        for (int off = 1; off < kVocThreads; off <<= 1) {
+            const double o = threadIdx.x + off < kVocThreads ? s_env[threadIdx.x + off] : 0.0;
+            const double m = fmax(s_env[threadIdx.x], o);
+            __syncthreads();
+            s_env[threadIdx.x] = m;
+            __syncthreads();
+        }
+        const double carry = s_carry;
+        if (valid) {
+            const double env = fmax(s_env[threadIdx.x], carry);
+            const double prev = i == lo ? 0.0 : voc_rec_at(cum, i - 1, base, npos);
+            if (rec != prev) area = __dadd_rn(area, __dmul_rn(__dsub_rn(rec, prev), env));
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) s_carry = fmax(carry, s_env[0]);
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {                           // the last step, to the appended recall 1 (precision 0)
+        const double last = hi > lo ? voc_rec_at(cum, hi - 1, base, npos) : 0.0;
+        if (1.0 != last) area = __dadd_rn(area, __dmul_rn(__dsub_rn(1.0, last), 0.0));
+    }
+    for (int o = 16; o; o >>= 1) {
+        area = __dadd_rn(area, __shfl_xor_sync(0xffffffffu, area, o));
+        for (int t = 0; t < 11; ++t) mx[t] = fmax(mx[t], __shfl_xor_sync(0xffffffffu, mx[t], o));
+    }
+    if (lane == 0) {
+        for (int t = 0; t < 11; ++t) s_red[w][t] = mx[t];
+        s_red[w][11] = area;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double ap = 0.0, a = 0.0;
+        for (int t = 0; t < 11; ++t) {
+            double m = -1.0;
+            for (int q = 0; q < kVocThreads / 32; ++q) m = fmax(m, s_red[q][t]);
+            ap = __dadd_rn(ap, __ddiv_rn(m < 0.0 ? 0.0 : m, 11.0));
+        }
+        for (int q = 0; q < kVocThreads / 32; ++q) a = __dadd_rn(a, s_red[q][11]);
+        ap07[c] = ap;
+        ap_area[c] = a;
+        cls_count[c] = hi - lo;
+        npos_out[c] = npos_i;
+    }
+}
+
+// ---- host side, shared by the library and the host-emulation build -----------------------------------------------
+#ifdef FSDET_HOST_EMULATION
+#define VOC_LAUNCH(grid, block, kernel, ...) emul::launch(dim3(grid), dim3(block), 0, [&]() { kernel(__VA_ARGS__); })
+#define VOC_CHECK(what) ((void)0)
+#else
+#define VOC_LAUNCH(grid, block, kernel, ...) kernel<<<(grid), (block), 0, st>>>(__VA_ARGS__)
+#define VOC_CHECK(what)                            \
+    do {                                           \
+        const int rc_ = launch_status(what);       \
+        if (rc_) return rc_;                       \
+    } while (0)
+#endif
+
+static inline size_t voc_align(size_t b) { return (b + 255) & ~(size_t)255; }
+
+struct VocWorkspace {
+    int32_t* gperm;
+    uint8_t* claimed;
+    uint32_t* keys[2];
+    int32_t* vals[2];
+    uint32_t* skeys;
+    unsigned long long* cnt;
+    unsigned long long* part;
+    unsigned long long* cum;
+    size_t bytes;
+};
+
+static VocWorkspace voc_workspace_layout(void* base, int n_det, int n_gt) {
+    const int ntiles = ceil_div(n_det, kVocTile);
+    const size_t n_cnt = (size_t)256 * ntiles;
+    const size_t n_part = (size_t)ceil_div((long long)(n_cnt > (size_t)n_det ? n_cnt : (size_t)n_det), kVocTile) + 1;
+    VocWorkspace w;
+    unsigned char* p = static_cast<unsigned char*>(base);
+    size_t off = 0;
+    auto take = [&](size_t bytes) { unsigned char* q = p ? p + off : nullptr; off += voc_align(bytes); return q; };
+    w.gperm = reinterpret_cast<int32_t*>(take((size_t)n_det * 4));
+    w.claimed = take((size_t)n_gt + 1);
+    w.keys[0] = reinterpret_cast<uint32_t*>(take((size_t)n_det * 4));
+    w.keys[1] = reinterpret_cast<uint32_t*>(take((size_t)n_det * 4));
+    w.vals[0] = reinterpret_cast<int32_t*>(take((size_t)n_det * 4));
+    w.vals[1] = reinterpret_cast<int32_t*>(take((size_t)n_det * 4));
+    w.skeys = nullptr;
+    w.cnt = reinterpret_cast<unsigned long long*>(take(n_cnt * 8));
+    w.part = reinterpret_cast<unsigned long long*>(take(n_part * 8));
+    w.cum = reinterpret_cast<unsigned long long*>(take((size_t)n_det * 8));
+    w.bytes = off;
+    return w;
+}
+
+static int voc_scan(unsigned long long* a, long long n, unsigned long long* part, int inclusive, cudaStream_t st) {
+    (void)st;
+    const int nb = ceil_div(n, kVocTile);
+    VOC_LAUNCH(nb, kVocThreads, voc_scan_partials_kernel, a, n, part);
+    VOC_CHECK("voc_scan_partials");
+    VOC_LAUNCH(1, kVocThreads, voc_scan_top_kernel, part, nb);
+    VOC_CHECK("voc_scan_top");
+    VOC_LAUNCH(nb, kVocThreads, voc_scan_apply_kernel, a, n, part, inclusive);
+    VOC_CHECK("voc_scan_apply");
+    return 0;
+}
+
+static int voc_gather_impl(const float* cand, const int32_t* keep, const int32_t* keep_count, int N, int cap, int H, int W,
+                           int n_cls, const int32_t* image_index, const double* image_size, uint32_t* rank_key,
+                           double* box, long long pool_cap, int32_t* groups, int group_cap, long long* counters,
+                           cudaStream_t st) {
+    (void)st;
+    VOC_LAUNCH(1, kVocThreads, voc_gather_plan_kernel, keep_count, N, n_cls, image_index, pool_cap, groups, group_cap,
+               counters);
+    VOC_CHECK("voc_gather_plan");
+    VOC_LAUNCH(N, kVocThreads, voc_gather_rows_kernel, cand, keep, cap, H, W, n_cls, image_size, groups, counters,
+               rank_key, box);
+    VOC_CHECK("voc_gather_rows");
+    return 0;
+}
+
+static int voc_evaluate_impl(const uint32_t* rank_key, const double* box, int n_det, const int32_t* groups, int n_groups,
+                             const int32_t* gt_ptr, const int32_t* gt_box, const uint8_t* gt_difficult, int n_gt,
+                             int n_cls, int n_images, double ovthresh, const VocThresholds& th, void* workspace,
+                             uint8_t* flags, int32_t* order, double* rec, double* prec, int32_t* cls_count,
+                             int32_t* npos, double* ap07, double* ap_area, cudaStream_t st) {
+    (void)st;
+    VocWorkspace w = voc_workspace_layout(workspace, n_det, n_gt);
+    const uint32_t* skeys = rank_key;
+    if (n_det > 0) {
+        if (n_groups > 0) {
+            VOC_LAUNCH(ceil_div(n_groups, kVocThreads / 32), kVocThreads, voc_match_kernel, rank_key, box, groups,
+                       n_groups, gt_ptr, gt_box, gt_difficult, n_images, ovthresh, w.gperm, w.claimed, flags);
+            VOC_CHECK("voc_match");
+        }
+        int bits = kVocKeyBits;
+        while ((1 << (bits - kVocKeyBits)) < n_cls) ++bits;
+        const int passes = (bits + 7) / 8;
+        const int ntiles = ceil_div(n_det, kVocTile);
+        const uint32_t* kin = rank_key;
+        const int32_t* vin = nullptr;
+        for (int p = 0; p < passes; ++p) {
+            const bool last = p == passes - 1;
+            uint32_t* kout = w.keys[p & 1];
+            int32_t* vout = last ? order : w.vals[p & 1];
+            VOC_LAUNCH(ntiles, kVocThreads, voc_radix_hist_kernel, kin, n_det, 8 * p, ntiles, w.cnt);
+            VOC_CHECK("voc_radix_hist");
+            const int rc = voc_scan(w.cnt, (long long)256 * ntiles, w.part, 0, st);
+            if (rc) return rc;
+            VOC_LAUNCH(ntiles, kVocThreads, voc_radix_scatter_kernel, kin, vin, n_det, 8 * p, ntiles, w.cnt, kout, vout);
+            VOC_CHECK("voc_radix_scatter");
+            kin = kout;
+            vin = vout;
+        }
+        skeys = kin;
+        VOC_LAUNCH(ceil_div(n_det, kVocThreads), kVocThreads, voc_pack_flags_kernel, order, flags, n_det, w.cum);
+        VOC_CHECK("voc_pack_flags");
+        const int rc = voc_scan(w.cum, n_det, w.part, 1, st);
+        if (rc) return rc;
+    }
+    VOC_LAUNCH(n_cls, kVocThreads, voc_ap_kernel, skeys, n_det, w.cum, gt_ptr, gt_difficult, n_images, th, rec, prec,
+               cls_count, npos, ap07, ap_area);
+    VOC_CHECK("voc_ap");
+    return 0;
+}
+
+}  // namespace fsdet
+
+#ifndef FSDET_HOST_EMULATION
+using namespace fsdet;
+
+extern "C" int fsdet_voc_round6(const double* x, double* y, double* n, long long count, void* stream) {
+    FSDET_CHECK_ARG(count >= 0 && (count == 0 || (x && y)), "voc_round6: null pointer");
+    if (count == 0) return 0;
+    const int blocks = (int)(count < (1ll << 20) ? ceil_div(count, kVocThreads) : 4096);
+    voc_round6_kernel<<<blocks, kVocThreads, 0, (cudaStream_t)stream>>>(x, y, n, count);
+    return launch_status("voc_round6");
+}
+
+extern "C" int fsdet_voc_gather(const float* cand, const int32_t* keep, const int32_t* keep_count, int N, int cap, int H,
+                                int W, int nC, int n_cls, const int32_t* image_index, const double* image_size,
+                                uint32_t* rank_key, double* box, long long pool_cap, int32_t* groups, int group_cap,
+                                long long* counters, void* stream) {
+    FSDET_CHECK_ARG(cand && keep && keep_count && image_index && image_size && rank_key && box && groups && counters,
+                    "voc_gather: null pointer");
+    FSDET_CHECK_ARG(nC == 1, "voc_gather: rows with %d (conf, id) pairs; only the meta detector's nC = 1 is supported", nC);
+    FSDET_CHECK_ARG(n_cls > 0 && n_cls <= kVocMaxClasses && N >= 0 && N % n_cls == 0,
+                    "voc_gather: %d rows are not images x %d classes (1..%d)", N, n_cls, kVocMaxClasses);
+    FSDET_CHECK_ARG(cap > 0 && H > 0 && W > 0 && pool_cap >= 0 && pool_cap <= 0x7fffffffll && group_cap >= 0,
+                    "voc_gather: bad shape");
+    if (N == 0) return 0;
+    return voc_gather_impl(cand, keep, keep_count, N, cap, H, W, n_cls, image_index, image_size, rank_key, box, pool_cap,
+                           groups, group_cap, counters, (cudaStream_t)stream);
+}
+
+extern "C" size_t fsdet_voc_workspace_bytes(int n_det, int n_gt) {
+    if (n_det < 0 || n_gt < 0) return 0;
+    return voc_workspace_layout(nullptr, n_det, n_gt).bytes;
+}
+
+extern "C" int fsdet_voc_evaluate(const uint32_t* rank_key, const double* box, int n_det, const int32_t* groups,
+                                  int n_groups, const int32_t* gt_ptr, const int32_t* gt_box, const uint8_t* gt_difficult,
+                                  int n_gt, int n_cls, int n_images, double ovthresh, const double* thresholds,
+                                  void* workspace, size_t workspace_bytes, uint8_t* flags, int32_t* order, double* rec,
+                                  double* prec, int32_t* cls_count, int32_t* npos, double* ap07, double* ap_area,
+                                  void* stream) {
+    FSDET_CHECK_ARG(gt_ptr && thresholds && cls_count && npos && ap07 && ap_area, "voc_evaluate: null pointer");
+    FSDET_CHECK_ARG(n_det == 0 || (rank_key && box && groups && flags && order && rec && prec && workspace),
+                    "voc_evaluate: null pointer");
+    FSDET_CHECK_ARG(n_gt == 0 || (gt_box && gt_difficult), "voc_evaluate: null ground-truth pointer");
+    FSDET_CHECK_ARG(n_det >= 0 && n_groups >= 0 && n_gt >= 0 && n_images > 0 && n_cls > 0 && n_cls <= kVocMaxClasses,
+                    "voc_evaluate: bad shape");
+    FSDET_CHECK_ARG(workspace_bytes >= voc_workspace_layout(nullptr, n_det, n_gt).bytes,
+                    "voc_evaluate: workspace of %zu bytes, %zu needed", workspace_bytes,
+                    voc_workspace_layout(nullptr, n_det, n_gt).bytes);
+    VocThresholds th;
+    for (int t = 0; t < 11; ++t) th.t[t] = thresholds[t];
+    return voc_evaluate_impl(rank_key, box, n_det, groups, n_groups, gt_ptr, gt_box, gt_difficult, n_gt, n_cls, n_images,
+                             ovthresh, th, workspace, flags, order, rec, prec, cls_count, npos, ap07, ap_area,
+                             (cudaStream_t)stream);
+}
+#endif  // FSDET_HOST_EMULATION

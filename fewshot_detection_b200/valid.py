@@ -10,6 +10,10 @@ same files:
     dets = detect(m, data, dw, n_cls)                                    # Detections, NMS done, still on the device
     write_detections(fps, dets, imgids, sizes, n_cls)                    # 'imgid prob x1 y1 x2 y2' per class file
 
+or, without the files, scores them where they are (voc_eval.DeviceVocEval, csrc/voc_eval.cu):
+
+    evaluator.add(dets, imgids, sizes); ...; evaluator.result()          # the dict voc_eval.mean_ap returns
+
 CUDA only (libfsdet.so); no host fallback.
 """
 import os
@@ -131,3 +135,20 @@ def valid_batches(m, meta_batches, image_batches, class_names, prefix, outfile):
         for fp in fps:
             fp.close()
     return dynamic_weights
+
+
+def valid_batches_ap(m, meta_batches, image_batches, evaluator, use_07_metric=True, novel_classes=(), fps=None):
+    """valid_batches followed by voc_eval.mean_ap, with the detections kept on the device: `evaluator` is a
+    voc_eval.DeviceVocEval over the evaluated image set, `image_batches` yields (data, imgids, sizes) with imgids
+    names of that set.  Returns mean_ap's dict.  fps (optional, one open file per class) also receives the result
+    lines valid_batches would write."""
+    n_cls = len(evaluator.classes)
+    m.eval()
+    dynamic_weights = ensemble_dynamic_weights(m, meta_batches, n_cls)
+    dev = next(m.parameters()).device
+    for data, imgids, sizes in image_batches:
+        dets = detect(m, data.to(dev), dynamic_weights, n_cls)
+        evaluator.add(dets, imgids, sizes)
+        if fps is not None:
+            write_detections(fps, dets, imgids, sizes, n_cls)
+    return evaluator.result(use_07_metric, novel_classes)

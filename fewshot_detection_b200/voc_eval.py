@@ -130,7 +130,179 @@ def voc_eval(detpath, annopath, imagesetfile, classname, cachedir, ovthresh=0.5,
 def mean_ap(detpath, annopath, imagesetfile, classes, cachedir, use_07_metric=True, novel_classes=()):
     """Per-class AP plus the base / novel means the reference prints (scripts/voc_eval.py:_do_python_eval)."""
     aps = dict((c, voc_eval(detpath, annopath, imagesetfile, c, cachedir, 0.5, use_07_metric)[2]) for c in classes)
+    return _ap_summary(classes, aps, novel_classes)
+
+
+def _ap_summary(classes, aps, novel_classes):
     base = [aps[c] for c in classes if c not in novel_classes]
     novel = [aps[c] for c in classes if c in novel_classes]
     return {'ap': aps, 'mean': float(np.mean(list(aps.values()))), 'mean_base': float(np.mean(base)) if base else None,
             'mean_novel': float(np.mean(novel)) if novel else None}
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# The same numbers without the result files: detections stay on the device (csrc/voc_eval.cu).
+VOC07_THRESHOLDS = np.arange(0., 1.1, 0.1)          # voc_ap's thresholds, handed to the device as computed here
+
+
+def gt_tables(classes, imagenames, recs):
+    """Ground truth as CSR over (class, image): gt_ptr int32 [n_cls*n_images + 1], boxes int32 [n_gt, 4] and
+    difficult uint8 [n_gt], objects in annotation order (the order voc_eval builds `R`)."""
+    cidx = dict((c, i) for i, c in enumerate(classes))
+    per = [[[] for _ in imagenames] for _ in classes]
+    for k, name in enumerate(imagenames):
+        for o in recs[name]:
+            i = cidx.get(o['name'])
+            if i is not None:
+                per[i][k].append(o)
+    ptr, boxes, diff = [0], [], []
+    for i in range(len(classes)):
+        for objs in per[i]:
+            boxes.extend([int(v) for v in o['bbox']] for o in objs)
+            diff.extend(1 if o['difficult'] else 0 for o in objs)
+            ptr.append(len(boxes))
+    return (np.array(ptr, dtype=np.int32), np.array(boxes, dtype=np.int32).reshape(-1, 4),
+            np.array(diff, dtype=np.uint8))
+
+
+def _call(name, *args):
+    from ._lib import call
+    return call(name, *args)
+
+
+def _ptr(t):
+    return None if t is None else t.data_ptr()
+
+
+def _stream():
+    import torch
+    return torch.cuda.current_stream().cuda_stream
+
+
+class DeviceVocEval(object):
+    """voc_eval / mean_ap over detections that never leave the device.
+
+        ev = DeviceVocEval(classes, imagenames, load_annotations(annopath, imagenames, cachedir))
+        for each batch:  ev.add(dets, image_indices, sizes)     # Detections after .nms(0.45), nC = 1 (meta detector)
+        ev.result(use_07_metric=True, novel_classes=())          # the dict mean_ap returns
+
+    `add` appends the batch's kept boxes in the order write_detections writes lines and computes them as those lines
+    read back: float64, the reference's operation order, '%f' rounding (csrc/voc_eval.cu).  `result` matches, ranks
+    and scores every class on the device; only per-class numbers come back (and, with curves=True, rec / prec).
+    Ranking differs from the file path in one deliberate way: detections with equal printed confidences keep
+    result-file order (a stable sort), where np.argsort's order at ties depends on numpy's sort implementation.
+    Each image of the set may be added once."""
+
+    def __init__(self, classes, imagenames, recs, device=None, ovthresh=0.5):
+        import torch
+        self.classes, self.imagenames = list(classes), list(imagenames)
+        self.index = dict((n, k) for k, n in enumerate(self.imagenames))
+        if len(self.index) != len(self.imagenames):
+            raise ValueError('image names must be distinct')
+        self.device = torch.device(device) if device is not None else torch.device('cuda', torch.cuda.current_device())
+        self.ovthresh = float(ovthresh)
+        ptr, boxes, diff = gt_tables(self.classes, self.imagenames, recs)
+        self.n_gt = int(len(diff))
+        self.gt_ptr = torch.from_numpy(ptr).to(self.device)
+        self.gt_box = torch.from_numpy(boxes).to(self.device)
+        self.gt_difficult = torch.from_numpy(diff).to(self.device)
+        self.group_cap = len(self.classes) * len(self.imagenames)
+        self.groups = torch.zeros(max(self.group_cap, 1), 4, dtype=torch.int32, device=self.device)
+        self.counters = torch.zeros(4, dtype=torch.int64, device=self.device)
+        self.pool_cap = 0
+        self.rank_key = self.box = None
+        self._known, self._pending = 0, 0          # records at the last read of counters[0], upper bound added since
+        self._added = set()
+        self.last = None
+
+    def _reserve(self, bound):
+        """Room for `bound` more records.  Reads the record count (8 bytes) only when the upper bound could overflow."""
+        import torch
+        if self._known + self._pending + bound <= self.pool_cap:
+            self._pending += bound
+            return
+        self._known, self._pending = int(self.counters[0]), 0
+        if self._known + bound > self.pool_cap:
+            cap = max(1 << 20, 2 * self.pool_cap, 8 * bound, self._known + bound)
+            cap = min(cap, 2 ** 31 - 1)
+            if self._known + bound > cap:
+                raise RuntimeError('more than 2^31 - 1 detections')
+            key = torch.empty(cap, dtype=torch.int32, device=self.device)
+            box = torch.empty(cap, 4, dtype=torch.float64, device=self.device)
+            if self._known:
+                key[:self._known].copy_(self.rank_key[:self._known])
+                box[:self._known].copy_(self.box[:self._known])
+            self.rank_key, self.box, self.pool_cap = key, box, cap
+        self._pending = bound
+
+    def add(self, dets, image_indices, sizes):
+        """dets: utils.Detections of one batch after .nms(); image_indices[b]: position in `imagenames` (or the
+        name) of image b; sizes[b] = (width, height)."""
+        import torch
+        n_cls = len(self.classes)
+        if dets.keep is None:
+            raise ValueError('Detections.nms() has not been run')
+        if dets.nC != 1:
+            raise ValueError('rows with %d class scores: only the meta detector (nC = 1) is supported' % dets.nC)
+        if dets.N % n_cls:
+            raise ValueError('%d rows are not images x %d classes' % (dets.N, n_cls))
+        bs = dets.N // n_cls
+        idx = [self.index[i] if isinstance(i, str) else int(i) for i in image_indices]
+        if len(idx) != bs or len(sizes) != bs:
+            raise ValueError('%d images in the batch, %d indices, %d sizes' % (bs, len(idx), len(sizes)))
+        for i in idx:
+            if not 0 <= i < len(self.imagenames):
+                raise IndexError('image index %d outside the image set' % i)
+            if i in self._added:
+                raise ValueError('image %s added twice' % self.imagenames[i])
+            self._added.add(i)
+        if bs == 0:
+            return
+        cap = dets.A * dets.H * dets.W
+        self._reserve(dets.N * cap)
+        idx_t = torch.tensor(idx, dtype=torch.int32).to(self.device)
+        size_t = torch.tensor([[float(w), float(h)] for w, h in sizes], dtype=torch.float64).to(self.device)
+        _call('fsdet_voc_gather', _ptr(dets.cand), _ptr(dets.keep), _ptr(dets.keep_count), dets.N, cap, dets.H, dets.W,
+              dets.nC, n_cls, _ptr(idx_t), _ptr(size_t), _ptr(self.rank_key), _ptr(self.box), self.pool_cap,
+              _ptr(self.groups), self.group_cap, _ptr(self.counters), _stream())
+
+    def result(self, use_07_metric=True, novel_classes=(), curves=False):
+        """The dict mean_ap returns; with curves=True also 'rec' / 'prec': {class: float64 array in rank order}.
+        The device results of the last call stay in `self.last` (flags, order, rec, prec, ... as tensors)."""
+        import torch
+        n_det, n_groups, _, overflow = [int(v) for v in self.counters.cpu()]
+        if overflow:
+            raise RuntimeError('detection pool overflow')
+        n_cls, dev = len(self.classes), self.device
+        ws = torch.empty(max(1, _call_size('fsdet_voc_workspace_bytes', n_det, self.n_gt)), dtype=torch.uint8, device=dev)
+        out = dict(flags=torch.empty(n_det, dtype=torch.uint8, device=dev),
+                   order=torch.empty(n_det, dtype=torch.int32, device=dev),
+                   rec=torch.empty(n_det, dtype=torch.float64, device=dev),
+                   prec=torch.empty(n_det, dtype=torch.float64, device=dev),
+                   cls_count=torch.empty(n_cls, dtype=torch.int32, device=dev),
+                   npos=torch.empty(n_cls, dtype=torch.int32, device=dev),
+                   ap07=torch.empty(n_cls, dtype=torch.float64, device=dev),
+                   ap_area=torch.empty(n_cls, dtype=torch.float64, device=dev))
+        th = np.ascontiguousarray(VOC07_THRESHOLDS, dtype=np.float64)
+        _call('fsdet_voc_evaluate', _ptr(self.rank_key) if n_det else None, _ptr(self.box) if n_det else None, n_det,
+              _ptr(self.groups), n_groups, _ptr(self.gt_ptr), _ptr(self.gt_box) if self.n_gt else None,
+              _ptr(self.gt_difficult) if self.n_gt else None, self.n_gt, n_cls, len(self.imagenames), self.ovthresh,
+              th.ctypes.data, _ptr(ws), ws.numel(), _ptr(out['flags']), _ptr(out['order']), _ptr(out['rec']),
+              _ptr(out['prec']), _ptr(out['cls_count']), _ptr(out['npos']), _ptr(out['ap07']), _ptr(out['ap_area']),
+              _stream())
+        self.last = out
+        ap = (out['ap07'] if use_07_metric else out['ap_area']).cpu().numpy()
+        aps = dict((c, float(ap[i])) for i, c in enumerate(self.classes))
+        r = _ap_summary(self.classes, aps, novel_classes)
+        if curves:
+            cnt = out['cls_count'].cpu().numpy().astype(np.int64)
+            starts = np.concatenate(([0], np.cumsum(cnt)))
+            rec, prec = out['rec'].cpu().numpy(), out['prec'].cpu().numpy()
+            r['rec'] = dict((c, rec[starts[i]:starts[i + 1]]) for i, c in enumerate(self.classes))
+            r['prec'] = dict((c, prec[starts[i]:starts[i + 1]]) for i, c in enumerate(self.classes))
+        return r
+
+
+def _call_size(name, *args):
+    from ._lib import lib
+    return int(getattr(lib, name)(*args))

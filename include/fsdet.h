@@ -371,6 +371,35 @@ int fsdet_nms_boxes64(const double* boxes, const int32_t* count, int N, int cap,
 int fsdet_rw_running_mean(float* enews, const int32_t* cnt_in, int32_t* cnt_out, const float* dw, const int32_t* ids,
                           int n, int n_cls, int C, void* stream);
 
+/* ---- evaluation: PASCAL VOC AP from device-resident detections (voc_eval.py) ---- */
+/* '%f' % x then float() for count doubles: y[i] = the value read back, n[i] (optional) = the integer of the
+ * millionths printed (round half to even on the exact binary value). */
+int fsdet_voc_round6(const double* x, double* y, double* n, long long count, void* stream);
+/* Appends one batch of meta-detector Detections after NMS (rows b*n_cls + i, nC = 1) to an accumulator, in the order
+ * valid.write_detections writes lines: per class, batch, then image, then survivor order.  Every kept box becomes a
+ * record: rank_key[d] = i << 20 | (2^20 - 1 - n), n the '%f' millionths of prob = det*cls; box[d][4] = x1, y1, x2, y2
+ * = ((v0/W) -/+ (v2/W)/2.0) * width ... after the '%f' round trip (float64, reference operation order).  Row r becomes
+ * group counters[1] + r = {first record, count, image_index[b], i}.  image_size float64 [bs][2] = (width, height).
+ * counters int64[4] = {records, groups, first group of the last batch, overflow}: a batch that does not fit pool_cap /
+ * group_cap sets the overflow flag and is dropped, as is every batch after it.  No synchronisation. */
+int fsdet_voc_gather(const float* cand, const int32_t* keep, const int32_t* keep_count, int N, int cap, int H, int W,
+                     int nC, int n_cls, const int32_t* image_index, const double* image_size, uint32_t* rank_key,
+                     double* box, long long pool_cap, int32_t* groups, int group_cap, long long* counters, void* stream);
+size_t fsdet_voc_workspace_bytes(int n_det, int n_gt);
+/* voc_eval.voc_eval for every class at once.  Records as fsdet_voc_gather writes them; groups int32 [n_groups][4]
+ * with distinct (image, class), each a contiguous run of records.  Ground truth: CSR over (class, image),
+ * gt_ptr int32 [n_cls*n_images + 1], gt_box int32 [n_gt][4] (xmin, ymin, xmax, ymax), gt_difficult uint8 [n_gt].
+ * Ranking: per class, a stable sort by confidence descending (ties keep record order).  Matching, rec / prec and the
+ * AP follow voc_eval.match_detections / voc_eval / voc_ap in float64; thresholds = 11 doubles on the host (the VOC07
+ * np.arange(0., 1.1, 0.1)).  Outputs: flags uint8 [n_det] (0 ignored (difficult), 1 TP, 2 FP, record order);
+ * order int32 [n_det] = record at each rank, classes in turn; rec, prec float64 [n_det] in that order; per class
+ * cls_count (records), npos, ap07 (11-point) and ap_area (precision envelope). */
+int fsdet_voc_evaluate(const uint32_t* rank_key, const double* box, int n_det, const int32_t* groups, int n_groups,
+                       const int32_t* gt_ptr, const int32_t* gt_box, const uint8_t* gt_difficult, int n_gt, int n_cls,
+                       int n_images, double ovthresh, const double* thresholds, void* workspace, size_t workspace_bytes,
+                       uint8_t* flags, int32_t* order, double* rec, double* prec, int32_t* cls_count, int32_t* npos,
+                       double* ap07, double* ap_area, void* stream);
+
 /* ---- training-input augmentation (SURVEY.md 8f row 3) ---------------------- */
 /* image.data_augmentation (image.py:52-87: crop with zero fill, PIL resize, horizontal flip, HSV jitter through
  * image.distort_image :19-37) + transforms.ToTensor for n images in one launch pair.

@@ -66,6 +66,35 @@ def make_dataset(root, n, seed=0):
         f.write('bird,bus,cow,motorbike,sofa\naeroplane,bottle,cow,horse,sofa\n')
 
 
+def make_devkit(root, n=4952, year='2007', seed=0):
+    """A VOCdevkit-shaped evaluation set without pixels: <root>/VOC<year>/Annotations/<id>.xml (1-4 objects per
+    image, about 10 % difficult) and ImageSets/Main/test.txt, n images of 500x375 or 375x500 (VOC2007 test has 4952).
+    Returns (image ids, {id: (width, height)})."""
+    rs = np.random.RandomState(seed)
+    voc = os.path.join(root, 'VOC' + year)
+    os.makedirs(os.path.join(voc, 'Annotations'), exist_ok=True)
+    os.makedirs(os.path.join(voc, 'ImageSets', 'Main'), exist_ok=True)
+    names, sizes = [], {}
+    obj = ('<object><name>%s</name><pose>Unspecified</pose><truncated>0</truncated><difficult>%d</difficult>'
+           '<bndbox><xmin>%d</xmin><ymin>%d</ymin><xmax>%d</xmax><ymax>%d</ymax></bndbox></object>')
+    for i in range(n):
+        name = '%06d' % (2 * i + 1)
+        w, h = (500, 375) if i % 3 else (375, 500)
+        objs = []
+        for _ in range(int(rs.randint(1, 5))):
+            bw, bh = int(rs.randint(w // 8, w)), int(rs.randint(h // 8, h))
+            x1, y1 = int(rs.randint(1, w - bw + 1)), int(rs.randint(1, h - bh + 1))
+            objs.append(obj % (VOC[rs.randint(0, 20)], int(rs.rand() < 0.1), x1, y1, x1 + bw - 1, y1 + bh - 1))
+        with open(os.path.join(voc, 'Annotations', name + '.xml'), 'w') as f:
+            f.write('<annotation><filename>%s.jpg</filename><size><width>%d</width><height>%d</height><depth>3</depth>'
+                    '</size>%s</annotation>' % (name, w, h, ''.join(objs)))
+        names.append(name)
+        sizes[name] = (w, h)
+    with open(os.path.join(voc, 'ImageSets', 'Main', 'test.txt'), 'w') as f:
+        f.write('\n'.join(names) + '\n')
+    return names, sizes
+
+
 def main():
     n = int(sys.argv[1]) if len(sys.argv) > 1 else 512
     epochs = int(sys.argv[2]) if len(sys.argv) > 2 else 3

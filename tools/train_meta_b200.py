@@ -9,8 +9,9 @@ The `.data` file drives everything as in the reference: `train` (image list or c
 from lists.build_dataset, the support index from lists.support_index, the step from trainer.MetaTrainer (CUDA-graph
 replay, one graph per multi-scale input size).  Under torchrun every rank builds the same lists with the same seeds,
 takes its slice of each global batch, and rank 0's parameters are broadcast once before the first step.
-What the reference's script does beyond that - the in-training test() pass - is not wired here;
-`fewshot_detection_b200.evaluate` / `valid` / `voc_eval` are the evaluation entry points.
+What the reference's script does beyond that - the in-training test() pass - is not wired here; a trained weight file
+is scored by tools/valid_ensemble_b200.py (valid_ensemble.py + scripts/voc_eval.py), built on
+`fewshot_detection_b200.evaluate` / `valid` / `voc_eval`.
 """
 import os
 import sys

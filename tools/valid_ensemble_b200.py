@@ -1,0 +1,127 @@
+#!/usr/bin/env python
+"""Evaluation command: the reference README's two evaluation steps (valid_ensemble.py, then scripts/voc_eval.py) in
+one run, with the detections scored on the GPU where decode and NMS leave them.
+
+    python tools/valid_ensemble_b200.py datacfg darknetcfg learnetcfg weightfile [--devkit DIR] [--write-results]
+
+The `.data` file is read as tools/train_meta_b200.py reads it: `valid` (image list), `meta` (support dictionary), the
+class list and the `novel` / `novelid` split.  The support images of every class are run through the reweighting net
+and averaged per class (valid_ensemble.py:86-100); every image of `valid` is detected with those vectors
+(conf_thresh 0.005, NMS 0.45).  Image ids are file basenames and sizes come from the image headers, as in the
+reference.
+
+--devkit DIR       DIR/VOC<year>/Annotations/<id>.xml and DIR/VOC<year>/ImageSets/Main/test.txt (annotations cached
+                   in DIR/annotations_cache as scripts/voc_eval.py does): prints the AP per class and the mean, base
+                   and novel mean AP (VOC07 11-point metric for years before 2010, as the reference).
+--write-results    writes the reference's result files results/<backup>/ene<ckpt>/comp4_det_test_<class>.txt.
+
+Ranking differs from the reference's file-based evaluation only for detections whose printed confidences tie: they
+keep result-file order here (voc_eval.DeviceVocEval).
+"""
+import argparse
+import os
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def read_list(path):
+    with open(path, 'r') as f:
+        return [l.rstrip() for l in f.readlines() if l.strip()]
+
+
+def result_prefix(weightfile):
+    """valid_ensemble.py:15-21: results/<directory of the weight file>/ene<weight file stem>."""
+    ckpt = os.path.basename(weightfile).split('.')[0]
+    backup = os.path.basename(os.path.dirname(os.path.abspath(weightfile)))
+    return os.path.join('results', backup, 'ene' + ckpt)
+
+
+def main(argv=None):
+    ap = argparse.ArgumentParser(description=__doc__.split('\n')[0])
+    ap.add_argument('datacfg')
+    ap.add_argument('darknetcfg')
+    ap.add_argument('learnetcfg')
+    ap.add_argument('weightfile')
+    ap.add_argument('--devkit', default=None, help='VOCdevkit directory: score the detections against its annotations')
+    ap.add_argument('--year', default='2007')
+    ap.add_argument('--write-results', action='store_true', help='write the per-class result files')
+    ap.add_argument('--batch-size', type=int, default=64, help='query images per forward')
+    ap.add_argument('--support-batch', type=int, default=64, help='support images per reweighting-net forward')
+    args = ap.parse_args(argv)
+    if args.devkit is None and not args.write_results:
+        ap.error('nothing to do: give --devkit and/or --write-results')
+
+    import torch
+    from fewshot_detection_b200.cfg import cfg, parse_cfg
+    from fewshot_detection_b200.utils import read_data_cfg, logging
+    from fewshot_detection_b200.darknet_meta import Darknet
+    from fewshot_detection_b200.dataset import DetectionBatcher, MetaBatcher
+    from fewshot_detection_b200 import lists as LS, valid as VA, voc_eval as VE
+
+    torch.cuda.set_device(0)
+    data_options = read_data_cfg(args.datacfg)
+    darknetcfg, learnetcfg = parse_cfg(args.darknetcfg), parse_cfg(args.learnetcfg)
+    cfg.config_data(data_options)
+    cfg.config_meta(learnetcfg[0])
+    cfg.config_net(darknetcfg[0])
+    classes = list(cfg.classes)
+    novel = list(cfg.novel_classes)
+
+    m = Darknet(darknetcfg, learnetcfg)
+    m.load_weights(args.weightfile)
+    m = m.cuda().eval()
+
+    metalines, inds = LS.support_index(data_options['meta'], classes, 0, ensemble=True)
+    mb = MetaBatcher(metalines, inds, classes=classes, train=False, ensemble=True, with_ids=True)
+    meta_batches = (mb.batch(range(s, min(s + args.support_batch, len(inds)))) for s in range(0, len(inds), args.support_batch))
+
+    lines = read_list(data_options['valid'])
+    db = DetectionBatcher(lines, shape=(m.width, m.height), shuffle=False, train=False, batch_size=args.batch_size)
+    imgids = [os.path.basename(l).split('.')[0] for l in lines]
+
+    def image_batches():
+        for s in range(0, len(lines), args.batch_size):
+            idx = range(s, min(s + args.batch_size, len(lines)))
+            data, _ = db.batch(idx)
+            yield data, [imgids[i] for i in idx], [db._entry(i).size() for i in idx]
+
+    fps = None
+    if args.write_results:
+        prefix = result_prefix(args.weightfile)
+        if not os.path.exists(prefix):
+            os.makedirs(prefix)
+        logging('saving to: %s' % prefix)
+        fps = [open(os.path.join(prefix, 'comp4_det_test_%s.txt' % c), 'w') for c in classes]
+    try:
+        if args.devkit is None:
+            n_cls = len(classes)
+            dw = VA.ensemble_dynamic_weights(m, meta_batches, n_cls)
+            for data, ids, sizes in image_batches():
+                VA.write_detections(fps, VA.detect(m, data, dw, n_cls), ids, sizes, n_cls)
+            return 0
+        voc = os.path.join(args.devkit, 'VOC' + args.year)
+        imagenames = read_list(os.path.join(voc, 'ImageSets', 'Main', 'test.txt'))
+        recs = VE.load_annotations(os.path.join(voc, 'Annotations', '{}.xml'), imagenames,
+                                   os.path.join(args.devkit, 'annotations_cache'))
+        use_07 = int(args.year) < 2010
+        ev = VE.DeviceVocEval(classes, imagenames, recs)
+        r = VA.valid_batches_ap(m, meta_batches, image_batches(), ev, use_07, novel_classes=novel, fps=fps)
+    finally:
+        if fps is not None:
+            for f in fps:
+                f.close()
+    print('VOC07 metric? ' + ('Yes' if use_07 else 'No'))
+    for c in classes:
+        print('AP for {} = {:.4f}{}'.format(c, r['ap'][c], ' (novel)' if c in novel else ''))
+    print('Mean AP = {:.4f}'.format(r['mean']))
+    if r['mean_base'] is not None and novel:
+        print('Mean Base AP = {:.4f}'.format(r['mean_base']))
+    if r['mean_novel'] is not None:
+        print('Mean Novel AP = {:.4f}'.format(r['mean_novel']))
+    return 0
+
+
+if __name__ == '__main__':
+    sys.exit(main())
