@@ -32,13 +32,6 @@ SIGNATURES = {
     'fsdet_conv_first_fwd_stats': ('pipippiiiiipp', 'i'),
     'fsdet_conv_first_wgrad': ('pipipippziiiip', 'i'),
     'fsdet_conv_first_wgrad_workspace_floats': ('iiii', 'z'),
-    'fsdet_conv_first_tc_supported': ('iii', 'i'),
-    'fsdet_conv_first_tc_rows': ('iii', 'i'),
-    'fsdet_conv_first_tc_stats': ('pipipppiiiip', 'i'),
-    'fsdet_conv_first_tc_apply': ('pipipp pp f pi pp i p iiii p'.replace(' ', ''), 'i'),
-    'fsdet_conv_first_tc_bwd_reduce': ('pipipp pppp f pi p iiii p'.replace(' ', ''), 'i'),
-    'fsdet_conv_first_tc_wgrad_workspace_floats': ('iii', 'z'),
-    'fsdet_conv_first_tc_bwd_wgrad': ('pipipp pppp p f pi p p pz iiii p'.replace(' ', ''), 'i'),
     'fsdet_weight_flip_transpose': ('ppiiip', 'i'),
     'fsdet_pad_channels': ('pipizp', 'i'),
     'fsdet_conv_tc_supported': ('iii', 'i'),
@@ -50,7 +43,6 @@ SIGNATURES = {
     'fsdet_conv_tc_wgrad': ('ppppppppziiiiiiip', 'i'),
     'fsdet_weight_prep': ('ppipip', 'i'),
     'fsdet_amax': ('piizpp', 'i'),
-    'fsdet_amax_acc': ('piizpp', 'i'),
     'fsdet_split_f16': ('piiizpppp', 'i'),
     'fsdet_colstats': ('pizipp', 'i'),
     'fsdet_colstats_rows': ('z', 'i'),

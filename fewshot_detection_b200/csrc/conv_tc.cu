@@ -482,17 +482,6 @@ extern "C" int fsdet_amax(const float* src, int ld, int C, size_t rows, float* a
     return launch_status("amax");
 }
 
-extern "C" int fsdet_amax_acc(const float* src, int ld, int C, size_t rows, float* amax_inout, void* stream) {
-    FSDET_CHECK_ARG(src && amax_inout && C % 4 == 0 && ld % 4 == 0 && ld >= C && aligned16(src), "amax_acc: C=%d ld=%d", C, ld);
-    long long n = (long long)rows * (C / 4);
-    if (n == 0) return 0;
-    FSDET_CHECK_ARG(n < (1ll << 31), "amax_acc: tensor too large for 32-bit indexing");
-    int blocks = ceil_div(n, 256 * 8);
-    if (blocks > 4 * kNumSMs) blocks = 4 * kNumSMs;
-    amax_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(src, ld, C / 4, (long long)rows, amax_inout);
-    return launch_status("amax_acc");
-}
-
 extern "C" int fsdet_split_f16(const float* src, int ld, int C, int Cpad, size_t rows, const float* amax, void* hi, void* lo,
                                void* stream) {
     FSDET_CHECK_ARG(src && hi && lo && C % 4 == 0 && ld % 4 == 0 && ld >= C && Cpad >= C && Cpad % 4 == 0,

@@ -1,5 +1,5 @@
-// PTX wrappers of the wgmma / TMA / mbarrier instructions used by the tensor-core kernels (conv_tc.cu,
-// conv_first_tc.cu).  Device code only; included inside namespace fsdet.  The host-emulation builds
+// PTX wrappers of the wgmma / TMA / mbarrier instructions used by the tensor-core kernels (conv_tc.cu).
+// Device code only; included inside namespace fsdet.  The host-emulation builds
 // (tools/host_emul/*_emul.cpp) provide functional models with the same names instead of this file.
 #pragma once
 
@@ -38,7 +38,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // the same wait executed by a whole converged warp (the issuing roles, see elect_one below)
 __device__ __forceinline__ void mbar_wait_warp(uint64_t* bar, uint32_t parity) { mbar_wait(bar, parity); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void tma_load_im2col_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c, int w, int h,
                                                    int n, uint16_t off_w, uint16_t off_h) {
     asm volatile(

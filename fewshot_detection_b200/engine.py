@@ -19,8 +19,6 @@ import os
 
 # tensor-core (wgmma) convolution path for layers with Cin % 64 == 0; FSDET_TC=0 selects the exact-fp32 SIMT kernels
 USE_TC = os.environ.get('FSDET_TC', '1') != '0'
-# 'first' = the recomputing first-block kernels (csrc/conv_first_tc.cuh): correct but slower than the store-z path they were
-# meant to replace (instruction-bound epilogues, DESIGN.md section 3) - opt-in only
 TC_PARTS = set(os.environ.get('FSDET_TC_PARTS', 'fwd,dgrad,wgrad,head').split(','))  # debugging: which GEMMs may use it
 
 
@@ -646,9 +644,6 @@ class NetRunner(object):
         else:
             wuse = w
         cout_p = _round_up(s.cout, 4)
-        if (bn is not None and x.nchw is not None and s.fuse_pool and not s.keep_full and USE_TC and 'first' in TC_PARTS
-                and cin_p == 4 and s.k == 3 and _lib.lib.fsdet_conv_first_tc_supported(H, W, s.cout)):
-            return self._first_tc_fwd(s, x, wuse, conv, bn, training, out_act, st)
         if bn is not None:
             assert cout_p == s.cout, 'BatchNorm conv with Cout % 4 != 0 is unsupported'
             z = Act.new(B, H, W, s.cout, dev)
@@ -742,93 +737,6 @@ class NetRunner(object):
         rec = ('convbias', s, x, wp, z, (ones, zeros), full, pooled, conv, cout_p)
         return ((full, pooled) if s.fuse_pool else full), rec
 
-    # -- first block without its pre-BN tensor (csrc/conv_first_tc.cuh) ------------------------------------------
-    def _first_tc_fwd(self, s, x, w4, conv, bn, training, out_act, st):
-        """conv 3x3 from the NCHW images + BatchNorm + LeakyReLU + max-pool in two recomputing passes: the layer's
-        pre-BN output (the largest tensor of the network) is never written; backward recomputes it too."""
-        dev = x.dev
-        B, H, W = x.B, x.H, x.W
-        in0, c0, in1, c1 = x.nchw
-        npix = x.npix
-        amax_x = torch.empty(1, dtype=torch.float32, device=dev)
-        call('fsdet_amax', ptr(in0), W, W, in0.numel() // W, ptr(amax_x), st)
-        if in1 is not None:
-            call('fsdet_amax_acc', ptr(in1), W, W, in1.numel() // W, ptr(amax_x), st)
-        use_batch_stats = training or not bn.track_running_stats
-        rows = _lib.lib.fsdet_conv_first_tc_rows(B, H, W)
-        stat = None
-        if use_batch_stats:
-            stat = _empty(rows + _lib.lib.fsdet_bn_stat_scratch_rows(), 4 * s.cout, device=dev)
-            self._timed('first_tc', 2.0 * npix * s.cout * 36, 'fsdet_conv_first_tc_stats', ptr(in0), c0, ptr(in1), c1, ptr(w4),
-                        ptr(amax_x), ptr(stat), B, H, W, s.cout, st)
-        vec = _empty(5, s.cout, device=dev)
-        vec.xh_ok = bool(use_batch_stats)
-        amax_y = _empty(1, device=dev) if use_batch_stats else None
-        upd = training and bn.track_running_stats
-        call('fsdet_bn_finalize', ptr(stat), rows, float(npix), ptr(bn.weight), ptr(bn.bias),
-             ptr(bn.running_mean) if (upd or not use_batch_stats) else None,
-             ptr(bn.running_var) if (upd or not use_batch_stats) else None,
-             BN_MOMENTUM if bn.momentum is None else float(bn.momentum), float(bn.eps),
-             ptr(vec[0]), ptr(vec[1]), ptr(vec[2]), ptr(vec[3]), s.slope, ptr(amax_y), ptr(vec[4]), s.cout,
-             1 if use_batch_stats else 0, st)
-        if upd and bn.num_batches_tracked is not None:
-            bn.num_batches_tracked += 1
-        pos = self.specs.index(s)
-        Hp, Wp = H // 2, W // 2
-        cp64 = _round_up(s.cout, 64)
-        planes_ok = (amax_y is not None and (s.idx + 1) not in self.placement and (s.idx + 1) not in self.routed
-                     and self._consumer_takes_planes(pos + 2, s.cout))
-        ppl = None
-        if planes_ok:
-            ppl = (torch.empty(B * Hp * Wp, cp64, dtype=torch.float16, device=dev),
-                   torch.empty(B * Hp * Wp, cp64, dtype=torch.float16, device=dev), amax_y)
-            pooled = Act.planes_only(B, Hp, Wp, s.cout, dev, ppl)
-        else:
-            pooled = out_act(s.idx + 1, B, Hp, Wp, s.cout)
-            pooled.amax = amax_y
-        p32 = pooled if pooled.buf is not None else None
-        self._timed('first_tc', 2.0 * npix * s.cout * 36, 'fsdet_conv_first_tc_apply', ptr(in0), c0, ptr(in1), c1, ptr(w4),
-                    ptr(amax_x), ptr(vec[2]), ptr(vec[3]), s.slope, p32.ptr if p32 else None, p32.ld if p32 else 0,
-                    ptr(ppl[0]) if ppl else None, ptr(ppl[1]) if ppl else None, cp64 if ppl else 0, ptr(amax_y) if ppl else None,
-                    B, H, W, s.cout, st)
-        rec = ('first_tc', s, x, w4, vec, pooled, conv, bn, amax_x)
-        return (None, pooled), rec
-
-    def _first_tc_bwd(self, rec, st):
-        _, s, x, w4, vec, pooled, conv, bn, amax_x = rec
-        dev = x.dev
-        B, H, W = x.B, x.H, x.W
-        in0, c0, in1, c1 = x.nchw
-        gp = pooled.grad_for_read()
-        gw, fin_w = self._param_grad(conv.weight)
-        gg, fin_g = self._param_grad(bn.weight)
-        gb, fin_b = self._param_grad(bn.bias)
-        if gp is None:
-            for t in (gw, gg, gb):
-                t.zero_()
-        else:
-            rows = _lib.lib.fsdet_conv_first_tc_rows(B, H, W)
-            part = _empty(rows + 1, 3 * s.cout, dtype=torch.float64, device=dev)
-            coef = _empty(2, s.cout, dtype=torch.float64, device=dev)
-            flops = 2.0 * x.npix * s.cout * 36
-            self._timed('first_tc', flops, 'fsdet_conv_first_tc_bwd_reduce', ptr(in0), c0, ptr(in1), c1, ptr(w4), ptr(amax_x),
-                        ptr(vec[2]), ptr(vec[3]), ptr(vec[0]), ptr(vec[1]), s.slope, gp.ptr, gp.ld, ptr(part), B, H, W, s.cout, st)
-            amax_dz = _empty(1, device=dev)
-            call('fsdet_bn_bwd_finalize', ptr(part), rows, float(x.npix), ptr(bn.weight), ptr(vec[1]), ptr(vec[4]), ptr(gg), ptr(gb),
-                 ptr(coef), ptr(amax_dz), s.cout, 1, st)
-            nws = _lib.lib.fsdet_conv_first_tc_wgrad_workspace_floats(B, H, W)
-            ws = _empty(max(nws, 4), device=dev)
-            gw4 = gw if s.cin == 4 else _empty(s.cout, 9, 4, device=dev)
-            self._timed('first_tc', 2 * flops, 'fsdet_conv_first_tc_bwd_wgrad', ptr(in0), c0, ptr(in1), c1, ptr(w4), ptr(amax_x),
-                        ptr(vec[2]), ptr(vec[3]), ptr(vec[0]), ptr(vec[1]), ptr(coef), s.slope, gp.ptr, gp.ld, ptr(amax_dz),
-                        ptr(gw4), ptr(ws), nws, B, H, W, s.cout, st)
-            if s.cin != 4:
-                call('fsdet_pad_channels', ptr(gw4), 4, ptr(gw), s.cin, s.cout * 9, st)
-        for f in (fin_w, fin_g, fin_b):
-            if f:
-                f()
-        self._done(conv.weight, bn.weight, bn.bias)
-
     def _head_fwd(self, s, head, x, rw, st):
         """dynamic_conv.DynamicConv2d.forward (dynamic_conv.py:125-164) + the
         following nn.Conv2d(K, O, 1): out[b*n_cls+c] = (W (.) rw[c]) x[b] + bias."""
@@ -896,8 +804,6 @@ class NetRunner(object):
                     call('fsdet_copy_channels', tgt.ptr, tgt.ld, g.ptr, g.ld, x.npix, x.C, 1, st)
             elif kind == 'convbn':
                 self._convbn_bwd(rec, st)
-            elif kind == 'first_tc':
-                self._first_tc_bwd(rec, st)
             elif kind == 'convbias':
                 self._convbias_bwd(rec, st)
             elif kind == 'maxpool':

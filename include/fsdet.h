@@ -89,33 +89,6 @@ int fsdet_conv_first_fwd_stats(const float* in0, int C0, const float* in1, int C
 int fsdet_conv_first_wgrad(const float* in0, int C0, const float* in1, int C1, const float* dz, int lddz, float* dw,
                            float* workspace, size_t workspace_floats, int B, int H, int W, int Cout, void* stream);
 size_t fsdet_conv_first_wgrad_workspace_floats(int B, int H, int W, int Cout);
-/* The same first block (conv 3x3 from <= 4 NCHW input channels into Cout <= 32 + train-mode BatchNorm + LeakyReLU +
- * MaxPool 2/2) WITHOUT storing its pre-BN output: every pass recomputes it from the input images with a wgmma GEMM
- * per 128-pixel tile (csrc/conv_first_tc.cuh).  Needs H % 8 == 0, W % 16 == 0 (fsdet_conv_first_tc_supported).
- * amax_x: device scalar >= max |input| (fsdet_amax over the input tensors).  w_pad4 as above.
- *   _stats      -> BatchNorm partial rows float [fsdet_conv_first_tc_rows(B,H,W)][4*Cout] for fsdet_bn_finalize
- *   _apply      -> leaky(z*scale+shift) max-pooled, as fp32 [B*(H/2)*(W/2)][ld_pool] and / or scaled fp16 hi/lo planes
- *                  [..][cpad] (cpad % 32 == 0, padding channels zero filled; amax_y from fsdet_bn_finalize)
- *   _bwd_reduce -> double [rows][3*Cout] = (sum du | sum du*xhat | max |du|) for fsdet_bn_bwd_finalize, du = dy_pool
- *                  routed to the first arg-max of each window (torch max_pool2d) times leaky'
- *   _bwd_wgrad  -> dw [Cout][9][4]: dz = scale*(du - c1 - xhat*c2) (coef = (c1 | c2) from fsdet_bn_bwd_finalize) is
- *                  formed tile by tile in shared memory and contracted with the im2col tile by a second GEMM; amax_dz
- *                  = the bound fsdet_bn_bwd_finalize writes; workspace float [fsdet_conv_first_tc_wgrad_workspace_floats] */
-int fsdet_conv_first_tc_supported(int H, int W, int Cout);
-int fsdet_conv_first_tc_rows(int B, int H, int W);
-int fsdet_conv_first_tc_stats(const float* in0, int C0, const float* in1, int C1, const float* w_pad4, const float* amax_x,
-                              float* stat_partial, int B, int H, int W, int Cout, void* stream);
-int fsdet_conv_first_tc_apply(const float* in0, int C0, const float* in1, int C1, const float* w_pad4, const float* amax_x,
-                              const float* scale, const float* shift, float slope, float* y_pool, int ld_pool, void* pool_hi,
-                              void* pool_lo, int cpad, const float* amax_y, int B, int H, int W, int Cout, void* stream);
-int fsdet_conv_first_tc_bwd_reduce(const float* in0, int C0, const float* in1, int C1, const float* w_pad4, const float* amax_x,
-                                   const float* scale, const float* shift, const float* mean, const float* invstd, float slope,
-                                   const float* dy_pool, int ld_dyp, double* partial, int B, int H, int W, int Cout, void* stream);
-size_t fsdet_conv_first_tc_wgrad_workspace_floats(int B, int H, int W);
-int fsdet_conv_first_tc_bwd_wgrad(const float* in0, int C0, const float* in1, int C1, const float* w_pad4, const float* amax_x,
-                                  const float* scale, const float* shift, const float* mean, const float* invstd,
-                                  const double* coef, float slope, const float* dy_pool, int ld_dyp, const float* amax_dz, float* dw,
-                                  float* workspace, size_t workspace_floats, int B, int H, int W, int Cout, void* stream);
 /* wt[ci][kk-1-tap][co] = w[co][tap][ci]  (weights for the input-gradient conv) */
 int fsdet_weight_flip_transpose(const float* w, float* wt, int Cout, int kk, int Cin, void* stream);
 /* copy [rows][cin] -> [rows][cout] channel-padded / -cropped (zero fill) */
@@ -191,8 +164,6 @@ int fsdet_weight_prep(const fsdet_weight_desc* descs_dev, const int32_t* tiles_d
                       int n_layers, void* stream);
 /* absolute maximum of fp32 [rows][ld] (first C columns) -> *amax_out (device float) */
 int fsdet_amax(const float* src, int ld, int C, size_t rows, float* amax_out, void* stream);
-/* the same without resetting the destination first: *amax_inout = max(*amax_inout, max |src|) */
-int fsdet_amax_acc(const float* src, int ld, int C, size_t rows, float* amax_inout, void* stream);
 /* fp32 [rows][ld] (first C columns) -> two dense fp16 planes [rows][Cpad] of the
  * tensor scaled as described above (amax NULL: no scaling); columns C..Cpad-1
  * are zero (lets 32-channel layers use the 64-channel K tiles) */

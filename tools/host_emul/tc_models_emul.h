@@ -95,7 +95,6 @@ static inline void mbar_wait_warp(uint64_t* bar, uint32_t parity) {
     __syncwarp();
 }
 static inline void fence_barrier_init() {}
-static inline void fence_proxy_async() {}
 static inline void tma_prefetch_desc(const CUtensorMap*) {}
 
 #include "wgmma_emul.h"
