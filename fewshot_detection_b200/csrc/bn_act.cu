@@ -14,6 +14,13 @@
 
 #include "common.cuh"
 
+// tools/host_emul compiles this file with g++ (threads = OS threads) to test the kernels without a GPU
+#ifdef FSDET_HOST_EMULATION
+#define FSDET_DYN_SMEM_F64(name) double* name = reinterpret_cast<double*>(emul::g_dyn_smem)
+#else
+#define FSDET_DYN_SMEM_F64(name) extern __shared__ double name[]
+#endif
+
 namespace fsdet {
 
 // power-of-two scale that maps a tensor with absolute maximum `a` into [512, 1024)  (same rule as conv_tc.cu)
@@ -439,7 +446,7 @@ __global__ void __launch_bounds__(256, 3) bn_act_bwd_kernel(const BwdArgs a) {
 
     if (!APPLY) {
         // reduce over threadIdx.y -> one partial row per blockIdx.x
-        extern __shared__ double red[];  // [blockDim.y][TC*16]
+        FSDET_DYN_SMEM_F64(red);  // [blockDim.y][TC*16]
         double* mine = red + ((size_t)threadIdx.y * TC + threadIdx.x) * 16;
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
@@ -556,7 +563,7 @@ __global__ void __launch_bounds__(256, 3) bn_act_bwd_pool_kernel(const BwdArgs a
     }
 
     if (!APPLY) {
-        extern __shared__ double red[];  // [blockDim.y][TC*16]
+        FSDET_DYN_SMEM_F64(red);  // [blockDim.y][TC*16]
         double* mine = red + ((size_t)threadIdx.y * TC + threadIdx.x) * 16;
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
@@ -603,7 +610,24 @@ static int bwd_rows(int B, int H, int W) {
     return (int)r;
 }
 
+// channel-vector lanes TC of the pooled forward and the backward blocks (TC x 256/TC threads), sized by the real
+// channels C
+static int chan_lanes(int C) {
+    const int C4 = C / 4;
+    return C4 >= 32 ? 32 : (C4 >= 16 ? 16 : (C4 >= 8 ? 8 : (C4 >= 4 ? 4 : (C4 >= 2 ? 2 : 1))));
+}
+
+// stage-1 split of bn_finalize: S blocks of rps conv partial rows each (S <= kBnSplits)
+static void stat_split(int nparts, int* S, int* rps) {
+    int s = ceil_div(nparts, 64);
+    if (s > kBnSplits) s = kBnSplits;
+    *rps = ceil_div(nparts, s);
+    *S = ceil_div(nparts, *rps);
+}
+
 }  // namespace fsdet
+
+#ifndef FSDET_HOST_EMULATION  // tools/host_emul/bn_act_emul.cpp launches the kernels above on the same geometry
 
 using namespace fsdet;
 
@@ -628,10 +652,8 @@ extern "C" int fsdet_bn_finalize(const float* stat_partial, int nparts, double c
     int S = 0;
     if (training) {
         // scratch for the stage-1 result lives behind the partial rows (fsdet_bn_stat_scratch_rows() extra rows)
-        S = ceil_div(nparts, 64);
-        if (S > kBnSplits) S = kBnSplits;
-        const int rps = ceil_div(nparts, S);
-        S = ceil_div(nparts, rps);
+        int rps;
+        stat_split(nparts, &S, &rps);
         double* scratch = reinterpret_cast<double*>(const_cast<float*>(stat_partial) + (size_t)nparts * 4 * C);
         dim3 block(32, 32), grid(ceil_div(C, 32), S);
         bn_stats_reduce_kernel<<<grid, block, 0, s>>>(stat_partial, nparts, rps, C, scratch, amax_y);
@@ -671,8 +693,7 @@ extern "C" int fsdet_bn_act_fwd(const float* z, int ldz, const float* scale, con
         if (nwin == 0) return 0;
         // channel-vector lanes sized by the REAL channels: the zero padding of the planes (pitch > C) is written by the
         // same threads in a second trip of their channel loop instead of by threads that never load anything
-        const int C4 = C / 4;
-        const int TC = C4 >= 32 ? 32 : (C4 >= 16 ? 16 : (C4 >= 8 ? 8 : (C4 >= 4 ? 4 : (C4 >= 2 ? 2 : 1))));
+        const int TC = chan_lanes(C);
         const int TY = 256 / TC;
         dim3 block(TC, TY), grid((unsigned)ceil_div(nwin, TY));
         if (a.yf || a.fh) bn_act_pool_kernel<true><<<grid, block, 0, s>>>(a);
@@ -684,7 +705,7 @@ extern "C" int fsdet_bn_act_fwd(const float* z, int ldz, const float* scale, con
 static int launch_bwd(bool apply, const BwdArgs& a, cudaStream_t s) {
     FSDET_CHECK_ARG((long long)a.B * a.H * a.W < (1ll << 31), "bn_act_bwd: tensor too large for 32-bit pixel indexing");
     int C4 = a.C / 4;
-    int TC = C4 >= 32 ? 32 : (C4 >= 16 ? 16 : (C4 >= 8 ? 8 : (C4 >= 4 ? 4 : (C4 >= 2 ? 2 : 1))));
+    int TC = chan_lanes(a.C);
     int TY = 256 / TC;
     dim3 block(TC, TY), grid(bwd_rows(a.B, a.H, a.W), ceil_div(C4, TC));
     const size_t smem = (size_t)TY * TC * 16 * sizeof(double);  // 32 KB (reduce pass)
@@ -746,3 +767,5 @@ extern "C" int fsdet_bn_act_bwd_apply(const float* z, int ldz, const float* dy_f
     a.B = B; a.H = H; a.W = W; a.C = C; a.slope = slope; a.has_bn = has_bn;
     return launch_bwd(true, a, (cudaStream_t)stream);
 }
+
+#endif  // FSDET_HOST_EMULATION
