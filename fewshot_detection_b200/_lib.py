@@ -78,7 +78,10 @@ SIGNATURES = {
     'fsdet_voc_gather': ('pppiiiiiippppqpipp', 'i'),
     'fsdet_voc_workspace_bytes': ('ii', 'z'),
     'fsdet_voc_evaluate': ('ppipipppiiidppzppppppppp', 'i'),
-    'fsdet_augment_workspace_bytes': ('iiii', 'z'),
+    'fsdet_coco_gather': ('pppiiiiiippippqpipp', 'i'),
+    'fsdet_coco_workspace_bytes': ('iiii', 'z'),
+    'fsdet_coco_evaluate': ('ppipippppiiippppp z pppp p'.replace(' ', ''), 'i'),
+    'fsdet_augment_workspace_bytes':('iiii', 'z'),
     'fsdet_augment_batch': ('pppiiiiipzpppp', 'i'),
     'fsdet_box_masks': ('piiipp', 'i'),
 }

@@ -152,3 +152,25 @@ def valid_batches_ap(m, meta_batches, image_batches, evaluator, use_07_metric=Tr
         if fps is not None:
             write_detections(fps, dets, imgids, sizes, n_cls)
     return evaluator.result(use_07_metric, novel_classes)
+
+
+def valid_batches_coco(m, meta_batches, image_batches, evaluator, novel_classes=(), results_fp=None):
+    """valid_batches scored with the COCO box metric on the device: `evaluator` is a coco_eval.DeviceCocoEval over the
+    evaluated image set, `image_batches` yields (data, imgids, sizes) with imgids names of that set.  Returns
+    coco_eval.coco_evaluate's dict.  results_fp (optional, an open text file) also receives the standard results json
+    of the same detections (copied to the host for it)."""
+    from . import coco_eval
+    n_cls = len(evaluator.classes)
+    m.eval()
+    dynamic_weights = ensemble_dynamic_weights(m, meta_batches, n_cls)
+    dev = next(m.parameters()).device
+    records = []
+    for data, imgids, sizes in image_batches:
+        dets = detect(m, data.to(dev), dynamic_weights, n_cls)
+        evaluator.add(dets, imgids, sizes)
+        if results_fp is not None:
+            records.extend(coco_eval.detection_records(dets, imgids, sizes, n_cls, evaluator.max_det))
+    if results_fp is not None:
+        ids = dict((n, i) for n, i in zip(evaluator.imagenames, evaluator.image_ids))
+        coco_eval.write_coco_results(results_fp, records, ids, evaluator.category_ids)
+    return evaluator.result(novel_classes)

@@ -371,6 +371,30 @@ int fsdet_voc_evaluate(const uint32_t* rank_key, const double* box, int n_det, c
                        uint8_t* flags, int32_t* order, double* rec, double* prec, int32_t* cls_count, int32_t* npos,
                        double* ap07, double* ap_area, void* stream);
 
+/* ---- COCO box AP / AR from device-resident detections (csrc/coco_eval.cu) -- */
+/* pycocotools COCOeval (bbox, useCats=1) as coco_eval.py defines it, bit for bit in float64.  The caller owns every
+ * buffer; nothing synchronises and nothing is copied to the host.
+ * fsdet_coco_gather: one batch of Detections after NMS -> per row its first max_det survivors by a stable sort on
+ *   score = det_conf * cls_conf (descending), appended as score[] and box[][4] = (x, y, w, h) of the unclipped
+ *   result-line corners, plus one group {first, count, image, class} per row.  counters (int64 [4]): records, groups,
+ *   first group of the last batch, overflow flag (a batch that does not fit is dropped, and so is everything after).
+ * fsdet_coco_evaluate: groups as the gather writes them (each (image, class) once, records in rank order, the groups
+ *   tiling records [0, n_det)); ground truth as CSR over (class, image): gt_ptr [n_cls*n_images + 1], gt_box [n][4]
+ *   (x, y, w, h), gt_area [n] (the json `area`), gt_crowd [n].  Params: iou_thrs [10], rec_thrs [101], max_dets [3],
+ *   area_rng [4][2].  Writes dt_flags [4][n_det] (TP bits 0-9 | FP bits 16-25 per area range), order [n_det] (records
+ *   ranked by class, then score descending, image and rank), precision [10][101][n_cls][4][3] and recall
+ *   [10][n_cls][4][3] in pycocotools' layout, -1 where undefined. */
+int fsdet_coco_gather(const float* cand, const int32_t* keep, const int32_t* keep_count, int N, int cap, int H, int W,
+                      int nC, int n_cls, const int32_t* image_index, const double* image_size, int max_det,
+                      double* score, double* box, long long pool_cap, int32_t* groups, int group_cap,
+                      long long* counters, void* stream);
+size_t fsdet_coco_workspace_bytes(int n_det, int n_gt, int n_cls, int n_images);
+int fsdet_coco_evaluate(const double* score, const double* box, int n_det, const int32_t* groups, int n_groups,
+                        const int32_t* gt_ptr, const double* gt_box, const double* gt_area, const uint8_t* gt_crowd,
+                        int n_gt, int n_cls, int n_images, const double* iou_thrs, const double* rec_thrs,
+                        const int32_t* max_dets, const double* area_rng, void* workspace, size_t workspace_bytes,
+                        uint32_t* dt_flags, int32_t* order, double* precision, double* recall, void* stream);
+
 /* ---- training-input augmentation (SURVEY.md 8f row 3) ---------------------- */
 /* image.data_augmentation (image.py:52-87: crop with zero fill, PIL resize, horizontal flip, HSV jitter through
  * image.distort_image :19-37) + transforms.ToTensor for n images in one launch pair.

@@ -78,6 +78,14 @@ static inline int atomicMax(int* p, int v) {   // CAS loop
     }
     return old;
 }
+static inline unsigned long long atomicMax(unsigned long long* p, unsigned long long v) {
+    unsigned long long old = __atomic_load_n(p, __ATOMIC_SEQ_CST);
+    while (old < v && !__atomic_compare_exchange_n(p, &old, v, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST)) {
+    }
+    return old;
+}
+static inline long long __double_as_longlong(double d) { long long v; memcpy(&v, &d, 8); return v; }
+static inline double __longlong_as_double(long long v) { double d; memcpy(&d, &v, 8); return d; }
 static inline double atomicAdd(double* p, double v) {   // CAS loop, like pre-sm_60 devices
     uint64_t old_bits, new_bits;
     double old;

@@ -3,6 +3,7 @@
 one run, with the detections scored on the GPU where decode and NMS leave them.
 
     python tools/valid_ensemble_b200.py datacfg darknetcfg learnetcfg weightfile [--devkit DIR] [--write-results]
+                                        [--coco-annotations instances_val2014.json] [--write-coco-results PATH]
 
 The `.data` file is read as tools/train_meta_b200.py reads it: `valid` (image list), `meta` (support dictionary), the
 class list and the `novel` / `novelid` split.  The support images of every class are run through the reweighting net
@@ -14,6 +15,12 @@ reference.
                    in DIR/annotations_cache as scripts/voc_eval.py does): prints the AP per class and the mean, base
                    and novel mean AP (VOC07 11-point metric for years before 2010, as the reference).
 --write-results    writes the reference's result files results/<backup>/ene<ckpt>/comp4_det_test_<class>.txt.
+--coco-annotations JSON
+                   scores the detections with the COCO box metric (coco_eval.DeviceCocoEval) against an
+                   instances_*.json whose images[].file_name stems are the image ids: prints pycocotools' twelve summary
+                   lines for all, base and novel classes, and the AP@[.5:.95] of each class.
+--write-coco-results PATH
+                   writes the standard COCO results json of the same detections (with --coco-annotations).
 
 Ranking differs from the reference's file-based evaluation only for detections whose printed confidences tie: they
 keep result-file order here (voc_eval.DeviceVocEval).
@@ -47,11 +54,19 @@ def main(argv=None):
     ap.add_argument('--devkit', default=None, help='VOCdevkit directory: score the detections against its annotations')
     ap.add_argument('--year', default='2007')
     ap.add_argument('--write-results', action='store_true', help='write the per-class result files')
+    ap.add_argument('--coco-annotations', default=None, help='instances_*.json: score with the COCO box metric')
+    ap.add_argument('--write-coco-results', default=None, help='COCO results json to write (with --coco-annotations)')
     ap.add_argument('--batch-size', type=int, default=64, help='query images per forward')
     ap.add_argument('--support-batch', type=int, default=64, help='support images per reweighting-net forward')
     args = ap.parse_args(argv)
-    if args.devkit is None and not args.write_results:
-        ap.error('nothing to do: give --devkit and/or --write-results')
+    if args.devkit is None and not args.write_results and args.coco_annotations is None:
+        ap.error('nothing to do: give --devkit, --coco-annotations and/or --write-results')
+    if args.coco_annotations is not None and args.devkit is not None:
+        ap.error('--devkit and --coco-annotations score the same detections twice: give one')
+    if args.write_coco_results is not None and args.coco_annotations is None:
+        ap.error('--write-coco-results needs --coco-annotations (the COCO image and category ids)')
+    if args.coco_annotations is not None and args.write_results:
+        ap.error('--write-results writes the VOC result files; with --coco-annotations use --write-coco-results')
 
     import torch
     from fewshot_detection_b200.cfg import cfg, parse_cfg
@@ -94,6 +109,8 @@ def main(argv=None):
             os.makedirs(prefix)
         logging('saving to: %s' % prefix)
         fps = [open(os.path.join(prefix, 'comp4_det_test_%s.txt' % c), 'w') for c in classes]
+    if args.coco_annotations is not None:
+        return coco_main(args, m, meta_batches, image_batches(), imgids, classes, novel)
     try:
         if args.devkit is None:
             n_cls = len(classes)
@@ -120,6 +137,28 @@ def main(argv=None):
         print('Mean Base AP = {:.4f}'.format(r['mean_base']))
     if r['mean_novel'] is not None:
         print('Mean Novel AP = {:.4f}'.format(r['mean_novel']))
+    return 0
+
+
+def coco_main(args, m, meta_batches, image_batches, imgids, classes, novel):
+    """--coco-annotations: the COCO box metric on the device, summary lines as pycocotools prints them."""
+    from fewshot_detection_b200 import coco_eval as CE, valid as VA
+    gt = CE.load_coco_annotations(args.coco_annotations, imgids, classes)
+    ev = CE.DeviceCocoEval(classes, imgids, gt)
+    results_fp = open(args.write_coco_results, 'w') if args.write_coco_results else None
+    try:
+        r = VA.valid_batches_coco(m, meta_batches, image_batches, ev, novel_classes=novel, results_fp=results_fp)
+    finally:
+        if results_fp is not None:
+            results_fp.close()
+    for title, key in (('all classes', 'all'), ('base classes', 'base'), ('novel classes', 'novel')):
+        if r[key] is None:
+            continue
+        print('COCO box metric, %s:' % title)
+        for line in CE.format_stats(r[key]):
+            print(line)
+    for c in classes:
+        print('AP for {} = {:.4f}{}'.format(c, r['ap'][c], ' (novel)' if c in novel else ''))
     return 0
 
 
