@@ -81,6 +81,9 @@ SIGNATURES = {
     'fsdet_coco_gather': ('pppiiiiiippippqpipp', 'i'),
     'fsdet_coco_workspace_bytes': ('iiii', 'z'),
     'fsdet_coco_evaluate': ('ppipippppiiippppp z pppp p'.replace(' ', ''), 'i'),
+    'fsdet_eval_merge_workspace_bytes': ('ii', 'z'),
+    'fsdet_voc_merge': ('ipppqpqipzppqpipp', 'i'),
+    'fsdet_coco_merge': ('ipppqpqipzppqpipp', 'i'),
     'fsdet_augment_workspace_bytes':('iiii', 'z'),
     'fsdet_augment_batch': ('pppiiiiipzpppp', 'i'),
     'fsdet_box_masks': ('piiipp', 'i'),

@@ -330,7 +330,9 @@ class DeviceCocoEval(object):
     `add` appends each row's first 100 kept boxes by score (csrc/coco_eval.cu), with detection_records' float64
     scores and boxes.  `result` matches and ranks on the device; only precision [T, R, K, A, M] and recall
     [T, K, A, M] come back, and the summary is computed from them on the host.  Every image of the set counts with
-    its ground truth, added or not; each image may be added once.  `last` keeps the device arrays of the last result."""
+    its ground truth, added or not; each image may be added once.  `last` keeps the device arrays of the last result.
+    `merge` and `gather` combine the pools of several evaluators as voc_eval.DeviceVocEval's do (shard.py)."""
+    POOL_KEY, MERGE_FN = 'score', 'fsdet_coco_merge'
 
     def __init__(self, classes, imagenames, gt, device=None, params=None):
         import torch
@@ -359,6 +361,34 @@ class DeviceCocoEval(object):
         self._known, self._pending = 0, 0          # records at the last read of counters[0], upper bound added since
         self._added = set()
         self.last = None
+
+    @property
+    def POOL_KEY_DTYPE(self):
+        import torch
+        return torch.float64
+
+    def empty_like(self):
+        """A new evaluator over the same classes, image set, ground truth and device, with no detections."""
+        import copy
+        import torch
+        ev = copy.copy(self)
+        ev.groups = torch.zeros_like(self.groups)
+        ev.counters = torch.zeros_like(self.counters)
+        ev.pool_cap, ev.score, ev.box = 0, None, None
+        ev._known, ev._pending, ev._added, ev.last = 0, 0, set(), None
+        return ev
+
+    @staticmethod
+    def merge(evaluators):
+        """One evaluator with the detections of `evaluators` (same image set, one device) in their order."""
+        from .shard import merge_pools
+        return merge_pools(evaluators)
+
+    def gather(self, process_group=None, dst=0, **result_kwargs):
+        """Collective: every rank's pool merged in rank order on rank `dst`, scored there once with
+        result(**result_kwargs); every rank returns that dict."""
+        from .shard import gather_result
+        return gather_result(self, process_group, dst, **result_kwargs)
 
     def _reserve(self, bound):
         """Room for `bound` more records.  Reads the record count (8 bytes) only when the upper bound could overflow."""
@@ -413,9 +443,9 @@ class DeviceCocoEval(object):
     def evaluate(self):
         """Run the device evaluation; returns the dict of device tensors (also kept in `last`)."""
         import torch
+        from .voc_eval import check_pool_flags
         n_det, n_groups, _, overflow = [int(v) for v in self.counters.cpu()]
-        if overflow:
-            raise RuntimeError('detection pool overflow')
+        check_pool_flags(overflow)
         n_cls, n_img, dev = len(self.classes), len(self.imagenames), self.device
         T, R, A, M = len(self.iou_thrs), len(self.rec_thrs), len(self.area_rng), len(self.max_dets)
         ws = torch.empty(max(1, _call_size('fsdet_coco_workspace_bytes', n_det, self.n_gt, n_cls, n_img)),

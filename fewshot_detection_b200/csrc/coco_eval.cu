@@ -520,6 +520,21 @@ extern "C" int fsdet_coco_gather(const float* cand, const int32_t* keep, const i
                             pool_cap, groups, group_cap, counters, (cudaStream_t)stream);
 }
 
+extern "C" int fsdet_coco_merge(int n_src, const long long* src_counters, const double* src_score, const double* src_box,
+                                long long src_pool_stride, const int32_t* src_groups, long long src_group_stride,
+                                int n_images, void* workspace, size_t workspace_bytes, double* score, double* box,
+                                long long pool_cap, int32_t* groups, int group_cap, long long* counters, void* stream) {
+    FSDET_CHECK_ARG(n_src > 0 && n_images > 0 && src_pool_stride >= 0 && src_group_stride >= 0 && pool_cap >= 0 &&
+                        pool_cap <= 0x7fffffffll && group_cap >= 0, "coco_merge: bad shape");
+    FSDET_CHECK_ARG(src_counters && workspace && counters && (src_group_stride == 0 || (src_groups && groups)) &&
+                        (src_pool_stride == 0 || (src_score && src_box && score && box)), "coco_merge: null pointer");
+    FSDET_CHECK_ARG(workspace_bytes >= merge_workspace_layout(nullptr, n_src, n_images).bytes,
+                    "coco_merge: workspace of %zu bytes, %zu needed", workspace_bytes,
+                    merge_workspace_layout(nullptr, n_src, n_images).bytes);
+    return eval_merge_impl(n_src, src_counters, src_score, src_box, src_pool_stride, src_groups, src_group_stride,
+                           n_images, workspace, score, box, pool_cap, groups, group_cap, counters, (cudaStream_t)stream);
+}
+
 extern "C" size_t fsdet_coco_workspace_bytes(int n_det, int n_gt, int n_cls, int n_images) {
     if (n_det < 0 || n_gt < 0 || n_cls <= 0 || n_images <= 0) return 0;
     return coco_workspace_layout(nullptr, n_det, n_gt, n_cls, n_images).bytes;

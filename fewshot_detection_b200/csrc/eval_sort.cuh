@@ -136,6 +136,110 @@ __global__ void __launch_bounds__(kVocThreads) voc_scan_apply_kernel(unsigned lo
     }
 }
 
+// ---- merge: the pools of several accumulators (one per rank of a sharded evaluation) -> one pool -----------------
+// Source s holds counters src_counters[s][4], records [s * src_pool_stride, + its record count) and groups
+// [s * src_group_stride, + its group count).  The merged pool takes the sources in order: records are copied, each
+// group's first record is rebased.  Error bits in counters[3]: overflow (a source overflowed, or the destination is
+// too small: nothing is written), an image in the groups of two sources, a group outside its source's records or
+// image range (written as an empty group).
+constexpr long long kMergeOverflow = 1, kMergeDuplicateImage = 2, kMergeBadGroup = 4;
+
+struct MergeWorkspace {
+    long long* rec_off;                               // [n_src + 1] first merged record of each source
+    long long* grp_off;                               // [n_src + 1] first merged group of each source
+    int32_t* owner;                                   // [n_images] the source whose groups name the image, or -1
+    size_t bytes;
+};
+
+static MergeWorkspace merge_workspace_layout(void* base, int n_src, int n_images) {
+    MergeWorkspace w;
+    unsigned char* p = static_cast<unsigned char*>(base);
+    size_t off = 0;
+    auto take = [&](size_t bytes) { unsigned char* q = p ? p + off : nullptr; off += (bytes + 255) & ~(size_t)255; return q; };
+    w.rec_off = reinterpret_cast<long long*>(take((size_t)(n_src + 1) * 8));
+    w.grp_off = reinterpret_cast<long long*>(take((size_t)(n_src + 1) * 8));
+    w.owner = reinterpret_cast<int32_t*>(take((size_t)n_images * 4));
+    w.bytes = off;
+    return w;
+}
+
+// One block: owner table cleared, source offsets by a serial pass over the (few) sources, destination counters set.
+__global__ void __launch_bounds__(kVocThreads) eval_merge_plan_kernel(const long long* __restrict__ src_counters, int n_src,
+                                                                      long long src_pool_stride, long long src_group_stride,
+                                                                      long long pool_cap, long long group_cap, int n_images,
+                                                                      MergeWorkspace w, long long* __restrict__ counters) {
+    for (int i = threadIdx.x; i < n_images; i += kVocThreads) w.owner[i] = -1;
+    if (threadIdx.x != 0) return;
+    long long r = 0, g = 0, err = 0;
+    for (int s = 0; s < n_src; ++s) {
+        const long long* c = src_counters + (size_t)s * 4;
+        long long nr = c[0], ng = c[1];
+        if (c[3] != 0 || nr < 0 || nr > src_pool_stride || ng < 0 || ng > src_group_stride) {
+            err |= kMergeOverflow | (c[3] & ~kMergeOverflow);
+            nr = ng = 0;
+        }
+        w.rec_off[s] = r;
+        w.grp_off[s] = g;
+        r += nr;
+        g += ng;
+    }
+    w.rec_off[n_src] = r;
+    w.grp_off[n_src] = g;
+    if (r > pool_cap || g > group_cap) err |= kMergeOverflow;
+    counters[0] = (err & kMergeOverflow) ? 0 : r;
+    counters[1] = (err & kMergeOverflow) ? 0 : g;
+    counters[2] = 0;
+    counters[3] = err;
+}
+
+// grid (blocks, n_src): group i of source s -> merged group grp_off[s] + i, its first record + rec_off[s]
+__global__ void __launch_bounds__(kVocThreads) eval_merge_groups_kernel(const int32_t* __restrict__ src_groups,
+                                                                        long long src_group_stride, int n_images,
+                                                                        MergeWorkspace w, int32_t* __restrict__ groups,
+                                                                        long long* counters) {
+    if (counters[3] & kMergeOverflow) return;
+    const int s = blockIdx.y;
+    const long long ng = w.grp_off[s + 1] - w.grp_off[s], nr = w.rec_off[s + 1] - w.rec_off[s];
+    unsigned long long* flag = reinterpret_cast<unsigned long long*>(counters + 3);
+    for (long long i = (long long)blockIdx.x * kVocThreads + threadIdx.x; i < ng; i += (long long)gridDim.x * kVocThreads) {
+        const int32_t* g = src_groups + ((size_t)s * src_group_stride + i) * 4;
+        const long long first = g[0];
+        const int count = g[1], img = g[2], cls = g[3];
+        int32_t* d = groups + (size_t)(w.grp_off[s] + i) * 4;
+        if (first < 0 || count < 0 || first + count > nr || img < 0 || img >= n_images) {
+            atomicOr(flag, (unsigned long long)kMergeBadGroup);
+            d[0] = (int32_t)w.rec_off[s];
+            d[1] = 0;
+            d[2] = 0;
+            d[3] = cls;
+            continue;
+        }
+        d[0] = (int32_t)(w.rec_off[s] + first);
+        d[1] = count;
+        d[2] = img;
+        d[3] = cls;
+        const int prev = atomicCAS(&w.owner[img], -1, s);
+        if (prev != -1 && prev != s) atomicOr(flag, (unsigned long long)kMergeDuplicateImage);
+    }
+}
+
+// grid (blocks, n_src): record i of source s -> merged record rec_off[s] + i (key and box[4])
+template <typename K>
+__global__ void __launch_bounds__(kVocThreads) eval_merge_records_kernel(const K* __restrict__ src_key,
+                                                                         const double* __restrict__ src_box,
+                                                                         long long src_pool_stride, MergeWorkspace w,
+                                                                         const long long* __restrict__ counters,
+                                                                         K* __restrict__ key, double* __restrict__ box) {
+    if (counters[3] & kMergeOverflow) return;
+    const int s = blockIdx.y;
+    const long long n = w.rec_off[s + 1] - w.rec_off[s], d0 = w.rec_off[s];
+    const size_t s0 = (size_t)s * src_pool_stride;
+    for (long long i = (long long)blockIdx.x * kVocThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kVocThreads) {
+        key[d0 + i] = src_key[s0 + i];
+        for (int q = 0; q < 4; ++q) box[(d0 + i) * 4 + q] = src_box[(s0 + i) * 4 + q];
+    }
+}
+
 // ---- host side, shared by the library and the host-emulation build -----------------------------------------------
 #ifdef FSDET_HOST_EMULATION
 #define VOC_LAUNCH(grid, block, kernel, ...) emul::launch(dim3(grid), dim3(block), 0, [&]() { kernel(__VA_ARGS__); })
@@ -160,6 +264,31 @@ static int voc_scan(unsigned long long* a, long long n, unsigned long long* part
     VOC_CHECK("voc_scan_top");
     VOC_LAUNCH(nb, kVocThreads, voc_scan_apply_kernel, a, n, part, inclusive);
     VOC_CHECK("voc_scan_apply");
+    return 0;
+}
+
+template <typename K>
+static int eval_merge_impl(int n_src, const long long* src_counters, const K* src_key, const double* src_box,
+                           long long src_pool_stride, const int32_t* src_groups, long long src_group_stride, int n_images,
+                           void* workspace, K* key, double* box, long long pool_cap, int32_t* groups, int group_cap,
+                           long long* counters, cudaStream_t st) {
+    (void)st;
+    const MergeWorkspace w = merge_workspace_layout(workspace, n_src, n_images);
+    VOC_LAUNCH(1, kVocThreads, eval_merge_plan_kernel, src_counters, n_src, src_pool_stride, src_group_stride, pool_cap,
+               (long long)group_cap, n_images, w, counters);
+    VOC_CHECK("eval_merge_plan");
+    if (src_group_stride > 0) {
+        const int gb = (int)(ceil_div(src_group_stride, kVocThreads) < 256 ? ceil_div(src_group_stride, kVocThreads) : 256);
+        VOC_LAUNCH(dim3(gb, n_src), kVocThreads, eval_merge_groups_kernel, src_groups, src_group_stride, n_images, w,
+                   groups, counters);
+        VOC_CHECK("eval_merge_groups");
+    }
+    if (src_pool_stride > 0) {
+        const int rb = (int)(ceil_div(src_pool_stride, kVocThreads) < 1024 ? ceil_div(src_pool_stride, kVocThreads) : 1024);
+        VOC_LAUNCH(dim3(rb, n_src), kVocThreads, eval_merge_records_kernel<K>, src_key, src_box, src_pool_stride, w,
+                   counters, key, box);
+        VOC_CHECK("eval_merge_records");
+    }
     return 0;
 }
 

@@ -450,6 +450,26 @@ extern "C" int fsdet_voc_gather(const float* cand, const int32_t* keep, const in
                            groups, group_cap, counters, (cudaStream_t)stream);
 }
 
+extern "C" size_t fsdet_eval_merge_workspace_bytes(int n_src, int n_images) {
+    if (n_src <= 0 || n_images < 0) return 0;
+    return merge_workspace_layout(nullptr, n_src, n_images).bytes;
+}
+
+extern "C" int fsdet_voc_merge(int n_src, const long long* src_counters, const uint32_t* src_key, const double* src_box,
+                               long long src_pool_stride, const int32_t* src_groups, long long src_group_stride,
+                               int n_images, void* workspace, size_t workspace_bytes, uint32_t* rank_key, double* box,
+                               long long pool_cap, int32_t* groups, int group_cap, long long* counters, void* stream) {
+    FSDET_CHECK_ARG(n_src > 0 && n_images > 0 && src_pool_stride >= 0 && src_group_stride >= 0 && pool_cap >= 0 &&
+                        pool_cap <= 0x7fffffffll && group_cap >= 0, "voc_merge: bad shape");
+    FSDET_CHECK_ARG(src_counters && workspace && counters && (src_group_stride == 0 || (src_groups && groups)) &&
+                        (src_pool_stride == 0 || (src_key && src_box && rank_key && box)), "voc_merge: null pointer");
+    FSDET_CHECK_ARG(workspace_bytes >= merge_workspace_layout(nullptr, n_src, n_images).bytes,
+                    "voc_merge: workspace of %zu bytes, %zu needed", workspace_bytes,
+                    merge_workspace_layout(nullptr, n_src, n_images).bytes);
+    return eval_merge_impl(n_src, src_counters, src_key, src_box, src_pool_stride, src_groups, src_group_stride, n_images,
+                           workspace, rank_key, box, pool_cap, groups, group_cap, counters, (cudaStream_t)stream);
+}
+
 extern "C" size_t fsdet_voc_workspace_bytes(int n_det, int n_gt) {
     if (n_det < 0 || n_gt < 0) return 0;
     return voc_workspace_layout(nullptr, n_det, n_gt).bytes;

@@ -61,11 +61,16 @@ def epoch_plan(model_seen, nsamples, batch_size, max_batches, tuning=False, max_
 
 class MetaTrainer(object):
     def __init__(self, model, optimizer, learning_rate, batch_size, steps, scales, make_train_batcher, make_meta_batcher,
-                 backupdir=None, save_interval=10, reducer=None, world=1, processed_batches=0, log=print, use_graph=None):
+                 backupdir=None, save_interval=10, reducer=None, world=1, processed_batches=0, log=print, use_graph=None,
+                 evaluate=None):
         """learning_rate: the cfg rate already divided by `lr_factor` (what the driver calls `learning_rate` after
         :136); batch_size: GLOBAL batch; make_train_batcher(seen) / make_meta_batcher(): the epoch's data streams.
         use_graph: replay the step from CUDA graphs (graph.GraphedTrainStep: one graph per input shape, neg_filter
-        staged from the host) - the default whenever the model's parameters live on a CUDA device."""
+        staged from the host) - the default whenever the model's parameters live on a CUDA device.
+        evaluate: optional evaluate(model, epoch), run on every rank at the end of each checkpoint epoch (every
+        `save_interval` epochs), after the weight file is written where one is written (rank 0 with a backupdir) and
+        whether or not one is: every rank takes part in a sharded evaluation.  What it returns is logged
+        (see evaluate_checkpoint)."""
         self.model, self.optimizer = model, optimizer
         self.region_loss = model.loss
         self.learning_rate, self.batch_size = learning_rate, batch_size
@@ -76,6 +81,7 @@ class MetaTrainer(object):
         self.processed_batches = processed_batches
         self.region_loss.seen = model.seen           # train_meta.py:93
         self.log = log
+        self.evaluate = evaluate
         self.losses = collections.deque(maxlen=100)   # detached loss tensors of the most recent steps (no host sync)
         import os
         if use_graph is None:
@@ -161,7 +167,34 @@ class MetaTrainer(object):
             self.log('save weights to %s' % path)
             self.model.seen = (epoch + 1) * len(batcher) * self.world
             self.model.save_weights(path)
+        if (epoch + 1) % self.save_interval == 0:
+            self.evaluate_checkpoint(epoch + 1)
         return nb
+
+    def evaluate_checkpoint(self, epoch):
+        """Run `evaluate(model, epoch)` without changing training: the model goes to eval() (BatchNorm uses and keeps
+        its running statistics) and back to its mode; the Python `random`, numpy and torch CPU generators that the
+        batchers and neg_filter draw from are restored.  The step graphs stay valid: the evaluation forwards reuse the
+        engine's weight plan (same weight tensors) and allocate outside the graphs' pool.  Returns and logs the
+        callback's value."""
+        if self.evaluate is None:
+            return None
+        import random
+        import numpy as np
+        import torch
+        py_state, np_state, torch_state = random.getstate(), np.random.get_state(), torch.get_rng_state()
+        was_training = self.model.training
+        try:
+            self.model.eval()
+            r = self.evaluate(self.model, epoch)
+        finally:
+            self.model.train(was_training)
+            random.setstate(py_state)
+            np.random.set_state(np_state)
+            torch.set_rng_state(torch_state)
+        if r is not None:
+            self.log('evaluation at epoch %d: %s' % (epoch, r))
+        return r
 
     def fit(self, init_epoch, max_epochs):
         for epoch in range(int(init_epoch), int(max_epochs)):

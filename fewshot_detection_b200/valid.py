@@ -174,3 +174,107 @@ def valid_batches_coco(m, meta_batches, image_batches, evaluator, novel_classes=
         ids = dict((n, i) for n, i in zip(evaluator.imagenames, evaluator.image_ids))
         coco_eval.write_coco_results(results_fp, records, ids, evaluator.category_ids)
     return evaluator.result(novel_classes)
+
+
+# ---- the same passes sharded over the ranks of a process group (shard.py) -------------------------------------------
+def sharded_ensemble_dynamic_weights(m, meta_batches, n_cls, process_group=None):
+    """ensemble_dynamic_weights over every rank's support batches, in rank order.  `meta_batches` are this rank's
+    block of the single-process batches (shard.shard_range).  Each rank runs the reweighting net on its own batches;
+    the vectors, class ids and batch sizes are all-gathered and every rank applies the running mean batch by batch in
+    the single-process order, so every rank returns the single-process result, bit for bit."""
+    import numpy as np
+    from .shard import all_gather_padded, group_info
+    world, _ = group_info(process_group)
+    dev = next(m.parameters()).device
+    rows, ids, sizes = [], [], []
+    with torch.no_grad():
+        for metax, mask, clsids in meta_batches:
+            dw = m.meta_forward(metax.to(dev), mask.to(dev))[0]
+            rows.append(dw.detach().reshape(dw.size(0), -1).float())
+            ids.extend(int(c) for c in clsids)
+            sizes.append(int(dw.size(0)))
+    C = int(rows[0].size(1)) if rows else 0
+    shape = torch.tensor([[len(sizes), len(ids), C]], dtype=torch.int64, device=dev)
+    shapes = all_gather_padded(shape, 1, process_group).reshape(world, 3).cpu().numpy()
+    C = int(shapes[:, 2].max())
+    if C == 0:
+        raise ValueError('no support batches')
+    if any(c not in (0, C) for c in shapes[:, 2]):
+        raise ValueError('ranks disagree on the reweighting vector size: %s' % shapes[:, 2].tolist())
+    nb, nr = max(1, int(shapes[:, 0].max())), max(1, int(shapes[:, 1].max()))
+    local = torch.cat(rows) if rows else torch.zeros(0, C, dtype=torch.float32, device=dev)
+    all_rows = all_gather_padded(local, nr, process_group)
+    all_ids = all_gather_padded(torch.tensor(ids, dtype=torch.int64).reshape(-1).to(dev), nr, process_group).cpu().numpy()
+    all_sizes = all_gather_padded(torch.tensor(sizes, dtype=torch.int64).reshape(-1).to(dev), nb, process_group).cpu().numpy()
+    ens = ReweightEnsembler(n_cls, C, dev)
+    for r in range(world):
+        off = 0
+        for b in range(int(shapes[r, 0])):
+            n = int(all_sizes[r, b])
+            ens.update(all_rows[r, off:off + n], np.asarray(all_ids[r, off:off + n]).tolist())
+            off += n
+    return ens.result()
+
+
+def gather_to(obj, process_group, dst):
+    """The objects of every rank, in rank order, on rank `dst` (None elsewhere)."""
+    import torch.distributed as dist
+    from .shard import global_rank, group_info
+    world, rank = group_info(process_group)
+    out = [None] * world if rank == dst else None
+    dist.gather_object(obj, out, dst=global_rank(process_group, dst), group=process_group)
+    return out
+
+
+def sharded_valid_ap(m, support_batches, image_batches, evaluator, use_07_metric=True, novel_classes=(), fps=None,
+                     process_group=None, dst=0):
+    """valid_batches_ap with this rank's block of the support and query batches (shard.shard_range); collective over
+    `process_group`.  The pools are merged in rank order and scored once on rank `dst`; every rank returns mean_ap's
+    dict, equal to the single-process one.  fps: the per-class result files, open on `dst`, and True on the other
+    ranks (their lines go to `dst`, which writes every rank's lines in rank order: the single-process files); None on
+    every rank for no files."""
+    from .shard import group_info
+    _, rank = group_info(process_group)
+    n_cls = len(evaluator.classes)
+    m.eval()
+    dynamic_weights = sharded_ensemble_dynamic_weights(m, support_batches, n_cls, process_group)
+    dev = next(m.parameters()).device
+    lines = dict((i, []) for i in range(n_cls))
+    for data, imgids, sizes in image_batches:
+        dets = detect(m, data.to(dev), dynamic_weights, n_cls)
+        evaluator.add(dets, imgids, sizes)
+        if fps is not None:
+            for i, l in detection_lines(dets, imgids, sizes, n_cls).items():
+                lines[i].extend(l)
+    if fps is not None:
+        parts = gather_to(lines, process_group, dst)
+        if rank == dst:
+            for part in parts:
+                for i in range(n_cls):
+                    fps[i].writelines(part[i])
+    return evaluator.gather(process_group, dst, use_07_metric=use_07_metric, novel_classes=novel_classes)
+
+
+def sharded_valid_coco(m, support_batches, image_batches, evaluator, novel_classes=(), results_fp=None,
+                       process_group=None, dst=0):
+    """valid_batches_coco sharded as sharded_valid_ap.  results_fp: the results json, open on `dst`, True on the
+    other ranks; None on every rank for no file."""
+    from . import coco_eval
+    from .shard import group_info
+    _, rank = group_info(process_group)
+    n_cls = len(evaluator.classes)
+    m.eval()
+    dynamic_weights = sharded_ensemble_dynamic_weights(m, support_batches, n_cls, process_group)
+    dev = next(m.parameters()).device
+    records = []
+    for data, imgids, sizes in image_batches:
+        dets = detect(m, data.to(dev), dynamic_weights, n_cls)
+        evaluator.add(dets, imgids, sizes)
+        if results_fp is not None:
+            records.extend(coco_eval.detection_records(dets, imgids, sizes, n_cls, evaluator.max_det))
+    if results_fp is not None:
+        parts = gather_to(records, process_group, dst)
+        if rank == dst:
+            ids = dict((n, i) for n, i in zip(evaluator.imagenames, evaluator.image_ids))
+            coco_eval.write_coco_results(results_fp, [r for p in parts for r in p], ids, evaluator.category_ids)
+    return evaluator.gather(process_group, dst, novel_classes=novel_classes)

@@ -191,7 +191,11 @@ class DeviceVocEval(object):
     and scores every class on the device; only per-class numbers come back (and, with curves=True, rec / prec).
     Ranking differs from the file path in one deliberate way: detections with equal printed confidences keep
     result-file order (a stable sort), where np.argsort's order at ties depends on numpy's sort implementation.
-    Each image of the set may be added once."""
+    Each image of the set may be added once.
+
+    Sharded over ranks (shard.py): each rank adds its own contiguous block of batches, then `gather` merges the pools
+    in rank order on one rank and scores them there; `merge` does the same for several evaluators on one device."""
+    POOL_KEY, MERGE_FN = 'rank_key', 'fsdet_voc_merge'
 
     def __init__(self, classes, imagenames, recs, device=None, ovthresh=0.5):
         import torch
@@ -214,6 +218,35 @@ class DeviceVocEval(object):
         self._known, self._pending = 0, 0          # records at the last read of counters[0], upper bound added since
         self._added = set()
         self.last = None
+
+    @property
+    def POOL_KEY_DTYPE(self):
+        import torch
+        return torch.int32
+
+    def empty_like(self):
+        """A new evaluator over the same classes, image set, ground truth and device, with no detections."""
+        import copy
+        import torch
+        ev = copy.copy(self)
+        ev.groups = torch.zeros_like(self.groups)
+        ev.counters = torch.zeros_like(self.counters)
+        ev.pool_cap, ev.rank_key, ev.box = 0, None, None
+        ev._known, ev._pending, ev._added, ev.last = 0, 0, set(), None
+        return ev
+
+    @staticmethod
+    def merge(evaluators):
+        """One evaluator with the detections of `evaluators` (same image set, one device) in their order: the pool a
+        single evaluator would hold had it been given their batches in that order."""
+        from .shard import merge_pools
+        return merge_pools(evaluators)
+
+    def gather(self, process_group=None, dst=0, **result_kwargs):
+        """Collective: the pools of every rank of `process_group` merged in rank order on rank `dst`, scored there
+        once with result(**result_kwargs); every rank returns that dict."""
+        from .shard import gather_result
+        return gather_result(self, process_group, dst, **result_kwargs)
 
     def _reserve(self, bound):
         """Room for `bound` more records.  Reads the record count (8 bytes) only when the upper bound could overflow."""
@@ -271,8 +304,7 @@ class DeviceVocEval(object):
         The device results of the last call stay in `self.last` (flags, order, rec, prec, ... as tensors)."""
         import torch
         n_det, n_groups, _, overflow = [int(v) for v in self.counters.cpu()]
-        if overflow:
-            raise RuntimeError('detection pool overflow')
+        check_pool_flags(overflow)
         n_cls, dev = len(self.classes), self.device
         ws = torch.empty(max(1, _call_size('fsdet_voc_workspace_bytes', n_det, self.n_gt)), dtype=torch.uint8, device=dev)
         out = dict(flags=torch.empty(n_det, dtype=torch.uint8, device=dev),
@@ -306,3 +338,13 @@ class DeviceVocEval(object):
 def _call_size(name, *args):
     from ._lib import lib
     return int(getattr(lib, name)(*args))
+
+
+def check_pool_flags(flags):
+    """Raise on the error bits the gather / merge kernels leave in counters[3]."""
+    if flags & 1:
+        raise RuntimeError('detection pool overflow')
+    if flags & 2:
+        raise RuntimeError('merged pools: an image was evaluated on two ranks')
+    if flags & 4:
+        raise RuntimeError('merged pools: a group outside its pool')

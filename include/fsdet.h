@@ -370,6 +370,18 @@ int fsdet_voc_evaluate(const uint32_t* rank_key, const double* box, int n_det, c
                        int n_images, double ovthresh, const double* thresholds, void* workspace, size_t workspace_bytes,
                        uint8_t* flags, int32_t* order, double* rec, double* prec, int32_t* cls_count, int32_t* npos,
                        double* ap07, double* ap_area, void* stream);
+/* The pools of several accumulators (one per rank of a sharded evaluation, gathered into padded buffers) -> one
+ * pool, sources in order.  Source s: counters src_counters[s][4] (as the gather leaves them), records
+ * [s * src_pool_stride, + records) and groups [s * src_group_stride, + groups).  Records are copied into place and each
+ * group's first record is rebased; counters (int64 [4]) get {records, groups, 0, error bits}: 1 = overflow (a source
+ * overflowed, or pool_cap / group_cap is too small: nothing is written), 2 = an image named by groups of two sources,
+ * 4 = a group outside its source's records or image range (written empty).  Nothing is written out of bounds.
+ * Workspace: fsdet_eval_merge_workspace_bytes(n_src, n_images).  No synchronisation. */
+size_t fsdet_eval_merge_workspace_bytes(int n_src, int n_images);
+int fsdet_voc_merge(int n_src, const long long* src_counters, const uint32_t* src_key, const double* src_box,
+                    long long src_pool_stride, const int32_t* src_groups, long long src_group_stride, int n_images,
+                    void* workspace, size_t workspace_bytes, uint32_t* rank_key, double* box, long long pool_cap,
+                    int32_t* groups, int group_cap, long long* counters, void* stream);
 
 /* ---- COCO box AP / AR from device-resident detections (csrc/coco_eval.cu) -- */
 /* pycocotools COCOeval (bbox, useCats=1) as coco_eval.py defines it, bit for bit in float64.  The caller owns every
@@ -394,6 +406,11 @@ int fsdet_coco_evaluate(const double* score, const double* box, int n_det, const
                         int n_gt, int n_cls, int n_images, const double* iou_thrs, const double* rec_thrs,
                         const int32_t* max_dets, const double* area_rng, void* workspace, size_t workspace_bytes,
                         uint32_t* dt_flags, int32_t* order, double* precision, double* recall, void* stream);
+/* fsdet_voc_merge for the COCO pools (score float64 instead of rank_key). */
+int fsdet_coco_merge(int n_src, const long long* src_counters, const double* src_score, const double* src_box,
+                     long long src_pool_stride, const int32_t* src_groups, long long src_group_stride, int n_images,
+                     void* workspace, size_t workspace_bytes, double* score, double* box, long long pool_cap,
+                     int32_t* groups, int group_cap, long long* counters, void* stream);
 
 /* ---- training-input augmentation (SURVEY.md 8f row 3) ---------------------- */
 /* image.data_augmentation (image.py:52-87: crop with zero fill, PIL resize, horizontal flip, HSV jitter through

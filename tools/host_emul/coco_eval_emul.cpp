@@ -20,6 +20,18 @@ extern "C" int emul_coco_gather(const float* cand, const int32_t* keep, const in
                             pool_cap, groups, group_cap, counters, nullptr);
 }
 
+extern "C" size_t emul_eval_merge_workspace_bytes(int n_src, int n_images) {
+    return merge_workspace_layout(nullptr, n_src, n_images).bytes;
+}
+
+extern "C" int emul_coco_merge(int n_src, const long long* src_counters, const double* src_score, const double* src_box,
+                               long long src_pool_stride, const int32_t* src_groups, long long src_group_stride,
+                               int n_images, void* workspace, double* score, double* box, long long pool_cap,
+                               int32_t* groups, int group_cap, long long* counters) {
+    return eval_merge_impl(n_src, src_counters, src_score, src_box, src_pool_stride, src_groups, src_group_stride,
+                           n_images, workspace, score, box, pool_cap, groups, group_cap, counters, nullptr);
+}
+
 extern "C" size_t emul_coco_workspace_bytes(int n_det, int n_gt, int n_cls, int n_images) {
     return coco_workspace_layout(nullptr, n_det, n_gt, n_cls, n_images).bytes;
 }

@@ -72,6 +72,13 @@ static inline int __float_as_int(float f) { int v; memcpy(&v, &f, 4); return v; 
 static inline unsigned __float_as_uint(float f) { unsigned v; memcpy(&v, &f, 4); return v; }
 static inline int atomicExch(int* p, int v) { return __atomic_exchange_n(p, v, __ATOMIC_SEQ_CST); }
 static inline int atomicAdd(int* p, int v) { return __atomic_fetch_add(p, v, __ATOMIC_SEQ_CST); }
+static inline int atomicCAS(int* p, int compare, int v) {
+    __atomic_compare_exchange_n(p, &compare, v, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST);
+    return compare;                               // the old value, whether or not it was swapped
+}
+static inline unsigned long long atomicOr(unsigned long long* p, unsigned long long v) {
+    return __atomic_fetch_or(p, v, __ATOMIC_SEQ_CST);
+}
 static inline int atomicMax(int* p, int v) {   // CAS loop
     int old = __atomic_load_n(p, __ATOMIC_SEQ_CST);
     while (old < v && !__atomic_compare_exchange_n(p, &old, v, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST)) {

@@ -30,6 +30,18 @@ extern "C" int emul_voc_gather(const float* cand, const int32_t* keep, const int
                            groups, group_cap, counters, nullptr);
 }
 
+extern "C" size_t emul_eval_merge_workspace_bytes(int n_src, int n_images) {
+    return merge_workspace_layout(nullptr, n_src, n_images).bytes;
+}
+
+extern "C" int emul_voc_merge(int n_src, const long long* src_counters, const uint32_t* src_key, const double* src_box,
+                              long long src_pool_stride, const int32_t* src_groups, long long src_group_stride,
+                              int n_images, void* workspace, uint32_t* rank_key, double* box, long long pool_cap,
+                              int32_t* groups, int group_cap, long long* counters) {
+    return eval_merge_impl(n_src, src_counters, src_key, src_box, src_pool_stride, src_groups, src_group_stride, n_images,
+                           workspace, rank_key, box, pool_cap, groups, group_cap, counters, nullptr);
+}
+
 extern "C" size_t emul_voc_workspace_bytes(int n_det, int n_gt) { return voc_workspace_layout(nullptr, n_det, n_gt).bytes; }
 
 extern "C" int emul_voc_evaluate(const uint32_t* rank_key, const double* box, int n_det, const int32_t* groups,

@@ -9,9 +9,13 @@ The `.data` file drives everything as in the reference: `train` (image list or c
 from lists.build_dataset, the support index from lists.support_index, the step from trainer.MetaTrainer (CUDA-graph
 replay, one graph per multi-scale input size).  Under torchrun every rank builds the same lists with the same seeds,
 takes its slice of each global batch, and rank 0's parameters are broadcast once before the first step.
-What the reference's script does beyond that - the in-training test() pass - is not wired here; a trained weight file
-is scored by tools/valid_ensemble_b200.py (valid_ensemble.py + scripts/voc_eval.py), built on
-`fewshot_detection_b200.evaluate` / `valid` / `voc_eval`.
+A trained weight file is scored by tools/valid_ensemble_b200.py (valid_ensemble.py + scripts/voc_eval.py).  Opt-in,
+every checkpoint is scored the same way while training runs, sharded over the ranks (valid.sharded_valid_ap):
+
+    --eval-devkit DIR [--eval-year Y]      VOC AP on the `valid` list: one line with mean, base and novel AP
+    --eval-coco-annotations JSON           COCO box AP on the `valid` list: one line with AP, AP50, AP75
+
+with the support set, batch sizes and thresholds of the evaluation command.
 """
 import os
 import sys
@@ -43,11 +47,66 @@ def broadcast_parameters(model, src=0):
             raise RuntimeError('replicas differ after the parameter broadcast')
 
 
+def checkpoint_evaluator(data_options, devkit, year, coco_annotations, world, rank, batch_size=64, support_batch=64):
+    """evaluate(model, epoch) for MetaTrainer: the evaluation command's pass over `valid`, this rank's shard of it;
+    returns the line rank 0 logs."""
+    from fewshot_detection_b200.cfg import cfg
+    from fewshot_detection_b200.dataset import DetectionBatcher, MetaBatcher
+    from fewshot_detection_b200.shard import rank0_first, shard_range
+    from fewshot_detection_b200 import lists as LS, valid as VA, voc_eval as VE, coco_eval as CE
+    classes, novel = list(cfg.classes), list(cfg.novel_classes)
+    metalines, inds = LS.support_index(data_options['meta'], classes, 0, ensemble=True)
+    lines = read_list(data_options['valid'])
+    imgids = [os.path.basename(l).split('.')[0] for l in lines]
+    if coco_annotations is not None:
+        proto = CE.DeviceCocoEval(classes, imgids, CE.load_coco_annotations(coco_annotations, imgids, classes))
+    else:
+        voc = os.path.join(devkit, 'VOC' + year)
+        names = read_list(os.path.join(voc, 'ImageSets', 'Main', 'test.txt'))
+        load = lambda: VE.load_annotations(os.path.join(voc, 'Annotations', '{}.xml'), names,
+                                           os.path.join(devkit, 'annotations_cache'))
+        recs = rank0_first(load) if world > 1 else load()  # rank 0 writes the cache, the others read it
+        proto = VE.DeviceVocEval(classes, names, recs)
+    s0, s1 = shard_range(len(inds), support_batch, world, rank)
+    q0, q1 = shard_range(len(lines), batch_size, world, rank)
+
+    def evaluate(model, epoch):
+        mb = MetaBatcher(metalines, inds, classes=classes, train=False, ensemble=True, with_ids=True)
+        meta = (mb.batch(range(s, min(s + support_batch, s1))) for s in range(s0, s1, support_batch))
+        db = DetectionBatcher(lines, shape=(model.width, model.height), shuffle=False, train=False, batch_size=batch_size)
+
+        def images():
+            for s in range(q0, q1, batch_size):
+                idx = range(s, min(s + batch_size, q1))
+                yield db.batch(idx)[0], [imgids[i] for i in idx], [db._entry(i).size() for i in idx]
+        ev = proto.empty_like()
+        if coco_annotations is not None:
+            fn = VA.sharded_valid_coco if world > 1 else VA.valid_batches_coco
+            r = fn(model, meta, images(), ev, novel_classes=novel)
+            return 'COCO AP %.4f AP50 %.4f AP75 %.4f' % tuple(r['all'][:3])
+        if world > 1:
+            r = VA.sharded_valid_ap(model, meta, images(), ev, int(year) < 2010, novel_classes=novel)
+        else:
+            r = VA.valid_batches_ap(model, meta, images(), ev, int(year) < 2010, novel_classes=novel)
+        fmt = lambda v: 'n/a' if v is None else '%.4f' % v
+        return 'mAP %s base %s novel %s' % (fmt(r['mean']), fmt(r['mean_base']), fmt(r['mean_novel']))
+    return evaluate
+
+
 def main():
-    if len(sys.argv) != 5:
+    import argparse
+    ap = argparse.ArgumentParser(add_help=False)
+    ap.add_argument('args', nargs='*')
+    ap.add_argument('--eval-devkit', default=None)
+    ap.add_argument('--eval-year', default='2007')
+    ap.add_argument('--eval-coco-annotations', default=None)
+    opts = ap.parse_args()
+    if len(opts.args) != 4 or (opts.eval_devkit is not None and opts.eval_coco_annotations is not None):
         print('Usage:')
-        print('python tools/train_meta_b200.py datacfg darknetcfg learnetcfg weightfile')
+        print('python tools/train_meta_b200.py datacfg darknetcfg learnetcfg weightfile '
+              '[--eval-devkit DIR [--eval-year Y] | --eval-coco-annotations JSON]')
         return 1
+    argv = [sys.argv[0]] + opts.args
     from fewshot_detection_b200.cfg import cfg, parse_cfg
     from fewshot_detection_b200.utils import read_data_cfg, logging
     from fewshot_detection_b200.darknet_meta import Darknet
@@ -64,8 +123,8 @@ def main():
     if world > 1:
         dist.init_process_group('nccl', device_id=torch.device('cuda', local))
 
-    data_options = read_data_cfg(sys.argv[1])
-    darknetcfg, learnetcfg = parse_cfg(sys.argv[2]), parse_cfg(sys.argv[3])
+    data_options = read_data_cfg(argv[1])
+    darknetcfg, learnetcfg = parse_cfg(argv[2]), parse_cfg(argv[3])
     net_options, meta_options = darknetcfg[0], learnetcfg[0]
     cfg.config_data(data_options)
     cfg.config_meta(meta_options)
@@ -76,10 +135,10 @@ def main():
     scales = [float(s) for s in net_options['scales'].split(',')]
 
     model = Darknet(darknetcfg, learnetcfg)
-    if os.path.exists(sys.argv[4]):
-        model.load_weights(sys.argv[4])
+    if os.path.exists(argv[4]):
+        model.load_weights(argv[4])
     else:
-        logging('weight file %s not found: training from the random initialisation' % sys.argv[4])
+        logging('weight file %s not found: training from the random initialisation' % argv[4])
     model = model.cuda()
     if world > 1:
         broadcast_parameters(model)
@@ -115,10 +174,17 @@ def main():
                                            shuffle=cfg.randmeta)
         return MetaBatcher(metalines, inds, classes=classes, train=True)
 
+    evaluate = None
+    if opts.eval_devkit is not None or opts.eval_coco_annotations is not None:
+        state = random.getstate(), np.random.get_state()          # the training lists' draws stay as without it
+        evaluate = checkpoint_evaluator(data_options, opts.eval_devkit, opts.eval_year, opts.eval_coco_annotations,
+                                        world, rank)
+        random.setstate(state[0])
+        np.random.set_state(state[1])
     tr = T.MetaTrainer(model, optimizer, float(net_options['learning_rate']) / factor, batch_size, steps, scales,
                        make_train_batcher, make_meta_batcher, backupdir=backupdir if rank == 0 else None,
                        save_interval=cfg.save_interval, reducer=reducer, world=world, processed_batches=processed,
-                       log=logging if rank == 0 else (lambda *_: None))
+                       log=logging if rank == 0 else (lambda *_: None), evaluate=evaluate)
     model.loss.verbose = rank == 0
     tr.fit(init_epoch, max_epochs)
     if world > 1:

@@ -24,6 +24,10 @@ reference.
 
 Ranking differs from the reference's file-based evaluation only for detections whose printed confidences tie: they
 keep result-file order here (voc_eval.DeviceVocEval).
+
+Under `torchrun --nproc-per-node N` every process takes the GPU of its LOCAL_RANK and a contiguous block of whole
+support and query batches (shard.shard_range); the support vectors and the detection pools are gathered in rank order,
+so the printed numbers and the written files are those of one process, bit for bit.  Only rank 0 prints and writes.
 """
 import argparse
 import os
@@ -69,13 +73,33 @@ def main(argv=None):
         ap.error('--write-results writes the VOC result files; with --coco-annotations use --write-coco-results')
 
     import torch
+
+    world = int(os.environ.get('WORLD_SIZE', '1'))
+    rank = int(os.environ.get('RANK', '0'))
+    if world > 1:
+        import torch.distributed as dist
+        local = int(os.environ['LOCAL_RANK'])
+        torch.cuda.set_device(local)
+        dist.init_process_group('nccl', device_id=torch.device('cuda', local))
+        try:
+            return run(args, world, dist.get_rank())
+        finally:
+            torch.cuda.synchronize()
+            dist.destroy_process_group()
+    torch.cuda.set_device(0)
+    return run(args, 1, 0)
+
+
+def run(args, world, rank):
+    """The evaluation on this process's shard (the whole set when world == 1)."""
+    import torch
     from fewshot_detection_b200.cfg import cfg, parse_cfg
     from fewshot_detection_b200.utils import read_data_cfg, logging
     from fewshot_detection_b200.darknet_meta import Darknet
     from fewshot_detection_b200.dataset import DetectionBatcher, MetaBatcher
+    from fewshot_detection_b200.shard import rank0_first, shard_range
     from fewshot_detection_b200 import lists as LS, valid as VA, voc_eval as VE
-
-    torch.cuda.set_device(0)
+    sharded, lead = world > 1, rank == 0
     data_options = read_data_cfg(args.datacfg)
     darknetcfg, learnetcfg = parse_cfg(args.darknetcfg), parse_cfg(args.learnetcfg)
     cfg.config_data(data_options)
@@ -90,45 +114,68 @@ def main(argv=None):
 
     metalines, inds = LS.support_index(data_options['meta'], classes, 0, ensemble=True)
     mb = MetaBatcher(metalines, inds, classes=classes, train=False, ensemble=True, with_ids=True)
-    meta_batches = (mb.batch(range(s, min(s + args.support_batch, len(inds)))) for s in range(0, len(inds), args.support_batch))
+    s0, s1 = shard_range(len(inds), args.support_batch, world, rank)
+    meta_batches = (mb.batch(range(s, min(s + args.support_batch, s1))) for s in range(s0, s1, args.support_batch))
 
     lines = read_list(data_options['valid'])
     db = DetectionBatcher(lines, shape=(m.width, m.height), shuffle=False, train=False, batch_size=args.batch_size)
     imgids = [os.path.basename(l).split('.')[0] for l in lines]
 
+    q0, q1 = shard_range(len(lines), args.batch_size, world, rank)
+
     def image_batches():
-        for s in range(0, len(lines), args.batch_size):
-            idx = range(s, min(s + args.batch_size, len(lines)))
+        for s in range(q0, q1, args.batch_size):
+            idx = range(s, min(s + args.batch_size, q1))
             data, _ = db.batch(idx)
             yield data, [imgids[i] for i in idx], [db._entry(i).size() for i in idx]
 
     fps = None
-    if args.write_results:
+    if args.write_results and not lead:
+        fps = True                                    # this rank's lines go to rank 0
+    elif args.write_results:
         prefix = result_prefix(args.weightfile)
         if not os.path.exists(prefix):
             os.makedirs(prefix)
         logging('saving to: %s' % prefix)
         fps = [open(os.path.join(prefix, 'comp4_det_test_%s.txt' % c), 'w') for c in classes]
     if args.coco_annotations is not None:
-        return coco_main(args, m, meta_batches, image_batches(), imgids, classes, novel)
+        return coco_main(args, m, meta_batches, image_batches(), imgids, classes, novel, sharded, lead)
     try:
         if args.devkit is None:
             n_cls = len(classes)
-            dw = VA.ensemble_dynamic_weights(m, meta_batches, n_cls)
+            if not sharded:
+                dw = VA.ensemble_dynamic_weights(m, meta_batches, n_cls)
+                for data, ids, sizes in image_batches():
+                    VA.write_detections(fps, VA.detect(m, data, dw, n_cls), ids, sizes, n_cls)
+                return 0
+            dw = VA.sharded_ensemble_dynamic_weights(m, meta_batches, n_cls)
+            mine = dict((i, []) for i in range(n_cls))
             for data, ids, sizes in image_batches():
-                VA.write_detections(fps, VA.detect(m, data, dw, n_cls), ids, sizes, n_cls)
+                for i, l in VA.detection_lines(VA.detect(m, data, dw, n_cls), ids, sizes, n_cls).items():
+                    mine[i].extend(l)
+            parts = VA.gather_to(mine, None, 0)
+            if lead:
+                for part in parts:
+                    for i in range(n_cls):
+                        fps[i].writelines(part[i])
             return 0
         voc = os.path.join(args.devkit, 'VOC' + args.year)
         imagenames = read_list(os.path.join(voc, 'ImageSets', 'Main', 'test.txt'))
-        recs = VE.load_annotations(os.path.join(voc, 'Annotations', '{}.xml'), imagenames,
-                                   os.path.join(args.devkit, 'annotations_cache'))
+        load = lambda: VE.load_annotations(os.path.join(voc, 'Annotations', '{}.xml'), imagenames,
+                                           os.path.join(args.devkit, 'annotations_cache'))
+        recs = rank0_first(load) if sharded else load()    # rank 0 writes the cache, the others read it
         use_07 = int(args.year) < 2010
         ev = VE.DeviceVocEval(classes, imagenames, recs)
-        r = VA.valid_batches_ap(m, meta_batches, image_batches(), ev, use_07, novel_classes=novel, fps=fps)
+        if sharded:
+            r = VA.sharded_valid_ap(m, meta_batches, image_batches(), ev, use_07, novel_classes=novel, fps=fps)
+        else:
+            r = VA.valid_batches_ap(m, meta_batches, image_batches(), ev, use_07, novel_classes=novel, fps=fps)
     finally:
-        if fps is not None:
+        if fps is not None and fps is not True:
             for f in fps:
                 f.close()
+    if not lead:
+        return 0
     print('VOC07 metric? ' + ('Yes' if use_07 else 'No'))
     for c in classes:
         print('AP for {} = {:.4f}{}'.format(c, r['ap'][c], ' (novel)' if c in novel else ''))
@@ -140,17 +187,24 @@ def main(argv=None):
     return 0
 
 
-def coco_main(args, m, meta_batches, image_batches, imgids, classes, novel):
+def coco_main(args, m, meta_batches, image_batches, imgids, classes, novel, sharded=False, lead=True):
     """--coco-annotations: the COCO box metric on the device, summary lines as pycocotools prints them."""
     from fewshot_detection_b200 import coco_eval as CE, valid as VA
     gt = CE.load_coco_annotations(args.coco_annotations, imgids, classes)
     ev = CE.DeviceCocoEval(classes, imgids, gt)
-    results_fp = open(args.write_coco_results, 'w') if args.write_coco_results else None
+    results_fp = None
+    if args.write_coco_results:
+        results_fp = open(args.write_coco_results, 'w') if lead else True
     try:
-        r = VA.valid_batches_coco(m, meta_batches, image_batches, ev, novel_classes=novel, results_fp=results_fp)
+        if sharded:
+            r = VA.sharded_valid_coco(m, meta_batches, image_batches, ev, novel_classes=novel, results_fp=results_fp)
+        else:
+            r = VA.valid_batches_coco(m, meta_batches, image_batches, ev, novel_classes=novel, results_fp=results_fp)
     finally:
-        if results_fp is not None:
+        if results_fp is not None and results_fp is not True:
             results_fp.close()
+    if not lead:
+        return 0
     for title, key in (('all classes', 'all'), ('base classes', 'base'), ('novel classes', 'novel')):
         if r[key] is None:
             continue
