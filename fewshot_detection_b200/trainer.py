@@ -152,7 +152,9 @@ class MetaTrainer(object):
             self.adjust_learning_rate(self.processed_batches)
             self.processed_batches = self.processed_batches + 1
             loss = self.train_step(data, metax, mask, target)
-            self.losses.append(loss.detach())
+            # a graph replay returns its static loss buffer, overwritten by the next replay of that graph (and, being in
+            # the graphs' shared pool, possibly by another graph's scratch): keep a device copy of this step's value
+            self.losses.append(loss.detach().clone() if self.graphed is not None else loss.detach())
             if prof:
                 t_step += time.time() - tp
                 tp = time.time()

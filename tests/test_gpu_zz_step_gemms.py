@@ -34,6 +34,15 @@ pytestmark = pytest.mark.gpu
 
 ELEM = 1e-4            # element-wise bar, as a fraction of the same GEMM over absolute values
 SMALLK_MAX = 2304      # conv_tc.cu tc_plan: K = k*k*Cin above this (Cin % 64 == 0) runs the long-K (folded) flavour
+# float64 references are built a few images at a time, at most this many elements per tensor (1 GB): at 608x608 and
+# B = 64 the first layer's output alone is 7.6e8 elements
+CHUNK = 1 << 27
+
+
+def image_chunks(B, per_image):
+    """[(b0, b1)] image ranges of at most CHUNK elements of `per_image` each (at least one image)"""
+    step = max(1, CHUNK // max(1, per_image))
+    return [(b, min(B, b + step)) for b in range(0, B, step)]
 
 
 class _Dev(object):
@@ -94,14 +103,15 @@ def elem_ratio(got, ref, absref):
     return torch.nan_to_num(r, nan=math.inf, posinf=math.inf).max().item()
 
 
-def fwd_refs(B, H, W, Cin, cpitch, Cout, k, terms, xh, xl, wh, wl, sx, sw):
+def fwd_refs(B, H, W, Cin, cpitch, Cout, k, terms, xh, xl, wh, wl, sx, sw, b0=0, b1=None):
     """(value, |value| bound) of the products mode `terms` multiplies (float64, unscaled): hi*hi (+ x_lo*w_hi)
-    (+ x_hi*w_lo) of the fp16 planes."""
+    (+ x_hi*w_lo) of the fp16 planes; output rows of images [b0, b1)."""
+    b1 = B if b1 is None else b1
     M = B * H * W
-    X = lambda p: nchw(dev(p, M * cpitch, torch.float16).view(B, H, W, cpitch)[..., :Cin])
+    X = lambda p: nchw(dev(p, M * cpitch, torch.float16).view(B, H, W, cpitch)[b0:b1, ..., :Cin])
     Wt = lambda p: nchw(dev(p, Cout * k * k * cpitch, torch.float16).view(Cout, k, k, cpitch)[..., :Cin])
     pad = (k - 1) // 2
-    conv = lambda a, b: F.conv2d(a, b, None, 1, pad).permute(0, 2, 3, 1).reshape(M, Cout)
+    conv = lambda a, b: F.conv2d(a, b, None, 1, pad).permute(0, 2, 3, 1).reshape((b1 - b0) * H * W, Cout)
     inv = 1.0 / (sx * sw)
     Xh, Wh = X(xh), Wt(wh)
     Xa, Wa = Xh.abs(), Wh.abs()
@@ -124,11 +134,16 @@ def fwd_refs(B, H, W, Cin, cpitch, Cout, k, terms, xh, xl, wh, wl, sx, sw):
 
 def check_stats(expect, S, z, what):
     """S [rows][4][C] partial rows (sum | sum of squares | min | max) against the stored z [M][C]."""
-    zz = z.double()
     s, q = S[:, 0].double().sum(0), S[:, 1].double().sum(0)
+    s_ref, a_ref, q_ref = (torch.zeros(z.shape[1], dtype=torch.float64, device=z.device) for _ in range(3))
+    for r0 in range(0, z.shape[0], CHUNK // z.shape[1]):
+        zz = z[r0:r0 + CHUNK // z.shape[1]].double()
+        s_ref += zz.sum(0)
+        a_ref += zz.abs().sum(0)
+        q_ref += (zz * zz).sum(0)
+    del zz
     # column sums cancel (pre-BatchNorm values of both signs): bounded against the column's absolute sum
-    expect(((s - zz.sum(0)).abs() <= 1e-5 * zz.abs().sum(0) + 1e-30).all().item(), (what, 'partial sums'))
-    q_ref = (zz * zz).sum(0)
+    expect(((s - s_ref).abs() <= 1e-5 * a_ref + 1e-30).all().item(), (what, 'partial sums'))
     expect(((q - q_ref).abs() <= 1e-5 * q_ref + 1e-30).all().item(), (what, 'partial sums of squares'))
     expect(torch.equal(S[:, 2].min(0).values, z.min(0).values), (what, 'partial minima'))
     expect(torch.equal(S[:, 3].max(0).values, z.max(0).values), (what, 'partial maxima'))
@@ -145,6 +160,7 @@ class StepChecker(object):
         self.cov = set()
         self.unknown = []
         self.failures = []
+        self.first_fwd = []     # (B, H, W) of every first-layer forward
 
     def expect(self, ok, what):
         """A failed check is recorded and raised when the step has finished, so that the whole table prints."""
@@ -205,14 +221,20 @@ class StepChecker(object):
         torch.cuda.synchronize()
         sx = scale_from_amax(dev(xa, 1).item())
         sw = scale_from_amax(dev(wa, 1).item())
-        ref, absref = fwd_refs(B, H, W, Cin, cpitch, Cout, k, terms, xh, xl, wh, wl, sx, sw)
-        got = z.double()
-        if acc:
-            got -= z0.double()
-            # the stored sum z0 + conv is rounded to fp32 once: half an ulp of the stored value on top of the bar
-            absref += (0.5 * 2.0 ** -23 / ELEM) * z.double().abs()
-        e, r = rel(got, ref), elem_ratio(got, ref, absref)
-        del got, ref, absref
+        err2 = ref2 = r = 0.0
+        for b0, b1 in image_chunks(B, H * W * max(cpitch, Cout)):
+            ref, absref = fwd_refs(B, H, W, Cin, cpitch, Cout, k, terms, xh, xl, wh, wl, sx, sw, b0, b1)
+            rs = slice(b0 * H * W, b1 * H * W)
+            got = z[rs].double()
+            if acc:
+                got -= z0[rs].double()
+                # the stored sum z0 + conv is rounded to fp32 once: half an ulp of the stored value on top of the bar
+                absref += (0.5 * 2.0 ** -23 / ELEM) * z[rs].double().abs()
+            err2 += (got - ref).norm().item() ** 2
+            ref2 += ref.norm().item() ** 2
+            r = max(r, elem_ratio(got, ref, absref))
+            del got, ref, absref
+        e = math.sqrt(err2) / max(math.sqrt(ref2), 1e-300)      # rel() over the whole output
         halo = self.lib.fsdet_conv_tc_uses_halo(B, H, W, Cin, Cout, k, mode) == 1
         fold = not halo and Cin % 64 == 0 and k * k * Cin > SMALLK_MAX
         flav = 'halo' if halo else ('im2col-long' if fold else 'im2col-short')
@@ -240,23 +262,26 @@ class StepChecker(object):
         rc = self.real(fn, *a)
         torch.cuda.synchronize()
         inv = 1.0 / (scale_from_amax(dev(da, 1).item()) * scale_from_amax(dev(xa, 1).item()))
-        X = lambda p: nchw(dev(p, M * Cin, torch.float16).view(B, H, W, Cin))
-        D = lambda p: nchw(dev(p, M * Cout, torch.float16).view(B, H, W, Cout))
+        X = lambda p, b0, b1: nchw(dev(p, M * Cin, torch.float16).view(B, H, W, Cin)[b0:b1])
+        D = lambda p, b0, b1: nchw(dev(p, M * Cout, torch.float16).view(B, H, W, Cout)[b0:b1])
         wg = lambda x, d: torch.nn.grad.conv2d_weight(x, (Cout, Cin, k, k), d, 1, (k - 1) // 2).permute(0, 2, 3, 1).reshape(-1)
-        Xh, Dh = X(xh), D(dh)
-        Xl, Dl = X(xl), D(dl)
-        # what the mode multiplies: dz_hi*x_hi (+ dz_lo*x_hi) (+ dz_hi*x_lo)
-        ref = wg(Xh, Dh + Dl if terms & 1 else Dh)
-        if terms & 2:
-            ref += wg(Xl, Dh)
-        absref = wg(Xh.abs() + (Xl.abs() if terms & 2 else 0), Dh.abs() + (Dl.abs() if terms & 1 else 0))
+        ref = absref = full = 0.0
+        for b0, b1 in image_chunks(B, H * W * max(Cin, Cout)):     # a sum over images: accumulated chunk by chunk
+            Xh, Dh = X(xh, b0, b1), D(dh, b0, b1)
+            Xl, Dl = X(xl, b0, b1), D(dl, b0, b1)
+            # what the mode multiplies: dz_hi*x_hi (+ dz_lo*x_hi) (+ dz_hi*x_lo)
+            ref = ref + wg(Xh, Dh + Dl if terms & 1 else Dh)
+            if terms & 2:
+                ref = ref + wg(Xl, Dh)
+            absref = absref + wg(Xh.abs() + (Xl.abs() if terms & 2 else 0), Dh.abs() + (Dl.abs() if terms & 1 else 0))
+            full = full + wg(Xh + Xl, Dh + Dl)      # fp32-grade operands: the value the budget is measured against
+            del Xh, Xl, Dh, Dl
         got = out.double()
         e, r = rel(got, ref * inv), elem_ratio(got, ref * inv, absref * inv)
         cancel = (absref.norm() / ref.norm()).item()       # how much the sum cancels: |x|*|dz| over x*dz
         del ref, absref
-        full = wg(Xh + Xl, Dh + Dl) * inv                # fp32-grade operands: the value the budget is measured against
-        ef = rel(got, full)
-        del full, Xh, Xl, Dh, Dl, got
+        ef = rel(got, full * inv)
+        del full, got
         taps = 1 if Cin >= 128 else 2
         splits = 0
         if self.lib.fsdet_conv_tc_wgrad_workspace_floats(B, H, W, Cin, Cout, k, mode) > 0:
@@ -272,10 +297,11 @@ class StepChecker(object):
         return rc
 
     # ---- exact-fp32 first layer
-    def _first_input(self, in0, c0, in1, c1, B, H, W):
-        x = dev(in0, B * c0 * H * W).view(B, c0, H, W)
+    def _first_input(self, in0, c0, in1, c1, B, H, W, b0=0, b1=None):
+        """float64 NCHW input of images [b0, b1)"""
+        x = dev(in0, B * c0 * H * W).view(B, c0, H, W)[b0:b1]
         if c1:
-            x = torch.cat([x, dev(in1, B * c1 * H * W).view(B, c1, H, W)], 1)
+            x = torch.cat([x, dev(in1, B * c1 * H * W).view(B, c1, H, W)[b0:b1]], 1)
         return x.double()
 
     def chk_conv_first_fwd_stats(self, fn, a):
@@ -296,12 +322,19 @@ class StepChecker(object):
             S.fill_(float('nan'))
         rc = self.real(fn, *a)
         torch.cuda.synchronize()
-        x = self._first_input(in0, c0, in1, c1, B, H, W)
+        self.first_fwd.append((B, H, W))
         wt = dev(w, Cout * 36).view(Cout, 3, 3, 4)[..., :c0 + c1].permute(0, 3, 1, 2).double()
-        ref = F.conv2d(x, wt, None, 1, 1).permute(0, 2, 3, 1).reshape(M, Cout)
-        absref = F.conv2d(x.abs(), wt.abs(), None, 1, 1).permute(0, 2, 3, 1).reshape(M, Cout)
-        got = z.double()
-        e, r = rel(got, ref), elem_ratio(got, ref, absref)
+        err2 = ref2 = r = 0.0
+        for b0, b1 in image_chunks(B, H * W * Cout):
+            x = self._first_input(in0, c0, in1, c1, B, H, W, b0, b1)
+            ref = F.conv2d(x, wt, None, 1, 1).permute(0, 2, 3, 1).reshape(-1, Cout)
+            absref = F.conv2d(x.abs(), wt.abs(), None, 1, 1).permute(0, 2, 3, 1).reshape(-1, Cout)
+            got = z[b0 * H * W:b1 * H * W].double()
+            err2 += (got - ref).norm().item() ** 2
+            ref2 += ref.norm().item() ** 2
+            r = max(r, elem_ratio(got, ref, absref))
+            del x, ref, absref, got
+        e = math.sqrt(err2) / max(math.sqrt(ref2), 1e-300)
         self.cov.add('first-fwd')
         self._record('first-fwd', '%dx%dx%dx%d->%d k3' % (B, H, W, c0 + c1, Cout), 'simt', e, r)
         self.expect(e < 1e-5 and r <= 1.0, ('first-layer forward', B, H, W, c0, c1, e, r))
@@ -316,11 +349,15 @@ class StepChecker(object):
         out.fill_(float('nan'))
         rc = self.real(fn, *a)
         torch.cuda.synchronize()
-        x = torch.zeros(B, 4, H, W, dtype=torch.float64, device='cuda')
-        x[:, :c0 + c1] = self._first_input(in0, c0, in1, c1, B, H, W)
-        d = nchw(rows_view(dz, M, Cout, lddz).view(B, H, W, Cout))
         wg = lambda xx, dd: torch.nn.grad.conv2d_weight(xx, (Cout, 4, 3, 3), dd, 1, 1).permute(0, 2, 3, 1).reshape(-1)
-        ref, absref = wg(x, d), wg(x.abs(), d.abs())
+        ref = absref = 0.0
+        for b0, b1 in image_chunks(B, H * W * Cout):
+            x = torch.zeros(b1 - b0, 4, H, W, dtype=torch.float64, device='cuda')
+            x[:, :c0 + c1] = self._first_input(in0, c0, in1, c1, B, H, W, b0, b1)
+            d = nchw(rows_view(dz, M, Cout, lddz).view(B, H, W, Cout)[b0:b1])
+            ref = ref + wg(x, d)
+            absref = absref + wg(x.abs(), d.abs())
+            del x, d
         got = out.double()
         e, r = rel(got, ref), elem_ratio(got, ref, absref)
         cancel = (absref.norm() / ref.norm()).item()
@@ -405,8 +442,11 @@ class StepChecker(object):
         self.log.append(dict(kind=kind, shape=shape, flavour=flav, rel=e, ratio=r, extra=extra, full=full))
 
 
-def _run_step(side, bs, cs, seed):
-    from fewshot_detection_b200 import _lib, engine
+def run_step(side, bs, cs, seed, wrap):
+    """One eager step (forward, RegionLossV2, backward) of the full network with `bs` query images of side x side and
+    `cs` classes (support images at 416x416), while engine.call is replaced by wrap(engine.call).  Returns the head
+    output (detached), the region loss module, the label tensor and the seconds the step took."""
+    from fewshot_detection_b200 import engine
     from test_gpu_zz_configs import _batch
     from fewshot_detection_b200 import netcfg
     from fewshot_detection_b200.darknet_meta import Darknet
@@ -418,17 +458,30 @@ def _run_step(side, bs, cs, seed):
     L = m.models[len(m.models) - 1]
     L.seen = 20000
     L.verbose = False
-    chk = StepChecker(engine.call, _lib.lib)
-    engine.call = chk
+    real = engine.call
+    engine.call = wrap(real)
     t0 = time.time()
     try:
-        loss = L(m(x.cuda(), metax.cuda(), mask.cuda()), tgt)
+        out = m(x.cuda(), metax.cuda(), mask.cuda())
+        loss = L(out, tgt)
         loss.backward()
         torch.cuda.synchronize()
     finally:
-        engine.call = chk.real
+        engine.call = real
     secs = time.time() - t0
     assert torch.isfinite(loss).item()
+    return out.detach(), L, tgt, secs
+
+
+def _run_step(side, bs, cs, seed):
+    from fewshot_detection_b200 import _lib
+    chk = []
+    secs = run_step(side, bs, cs, seed, lambda real: chk.append(StepChecker(real, _lib.lib)) or chk[0])[3]
+    return report(chk[0], secs)
+
+
+def report(chk, secs):
+    """Prints the worst ratio per GEMM class of one checked step and fails if any check failed."""
     assert not chk.unknown, chk.unknown
     tc = [l for l in chk.log if l['flavour'] not in ('split',)]
     worst = {}

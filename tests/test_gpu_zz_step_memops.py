@@ -34,7 +34,7 @@ import time
 import pytest
 import torch
 
-from test_gpu_zz_step_gemms import scale_from_amax
+from test_gpu_zz_step_gemms import run_step, scale_from_amax
 
 pytestmark = pytest.mark.gpu
 
@@ -724,29 +724,14 @@ class MemChecker(object):
 
 
 def _run_step(side, bs, cs, seed):
-    from fewshot_detection_b200 import _lib, engine
-    from test_gpu_zz_configs import _batch
-    from fewshot_detection_b200 import netcfg
-    from fewshot_detection_b200.darknet_meta import Darknet
-    from seeding import seeded_init
-    m = Darknet(netcfg.darknet_dynamic_blocks(side, side), netcfg.reweighting_net_blocks())
-    seeded_init(m, seed)
-    m = m.cuda().train()
-    x, metax, mask, tgt = _batch(bs, cs, side, seed + 1)
-    L = m.models[len(m.models) - 1]
-    L.seen = 20000
-    L.verbose = False
-    chk = MemChecker(engine.call, _lib.lib)
-    engine.call = chk
-    t0 = time.time()
-    try:
-        loss = L(m(x.cuda(), metax.cuda(), mask.cuda()), tgt)
-        loss.backward()
-        torch.cuda.synchronize()
-    finally:
-        engine.call = chk.real
-    secs = time.time() - t0
-    assert torch.isfinite(loss).item()
+    from fewshot_detection_b200 import _lib
+    chk = []
+    secs = run_step(side, bs, cs, seed, lambda real: chk.append(MemChecker(real, _lib.lib)) or chk[0])[3]
+    return report(chk[0], secs)
+
+
+def report(chk, secs):
+    """Prints the worst ratio per kernel class of one checked step and fails if any check failed."""
     assert not chk.unknown, chk.unknown
     worst = {}
     for l in chk.log:
