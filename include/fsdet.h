@@ -188,9 +188,10 @@ int fsdet_debug_im2col_tile(const void* x_plane, int B, int H, int W, int C, int
  * absolute maximum of y = leaky(z*scale+shift, slope) over the tensor, derived
  * from the per-channel range of z (scale of the fp16 planes of y).  In eval mode
  * (training == 0) scale/shift come from the running statistics, stat_partial is
- * ignored and amax_y is not written.  xhat_absmax (optional, [C]): max over
+ * ignored, and amax_y and xhat_absmax (when given) are set to 0: there is no
+ * batch range to derive them from.  xhat_absmax (optional, [C]): max over
  * the batch of |(z - mean) * invstd| per channel (used by the backward pass
- * to bound max|dz|). */
+ * to bound max|dz|).  Outputs passed as NULL are not written. */
 int fsdet_bn_finalize(const float* stat_partial, int nparts, double count, const float* gamma, const float* beta,
                       float* running_mean, float* running_var, float momentum, float eps, float* mean,
                       float* invstd, float* scale, float* shift, float slope, float* amax_y, float* xhat_absmax,

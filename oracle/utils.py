@@ -142,13 +142,14 @@ def get_region_boxes_v2(output, n_models, conf_thresh, num_classes, anchors, num
                     conf_thresh, only_objectness, validation)
 
 
-def ensemble_reweights(batches, n_cls):
+def ensemble_reweights(batches, n_cls, dtype=torch.float32):
     """valid_ensemble.py:86-100: running mean of the support net's vectors per class.  `batches` yields
-    (dw float32 [n, C], clsids [n]).  Returns float32 [n_cls, C]."""
+    (dw [n, C], clsids [n]).  Returns [n_cls, C] in `dtype` (float32 as in the reference; float64 for a float64
+    oracle of the whole evaluation pass)."""
     enews = [0.0] * n_cls
     cnt = [0.0] * n_cls
     for dw, clsids in batches:
-        dw = torch.as_tensor(dw, dtype=torch.float32)
+        dw = torch.as_tensor(dw, dtype=dtype)
         for ci, c in enumerate(clsids):
             c = int(c)
             enews[c] = enews[c] * cnt[c] / (cnt[c] + 1) + dw[ci] / (cnt[c] + 1)

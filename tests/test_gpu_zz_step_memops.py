@@ -10,7 +10,10 @@ silently.
 
   fsdet_bn_finalize        mean / invstd against float64 of z (|d| <= 1e-5 std, 1e-5 invstd), scale and shift within
                            an ulp, running statistics, amax_y within an ulp of max|leaky(z*scale+shift)|, xhat_absmax
-                           bit-equal to the fp32 max|(z - mean)*invstd|; max |mean|/std per layer is reported
+                           bit-equal to the fp32 max|(z - mean)*invstd|; max |mean|/std per layer is reported.
+                           Eval mode: the running statistics as mean / 1 / sqrtf(var + eps), scale and shift within an
+                           ulp, running statistics bit-unchanged, xhat_absmax and amax_y 0 when given and untouched
+                           when not
   fsdet_bn_act_fwd         fp32 outputs bit-equal to the fp32 arithmetic (one fma, one multiply by the slope) and within
                            two roundings of float64; pooled = max of its window; fp16 planes bit-equal to the split;
                            padding zero; amax_y >= every value written
@@ -206,10 +209,7 @@ class MemChecker(object):
         b = dev(beta, C).double() if beta else torch.zeros(C, dtype=torch.float64, device='cuda')
         self.amax_of[scale] = amax_y
         if not training:
-            self.cov.add('finalize-eval')
-            self.expect(torch.equal(m, rm0) and torch.equal(inv, 1 / torch.sqrt(rv0 + eps)), ('eval finalize', C))
-            self._record('bn_finalize', 'eval C%d' % C, 'eval', 0.0)
-            return rc
+            return self._finalize_eval(fn, a, rc, m, inv, sc, sh, g, b, rm0, rv0)
         zp, ldz, B, H, W, zc = self.stat_src[stat]
         assert zc == C, (zc, C)
         z = act(zp, B, H, W, C, ldz)
@@ -255,6 +255,41 @@ class MemChecker(object):
         self.stats[mean] = (mu, var)
         self.cov.add('finalize-train')
         self._record('bn_finalize', '%dx%dx%dx%d' % (B, H, W, C), 'train', max(rmean, rinv), '  |mean|/std %.2f' % ms)
+        return rc
+
+    def _finalize_eval(self, fn, a, rc, m, inv, sc, sh, g, b, rm0, rv0):
+        """Eval mode: mean and invstd are the running statistics (invstd = 1 / sqrtf(running_var + eps), three fp32
+        roundings), scale and shift within an ulp as in training, the running statistics untouched, and nothing
+        derived from a batch range: xhat_absmax (when given) is 0, amax_y (when given) is 0.  Then the same finalize is
+        run once more into a NaN-filled [5][C] buffer with both optional outputs left out: the four coefficient rows must
+        equal the first call's and the fifth row, where xhat_absmax would go, must keep its NaN bits."""
+        stat, nparts, count, gamma, beta, rm, rv, mom, eps, mean, invstd, scale, shift, slope, amax_y, xhat, C, training, st = a
+        ok_stats = torch.equal(m, rm0) and torch.equal(inv, 1 / torch.sqrt(rv0 + eps))
+        self.expect(ok_stats, ('eval finalize mean / invstd', C))
+        r_sc = ulps(sc, g * inv.double()).max().item()
+        r_sh = ulps(sh, b - m.double() * sc.double()).max().item()
+        self.expect(r_sc <= 1, ('eval finalize scale', C, r_sc))
+        self.expect(r_sh <= 1, ('eval finalize shift', C, r_sh))
+        self.expect(torch.equal(bits(dev(rm, C)), bits(rm0)) and torch.equal(bits(dev(rv, C)), bits(rv0)),
+                    ('eval finalize wrote the running statistics', C))
+        if xhat:
+            self.expect(torch.equal(bits(dev(xhat, C)), torch.zeros(C, dtype=torch.int32, device='cuda')),
+                        ('eval finalize xhat_absmax', C))
+        if amax_y:
+            self.expect(dev(amax_y, 1).item() == 0.0, ('eval finalize amax_y', C))
+        probe = torch.full((5 * C + 1,), float('nan'), device='cuda')
+        P = lambda i: probe.data_ptr() + 4 * i * C
+        self.real(fn, stat, nparts, count, gamma, beta, rm, rv, mom, eps, P(0), P(1), P(2), P(3), slope, None, None, C,
+                  training, st)
+        torch.cuda.synchronize()
+        same = all(torch.equal(bits(probe[i * C:(i + 1) * C]), bits(t)) for i, t in enumerate((m, inv, sc, sh)))
+        self.expect(same, ('eval finalize: a second call gives other coefficients', C))
+        self.expect(torch.isnan(probe[4 * C:]).all().item(), ('eval finalize wrote an output it was not given', C))
+        self.expect(torch.equal(bits(dev(rm, C)), bits(rm0)) and torch.equal(bits(dev(rv, C)), bits(rv0)),
+                    ('eval finalize wrote the running statistics', C))
+        self.cov.add('finalize-eval')
+        self._record('bn_finalize', 'eval C%d' % C, 'eval', max(r_sc, r_sh) if ok_stats else math.inf,
+                     '  scale / shift in ulps')
         return rc
 
     # ----------------------------------------------------------------- forward
@@ -741,8 +776,9 @@ def report(chk, secs):
     print('\n%d checked calls, %.1f s (step + float64 references); worst ratio to the bar per class:' % (len(chk.log), secs))
     for k, w in sorted(worst.items()):
         print('  %-18s %-22s n=%3d  %.3f' % (k[0], k[1], w[1], w[0]))
-    print('worst |mean|/std %.2f, worst cancellation sum|du|/|sum du| %.0f, amax_bound / max|dz| in [%.2f, %.2f]' % (
-        max(chk.meanstd), max(chk.cancel), min(chk.bound_ratio), max(chk.bound_ratio)))
+    if chk.meanstd:         # a training step (an evaluation pass has no batch statistics and no backward)
+        print('worst |mean|/std %.2f, worst cancellation sum|du|/|sum du| %.0f, amax_bound / max|dz| in [%.2f, %.2f]' % (
+            max(chk.meanstd), max(chk.cancel), min(chk.bound_ratio), max(chk.bound_ratio)))
     print('coverage:', sorted(chk.cov))
     assert not chk.failures, chk.failures
     return chk
