@@ -25,6 +25,9 @@ import os
 
 import numpy as np
 
+from . import eval_pool
+from .eval_pool import DetectionPool, _ptr, check_pool_flags
+
 # coco.names (cfg.coco_classes) spells six classes the VOC way
 COCO_ALIASES = {'motorbike': 'motorcycle', 'aeroplane': 'airplane', 'sofa': 'couch', 'pottedplant': 'potted plant',
                 'diningtable': 'dining table', 'tvmonitor': 'tv'}
@@ -301,26 +304,7 @@ def device_params(p=None):
     return arrs
 
 
-def _call(name, *args):
-    from ._lib import call
-    return call(name, *args)
-
-
-def _call_size(name, *args):
-    from ._lib import lib
-    return int(getattr(lib, name)(*args))
-
-
-def _ptr(t):
-    return None if t is None else t.data_ptr()
-
-
-def _stream():
-    import torch
-    return torch.cuda.current_stream().cuda_stream
-
-
-class DeviceCocoEval(object):
+class DeviceCocoEval(DetectionPool):
     """coco_evaluate over detections that never leave the device.
 
         ev = DeviceCocoEval(classes, imagenames, load_coco_annotations(json_path, imagenames, classes))
@@ -331,18 +315,14 @@ class DeviceCocoEval(object):
     scores and boxes.  `result` matches and ranks on the device; only precision [T, R, K, A, M] and recall
     [T, K, A, M] come back, and the summary is computed from them on the host.  Every image of the set counts with
     its ground truth, added or not; each image may be added once.  `last` keeps the device arrays of the last result.
-    `merge` and `gather` combine the pools of several evaluators as voc_eval.DeviceVocEval's do (shard.py)."""
-    POOL_KEY, MERGE_FN = 'score', 'fsdet_coco_merge'
+    `merge` and `gather` combine the pools of several evaluators (eval_pool.DetectionPool)."""
+    KEY_DTYPE, MERGE_FN = 'float64', 'fsdet_coco_merge'
 
     def __init__(self, classes, imagenames, gt, device=None, params=None):
         import torch
-        self.classes, self.imagenames = list(classes), list(imagenames)
-        self.index = dict((n, k) for k, n in enumerate(self.imagenames))
-        if len(self.index) != len(self.imagenames):
-            raise ValueError('image names must be distinct')
+        DetectionPool.__init__(self, classes, imagenames, device)
         if len(gt['anns']) != len(self.imagenames):
             raise ValueError('ground truth of %d images for %d names' % (len(gt['anns']), len(self.imagenames)))
-        self.device = torch.device(device) if device is not None else torch.device('cuda', torch.cuda.current_device())
         self.params = params or Params()
         self.image_ids, self.category_ids = list(gt['image_ids']), list(gt['category_ids'])
         self.iou_thrs, self.rec_thrs, self.max_dets, self.area_rng = device_params(self.params)
@@ -353,113 +333,45 @@ class DeviceCocoEval(object):
         self.gt_box = torch.from_numpy(box).to(self.device)
         self.gt_area = torch.from_numpy(area).to(self.device)
         self.gt_crowd = torch.from_numpy(crowd).to(self.device)
-        self.group_cap = len(self.classes) * len(self.imagenames)
-        self.groups = torch.zeros(max(self.group_cap, 1), 4, dtype=torch.int32, device=self.device)
-        self.counters = torch.zeros(4, dtype=torch.int64, device=self.device)
-        self.pool_cap = 0
-        self.score = self.box = None
-        self._known, self._pending = 0, 0          # records at the last read of counters[0], upper bound added since
-        self._added = set()
-        self.last = None
 
-    @property
-    def POOL_KEY_DTYPE(self):
-        import torch
-        return torch.float64
+    def _row_bound(self, cap):
+        return min(cap, self.max_det)
 
-    def empty_like(self):
-        """A new evaluator over the same classes, image set, ground truth and device, with no detections."""
-        import copy
-        import torch
-        ev = copy.copy(self)
-        ev.groups = torch.zeros_like(self.groups)
-        ev.counters = torch.zeros_like(self.counters)
-        ev.pool_cap, ev.score, ev.box = 0, None, None
-        ev._known, ev._pending, ev._added, ev.last = 0, 0, set(), None
-        return ev
+    def _gather(self, dets, cap, image_index, image_size):
+        eval_pool._call('fsdet_coco_gather', _ptr(dets.cand), _ptr(dets.keep), _ptr(dets.keep_count), dets.N, cap,
+                        dets.H, dets.W, dets.nC, len(self.classes), _ptr(image_index), _ptr(image_size), self.max_det,
+                        _ptr(self.key), _ptr(self.box), self.pool_cap, _ptr(self.groups), self.group_cap,
+                        _ptr(self.counters), eval_pool._stream())
 
-    @staticmethod
-    def merge(evaluators):
-        """One evaluator with the detections of `evaluators` (same image set, one device) in their order."""
-        from .shard import merge_pools
-        return merge_pools(evaluators)
+    def result_file_part(self, dets, imgids, sizes):
+        """The results-json records of one added batch: detection_records' tuples."""
+        return detection_records(dets, imgids, sizes, len(self.classes), self.max_det)
 
-    def gather(self, process_group=None, dst=0, **result_kwargs):
-        """Collective: every rank's pool merged in rank order on rank `dst`, scored there once with
-        result(**result_kwargs); every rank returns that dict."""
-        from .shard import gather_result
-        return gather_result(self, process_group, dst, **result_kwargs)
-
-    def _reserve(self, bound):
-        """Room for `bound` more records.  Reads the record count (8 bytes) only when the upper bound could overflow."""
-        import torch
-        if self._known + self._pending + bound <= self.pool_cap:
-            self._pending += bound
-            return
-        self._known, self._pending = int(self.counters[0]), 0
-        if self._known + bound > self.pool_cap:
-            cap = min(max(1 << 20, 2 * self.pool_cap, 8 * bound, self._known + bound), 2 ** 31 - 1)
-            if self._known + bound > cap:
-                raise RuntimeError('more than 2^31 - 1 detections')
-            score = torch.empty(cap, dtype=torch.float64, device=self.device)
-            box = torch.empty(cap, 4, dtype=torch.float64, device=self.device)
-            if self._known:
-                score[:self._known].copy_(self.score[:self._known])
-                box[:self._known].copy_(self.box[:self._known])
-            self.score, self.box, self.pool_cap = score, box, cap
-        self._pending = bound
-
-    def add(self, dets, image_indices, sizes):
-        """dets: utils.Detections of one batch after .nms(); image_indices[b]: position in `imagenames` (or the
-        name) of image b; sizes[b] = (width, height)."""
-        import torch
-        n_cls = len(self.classes)
-        if dets.keep is None:
-            raise ValueError('Detections.nms() has not been run')
-        if dets.nC != 1:
-            raise ValueError('rows with %d class scores: only the meta detector (nC = 1) is supported' % dets.nC)
-        if dets.N % n_cls:
-            raise ValueError('%d rows are not images x %d classes' % (dets.N, n_cls))
-        bs = dets.N // n_cls
-        idx = [self.index[i] if isinstance(i, str) else int(i) for i in image_indices]
-        if len(idx) != bs or len(sizes) != bs:
-            raise ValueError('%d images in the batch, %d indices, %d sizes' % (bs, len(idx), len(sizes)))
-        for i in idx:
-            if not 0 <= i < len(self.imagenames):
-                raise IndexError('image index %d outside the image set' % i)
-            if i in self._added:
-                raise ValueError('image %s added twice' % self.imagenames[i])
-            self._added.add(i)
-        if bs == 0:
-            return
-        cap = dets.A * dets.H * dets.W
-        self._reserve(dets.N * min(cap, self.max_det))
-        idx_t = torch.tensor(idx, dtype=torch.int32).to(self.device)
-        size_t = torch.tensor([[float(w), float(h)] for w, h in sizes], dtype=torch.float64).to(self.device)
-        _call('fsdet_coco_gather', _ptr(dets.cand), _ptr(dets.keep), _ptr(dets.keep_count), dets.N, cap, dets.H, dets.W,
-              dets.nC, n_cls, _ptr(idx_t), _ptr(size_t), self.max_det, _ptr(self.score), _ptr(self.box), self.pool_cap,
-              _ptr(self.groups), self.group_cap, _ptr(self.counters), _stream())
+    def write_result_file(self, fp, parts):
+        """Write result_file_part's batches, in order, to the open file `fp` as one results json."""
+        ids = dict((n, i) for n, i in zip(self.imagenames, self.image_ids))
+        write_coco_results(fp, [r for part in parts for r in part], ids, self.category_ids)
 
     def evaluate(self):
         """Run the device evaluation; returns the dict of device tensors (also kept in `last`)."""
         import torch
-        from .voc_eval import check_pool_flags
         n_det, n_groups, _, overflow = [int(v) for v in self.counters.cpu()]
         check_pool_flags(overflow)
         n_cls, n_img, dev = len(self.classes), len(self.imagenames), self.device
         T, R, A, M = len(self.iou_thrs), len(self.rec_thrs), len(self.area_rng), len(self.max_dets)
-        ws = torch.empty(max(1, _call_size('fsdet_coco_workspace_bytes', n_det, self.n_gt, n_cls, n_img)),
+        ws = torch.empty(max(1, eval_pool._call_size('fsdet_coco_workspace_bytes', n_det, self.n_gt, n_cls, n_img)),
                          dtype=torch.uint8, device=dev)
         out = dict(dt_flags=torch.empty(A, max(n_det, 1), dtype=torch.int32, device=dev),
                    order=torch.empty(max(n_det, 1), dtype=torch.int32, device=dev),
                    precision=torch.empty(T, R, n_cls, A, M, dtype=torch.float64, device=dev),
                    recall=torch.empty(T, n_cls, A, M, dtype=torch.float64, device=dev))
-        _call('fsdet_coco_evaluate', _ptr(self.score) if n_det else None, _ptr(self.box) if n_det else None, n_det,
-              _ptr(self.groups), n_groups, _ptr(self.gt_ptr), _ptr(self.gt_box) if self.n_gt else None,
-              _ptr(self.gt_area) if self.n_gt else None, _ptr(self.gt_crowd) if self.n_gt else None, self.n_gt, n_cls,
-              n_img, self.iou_thrs.ctypes.data, self.rec_thrs.ctypes.data, self.max_dets.ctypes.data,
-              self.area_rng.ctypes.data, _ptr(ws), ws.numel(), _ptr(out['dt_flags']), _ptr(out['order']),
-              _ptr(out['precision']), _ptr(out['recall']), _stream())
+        eval_pool._call('fsdet_coco_evaluate', _ptr(self.key) if n_det else None, _ptr(self.box) if n_det else None,
+                        n_det, _ptr(self.groups), n_groups, _ptr(self.gt_ptr), _ptr(self.gt_box) if self.n_gt else None,
+                        _ptr(self.gt_area) if self.n_gt else None, _ptr(self.gt_crowd) if self.n_gt else None,
+                        self.n_gt, n_cls, n_img, self.iou_thrs.ctypes.data, self.rec_thrs.ctypes.data,
+                        self.max_dets.ctypes.data, self.area_rng.ctypes.data, _ptr(ws), ws.numel(),
+                        _ptr(out['dt_flags']), _ptr(out['order']), _ptr(out['precision']), _ptr(out['recall']),
+                        eval_pool._stream())
         self.last = out
         return out
 

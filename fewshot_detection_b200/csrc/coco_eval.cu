@@ -35,48 +35,8 @@ struct CocoParams {
 };
 
 // ---- gather: one batch of Detections (after NMS) -> records + group descriptors ---------------------------------
-// counters (int64): [0] records in the pool, [1] groups, [2] first group of the last batch, [3] overflow flag.
-__global__ void __launch_bounds__(kVocThreads) coco_gather_plan_kernel(const int32_t* __restrict__ keep_count, int N,
-                                                                       int n_cls, const int32_t* __restrict__ image_index,
-                                                                       int max_det, long long pool_cap,
-                                                                       int32_t* __restrict__ groups, int group_cap,
-                                                                       long long* counters) {
-    __shared__ unsigned long long s[kVocThreads];
-    __shared__ int s_ok;
-    const long long pool0 = counters[0], group0 = counters[1];
-    unsigned long long sum = 0;
-    for (int r = threadIdx.x; r < N; r += kVocThreads) sum += (unsigned long long)min(max(keep_count[r], 0), max_det);
-    unsigned long long total;
-    voc_block_scan(sum, s, total);
-    if (threadIdx.x == 0)
-        s_ok = counters[3] == 0 && pool0 + (long long)total <= pool_cap && group0 + N <= (long long)group_cap;
-    __syncthreads();
-    if (!s_ok) {
-        if (threadIdx.x == 0) counters[3] = 1;
-        return;
-    }
-    unsigned long long base = 0;
-    for (int r0 = 0; r0 < N; r0 += kVocThreads) {
-        const int r = r0 + threadIdx.x;
-        const int c = r < N ? min(max(keep_count[r], 0), max_det) : 0;
-        unsigned long long chunk;
-        const unsigned long long pre = voc_block_scan((unsigned long long)c, s, chunk);
-        if (r < N) {
-            int32_t* g = groups + (group0 + r) * 4;
-            g[0] = (int32_t)(pool0 + (long long)(base + pre));
-            g[1] = c;
-            g[2] = image_index[r / n_cls];
-            g[3] = r % n_cls;
-        }
-        base += chunk;
-    }
-    if (threadIdx.x == 0) {
-        counters[0] = pool0 + (long long)total;
-        counters[1] = group0 + N;
-        counters[2] = group0;
-    }
-}
-
+// eval_gather_plan_kernel (eval_sort.cuh) lays out the batch's groups and counters, each row cut to max_det records;
+// coco_gather_rows_kernel fills the records.
 __device__ __forceinline__ double coco_score(const float* __restrict__ cand, const int32_t* __restrict__ keep, int r,
                                              int cap, int j) {
     const float* v = cand + ((size_t)r * cap + keep[(size_t)r * cap + j]) * 8;
@@ -420,7 +380,7 @@ static int coco_gather_impl(const float* cand, const int32_t* keep, const int32_
                             double* score, double* box, long long pool_cap, int32_t* groups, int group_cap,
                             long long* counters, cudaStream_t st) {
     (void)st;
-    VOC_LAUNCH(1, kVocThreads, coco_gather_plan_kernel, keep_count, N, n_cls, image_index, max_det, pool_cap, groups,
+    VOC_LAUNCH(1, kVocThreads, eval_gather_plan_kernel, keep_count, N, n_cls, image_index, max_det, pool_cap, groups,
                group_cap, counters);
     VOC_CHECK("coco_gather_plan");
     VOC_LAUNCH(N, kVocThreads, coco_gather_rows_kernel, cand, keep, keep_count, cap, H, W, n_cls, max_det, image_size,

@@ -1,5 +1,5 @@
-// Block scan, stable LSD radix sort and uint64 prefix sums shared by the device evaluators (voc_eval.cu, coco_eval.cu),
-// with the launch macros that run them either on the device or under host emulation (tools/host_emul).
+// Block scan, stable LSD radix sort, uint64 prefix sums, the gather plan and the pool merge shared by the device
+// evaluators (voc_eval.cu, coco_eval.cu), with the launch macros that run them either on the device or under host emulation (tools/host_emul).
 // Internal linkage: every evaluator translation unit gets its own copy of the kernels.
 #pragma once
 #include "common.cuh"
@@ -136,7 +136,55 @@ __global__ void __launch_bounds__(kVocThreads) voc_scan_apply_kernel(unsigned lo
     }
 }
 
-// ---- merge: the pools of several accumulators (one per rank of a sharded evaluation) -> one pool -----------------
+// ---- gather plan: one batch of Detections (after NMS) -> group descriptors --------------------------------------
+// counters (int64): [0] records in the pool, [1] groups, [2] first group of the last batch, [3] overflow flag.
+// One block: the batch's rows get consecutive groups and record ranges (row order = result-file order per class); row r
+// takes min(keep_count[r], row_limit) records.  A batch that does not fit, or follows an overflow, sets the flag and
+// writes nothing.
+__global__ void __launch_bounds__(kVocThreads) eval_gather_plan_kernel(const int32_t* __restrict__ keep_count, int N,
+                                                                       int n_cls, const int32_t* __restrict__ image_index,
+                                                                       int row_limit, long long pool_cap,
+                                                                       int32_t* __restrict__ groups, int group_cap,
+                                                                       long long* counters) {
+    __shared__ unsigned long long s[kVocThreads];
+    __shared__ int s_ok;
+    const long long pool0 = counters[0], group0 = counters[1];
+    // pass 1: total, to decide whether the batch fits
+    unsigned long long sum = 0;
+    for (int r = threadIdx.x; r < N; r += kVocThreads) sum += (unsigned long long)min(max(keep_count[r], 0), row_limit);
+    unsigned long long total;
+    voc_block_scan(sum, s, total);
+    if (threadIdx.x == 0)
+        s_ok = counters[3] == 0 && pool0 + (long long)total <= pool_cap && group0 + N <= (long long)group_cap;
+    __syncthreads();
+    if (!s_ok) {
+        if (threadIdx.x == 0) counters[3] = 1;
+        return;
+    }
+    // pass 2: ordered ranges
+    unsigned long long base = 0;
+    for (int r0 = 0; r0 < N; r0 += kVocThreads) {
+        const int r = r0 + threadIdx.x;
+        const int c = r < N ? min(max(keep_count[r], 0), row_limit) : 0;
+        unsigned long long chunk;
+        const unsigned long long pre = voc_block_scan((unsigned long long)c, s, chunk);
+        if (r < N) {
+            int32_t* g = groups + (group0 + r) * 4;
+            g[0] = (int32_t)(pool0 + (long long)(base + pre));
+            g[1] = c;
+            g[2] = image_index[r / n_cls];
+            g[3] = r % n_cls;
+        }
+        base += chunk;
+    }
+    if (threadIdx.x == 0) {
+        counters[0] = pool0 + (long long)total;
+        counters[1] = group0 + N;
+        counters[2] = group0;
+    }
+}
+
+// ---- merge:the pools of several accumulators (one per rank of a sharded evaluation) -> one pool -----------------
 // Source s holds counters src_counters[s][4], records [s * src_pool_stride, + its record count) and groups
 // [s * src_group_stride, + its group count).  The merged pool takes the sources in order: records are copied, each
 // group's first record is rebased.  Error bits in counters[3]: overflow (a source overflowed, or the destination is

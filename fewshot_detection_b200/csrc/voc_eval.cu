@@ -61,50 +61,7 @@ __global__ void voc_round6_kernel(const double* __restrict__ x, double* __restri
 }
 
 // ---- gather: one batch of Detections (after NMS) -> records + group descriptors ---------------------------------
-// counters (int64): [0] records in the pool, [1] groups, [2] first group of the last batch, [3] overflow flag.
-
-// One block: the batch's rows get consecutive groups and record ranges (row order = result-file order per class).
-__global__ void __launch_bounds__(kVocThreads) voc_gather_plan_kernel(const int32_t* __restrict__ keep_count, int N,
-                                                                      int n_cls, const int32_t* __restrict__ image_index,
-                                                                      long long pool_cap, int32_t* __restrict__ groups,
-                                                                      int group_cap, long long* counters) {
-    __shared__ unsigned long long s[kVocThreads];
-    __shared__ int s_ok;
-    const long long pool0 = counters[0], group0 = counters[1];
-    // pass 1: total, to decide whether the batch fits
-    unsigned long long sum = 0;
-    for (int r = threadIdx.x; r < N; r += kVocThreads) sum += (unsigned long long)max(keep_count[r], 0);
-    unsigned long long total;
-    voc_block_scan(sum, s, total);
-    if (threadIdx.x == 0)
-        s_ok = counters[3] == 0 && pool0 + (long long)total <= pool_cap && group0 + N <= (long long)group_cap;
-    __syncthreads();
-    if (!s_ok) {
-        if (threadIdx.x == 0) counters[3] = 1;
-        return;
-    }
-    // pass 2: ordered ranges
-    unsigned long long base = 0;
-    for (int r0 = 0; r0 < N; r0 += kVocThreads) {
-        const int r = r0 + threadIdx.x;
-        const int c = r < N ? max(keep_count[r], 0) : 0;
-        unsigned long long chunk;
-        const unsigned long long pre = voc_block_scan((unsigned long long)c, s, chunk);
-        if (r < N) {
-            int32_t* g = groups + (group0 + r) * 4;
-            g[0] = (int32_t)(pool0 + (long long)(base + pre));
-            g[1] = c;
-            g[2] = image_index[r / n_cls];
-            g[3] = r % n_cls;
-        }
-        base += chunk;
-    }
-    if (threadIdx.x == 0) {
-        counters[0] = pool0 + (long long)total;
-        counters[1] = group0 + N;
-        counters[2] = group0;
-    }
-}
+// eval_gather_plan_kernel (eval_sort.cuh) lays out the batch's groups and counters; the kernel below fills the records.
 
 // One block per row: the kept boxes of row r in survivor order, as valid.detection_lines computes and prints them:
 // box = [xs/W, ys/H, ws/W, hs/H, det, cls] (float64 of the float32 candidate), x1 = (box[0] - box[2]/2.0) * width, ...,
@@ -367,8 +324,8 @@ static int voc_gather_impl(const float* cand, const int32_t* keep, const int32_t
                            double* box, long long pool_cap, int32_t* groups, int group_cap, long long* counters,
                            cudaStream_t st) {
     (void)st;
-    VOC_LAUNCH(1, kVocThreads, voc_gather_plan_kernel, keep_count, N, n_cls, image_index, pool_cap, groups, group_cap,
-               counters);
+    VOC_LAUNCH(1, kVocThreads, eval_gather_plan_kernel, keep_count, N, n_cls, image_index, cap, pool_cap, groups,
+               group_cap, counters);                  // a row keeps at most cap boxes: the limit never binds
     VOC_CHECK("voc_gather_plan");
     VOC_LAUNCH(N, kVocThreads, voc_gather_rows_kernel, cand, keep, cap, H, W, n_cls, image_size, groups, counters,
                rank_key, box);

@@ -4,10 +4,9 @@ Each rank runs a contiguous block of whole batches (`shard_range`), so every bat
 process would have run, with the same size and contents.  Ranks that run batches in rank order therefore see the
 sample sequence of the single process cut into consecutive pieces, and the pieces are put back together in rank
 order: the support vectors before the running mean (valid.sharded_ensemble_dynamic_weights) and the detection pools
-of the device evaluators before scoring (`merge_pools`, `gather_pools`: csrc/voc_eval.cu / coco_eval.cu
-fsdet_*_merge).
+of the device evaluators before scoring (eval_pool.DetectionPool.gather).  This module holds the shard plan and the
+collectives they use.
 """
-from ._lib import call, ptr, lib
 
 
 def shard_range(n_items, batch_size, world, rank):
@@ -45,52 +44,6 @@ def all_gather_padded(t, rows, process_group=None):
     return out.view((world, rows) + tuple(t.shape[1:]))
 
 
-def _pool(ev):
-    """The key (rank_key or score), box and group tensors of a DeviceVocEval / DeviceCocoEval."""
-    return getattr(ev, ev.POOL_KEY), ev.box, ev.groups
-
-
-def _merge_stacked(dst, counters, key, box, groups, total):
-    """Write the stacked pools of R sources (counters [R, 4] int64, key [R, P], box [R, P, 4], groups [R, G, 4], all
-    on dst's device) into the empty evaluator `dst`; `total` = the sum of the sources' record counts."""
-    import torch
-    n_src, stride_p, stride_g = int(counters.size(0)), int(key.size(1)), int(groups.size(1))
-    dst._reserve(total)
-    ws = torch.empty(int(lib.fsdet_eval_merge_workspace_bytes(n_src, len(dst.imagenames))), dtype=torch.uint8,
-                     device=dst.device)
-    dkey, dbox, dgroups = _pool(dst)
-    call(dst.MERGE_FN, n_src, ptr(counters), ptr(key), ptr(box), stride_p, ptr(groups), stride_g, len(dst.imagenames),
-         ptr(ws), ws.numel(), ptr(dkey), ptr(dbox), dst.pool_cap, ptr(dgroups), dst.group_cap, ptr(dst.counters),
-         torch.cuda.current_stream(dst.device).cuda_stream)
-    return dst
-
-
-def merge_pools(evaluators):
-    """One evaluator holding the detections of `evaluators` (same class, image set and device), in their order."""
-    import torch
-    evs = list(evaluators)
-    if not evs:
-        raise ValueError('nothing to merge')
-    counters = torch.stack([e.counters for e in evs])
-    host = counters.cpu()
-    P, G = max(1, int(host[:, 0].max())), max(1, int(host[:, 1].max()))
-    key = torch.zeros(len(evs), P, dtype=evs[0].POOL_KEY_DTYPE, device=evs[0].device)
-    box = torch.zeros(len(evs), P, 4, dtype=torch.float64, device=evs[0].device)
-    groups = torch.zeros(len(evs), G, 4, dtype=torch.int32, device=evs[0].device)
-    for r, e in enumerate(evs):
-        n, g = int(host[r, 0]), int(host[r, 1])
-        ek, eb, eg = _pool(e)
-        if n:
-            key[r, :n].copy_(ek[:n])
-            box[r, :n].copy_(eb[:n])
-        if g:
-            groups[r, :g].copy_(eg[:g])
-    dst = evs[0].empty_like()
-    for e in evs:
-        dst._added |= e._added
-    return _merge_stacked(dst, counters, key, box, groups, int(host[:, 0].sum()))
-
-
 def gather_padded(t, rows, process_group=None, dst=0):
     """Every rank's `t` ([n_r, ...], n_r <= rows), zero padded, as one [world, rows, ...] tensor on rank `dst` (a
     rank of the group); None on the other ranks.  Only `dst` holds the world's buffers."""
@@ -116,42 +69,3 @@ def rank0_first(fn, process_group=None):
     if rank == 0:
         dist.barrier(group=process_group)
     return r
-
-
-def gather_pools(ev, process_group=None, dst=0):
-    """Collective over `process_group`: every rank's pool, in rank order, merged into a new evaluator on rank `dst`
-    (a rank of the group).  Returns it on `dst`, None elsewhere.  The counts are all-gathered first; the padded
-    records and groups then go to `dst` alone."""
-    import torch
-    world, rank = group_info(process_group)
-    counters = all_gather_padded(ev.counters.reshape(1, 4), 1, process_group).reshape(world, 4)
-    host = counters.cpu()
-    P, G = max(1, int(host[:, 0].max())), max(1, int(host[:, 1].max()))
-    n, g = int(host[rank, 0]), int(host[rank, 1])
-    ek, eb, eg = _pool(ev)
-    empty_key = torch.zeros(0, dtype=ev.POOL_KEY_DTYPE, device=ev.device)
-    key = gather_padded(ek[:n] if n else empty_key, P, process_group, dst)
-    box = gather_padded(eb[:n] if n else torch.zeros(0, 4, dtype=torch.float64, device=ev.device), P, process_group,
-                        dst)
-    groups = gather_padded(eg[:g], G, process_group, dst)
-    if rank != dst:
-        return None
-    return _merge_stacked(ev.empty_like(), counters, key, box, groups, int(host[:, 0].sum()))
-
-
-def gather_result(ev, process_group=None, dst=0, **result_kwargs):
-    """gather_pools, `result(**result_kwargs)` once on `dst`, and the small result dict broadcast to every rank.  An
-    error of the scoring on `dst` (for example a pool flag) is broadcast instead and raised on every rank."""
-    import torch.distributed as dist
-    merged = gather_pools(ev, process_group, dst)
-    box = [None]
-    if merged is not None:
-        try:
-            box = [('ok', merged.result(**result_kwargs))]
-        except Exception as e:                        # every rank raises, none waits in the broadcast
-            box = [('error', '%s: %s' % (type(e).__name__, e))]
-    dist.broadcast_object_list(box, src=global_rank(process_group, dst), group=process_group)
-    status, value = box[0]
-    if status == 'error':
-        raise RuntimeError(value)
-    return value

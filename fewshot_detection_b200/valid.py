@@ -10,9 +10,11 @@ same files:
     dets = detect(m, data, dw, n_cls)                                    # Detections, NMS done, still on the device
     write_detections(fps, dets, imgids, sizes, n_cls)                    # 'imgid prob x1 y1 x2 y2' per class file
 
-or, without the files, scores them where they are (voc_eval.DeviceVocEval, csrc/voc_eval.cu):
+or, without the files, scores them where they are (voc_eval.DeviceVocEval, coco_eval.DeviceCocoEval):
 
     evaluator.add(dets, imgids, sizes); ...; evaluator.result()          # the dict voc_eval.mean_ap returns
+
+`score_batches` runs that whole pass, in one process or sharded over the ranks of a process group.
 
 CUDA only (libfsdet.so); no host fallback.
 """
@@ -137,46 +139,45 @@ def valid_batches(m, meta_batches, image_batches, class_names, prefix, outfile):
     return dynamic_weights
 
 
-def valid_batches_ap(m, meta_batches, image_batches, evaluator, use_07_metric=True, novel_classes=(), fps=None):
-    """valid_batches followed by voc_eval.mean_ap, with the detections kept on the device: `evaluator` is a
-    voc_eval.DeviceVocEval over the evaluated image set, `image_batches` yields (data, imgids, sizes) with imgids
-    names of that set.  Returns mean_ap's dict.  fps (optional, one open file per class) also receives the result
-    lines valid_batches would write."""
+def score_batches(m, support_batches, image_batches, evaluator, out=None, sharded=False, process_group=None, dst=0,
+                  **result_kwargs):
+    """valid_batches scored on the device: `evaluator` is a voc_eval.DeviceVocEval or coco_eval.DeviceCocoEval over
+    the evaluated image set, `support_batches` are as ensemble_dynamic_weights' meta_batches, `image_batches` yields
+    (data, imgids, sizes) with imgids names of that set.  Returns evaluator.result(**result_kwargs): mean_ap's dict
+    (use_07_metric=, novel_classes=, curves=) or coco_evaluate's (novel_classes=).
+
+    out (optional) also receives the result files of the same detections, copied to the host for them: for VOC the
+    per-class files valid_batches writes (a list of open files), for COCO the standard results json (an open file).
+
+    sharded=True: collective over `process_group`, each rank running its own block of the single-process support and
+    query batches (shard.shard_range).  The pools are merged in rank order and scored once on rank `dst`; every rank
+    returns the single-process dict.  `out` is open on `dst` and True on the other ranks, whose parts go to `dst`,
+    which writes every rank's in rank order: the single-process files.  None on every rank for no files."""
     n_cls = len(evaluator.classes)
     m.eval()
-    dynamic_weights = ensemble_dynamic_weights(m, meta_batches, n_cls)
+    if sharded:
+        dynamic_weights = sharded_ensemble_dynamic_weights(m, support_batches, n_cls, process_group)
+    else:
+        dynamic_weights = ensemble_dynamic_weights(m, support_batches, n_cls)
     dev = next(m.parameters()).device
+    parts = []
     for data, imgids, sizes in image_batches:
         dets = detect(m, data.to(dev), dynamic_weights, n_cls)
         evaluator.add(dets, imgids, sizes)
-        if fps is not None:
-            write_detections(fps, dets, imgids, sizes, n_cls)
-    return evaluator.result(use_07_metric, novel_classes)
+        if out is not None:
+            parts.append(evaluator.result_file_part(dets, imgids, sizes))
+    if out is not None:
+        if sharded:
+            ranks = gather_to(parts, process_group, dst)                # None except on `dst`
+            parts = None if ranks is None else [p for r in ranks for p in r]
+        if parts is not None:
+            evaluator.write_result_file(out, parts)
+    if sharded:
+        return evaluator.gather(process_group, dst, **result_kwargs)
+    return evaluator.result(**result_kwargs)
 
 
-def valid_batches_coco(m, meta_batches, image_batches, evaluator, novel_classes=(), results_fp=None):
-    """valid_batches scored with the COCO box metric on the device: `evaluator` is a coco_eval.DeviceCocoEval over the
-    evaluated image set, `image_batches` yields (data, imgids, sizes) with imgids names of that set.  Returns
-    coco_eval.coco_evaluate's dict.  results_fp (optional, an open text file) also receives the standard results json
-    of the same detections (copied to the host for it)."""
-    from . import coco_eval
-    n_cls = len(evaluator.classes)
-    m.eval()
-    dynamic_weights = ensemble_dynamic_weights(m, meta_batches, n_cls)
-    dev = next(m.parameters()).device
-    records = []
-    for data, imgids, sizes in image_batches:
-        dets = detect(m, data.to(dev), dynamic_weights, n_cls)
-        evaluator.add(dets, imgids, sizes)
-        if results_fp is not None:
-            records.extend(coco_eval.detection_records(dets, imgids, sizes, n_cls, evaluator.max_det))
-    if results_fp is not None:
-        ids = dict((n, i) for n, i in zip(evaluator.imagenames, evaluator.image_ids))
-        coco_eval.write_coco_results(results_fp, records, ids, evaluator.category_ids)
-    return evaluator.result(novel_classes)
-
-
-# ---- the same passes sharded over the ranks of a process group (shard.py) -------------------------------------------
+# ---- the sharded pieces of the pass (shard.py) ----------------------------------------------------------------------
 def sharded_ensemble_dynamic_weights(m, meta_batches, n_cls, process_group=None):
     """ensemble_dynamic_weights over every rank's support batches, in rank order.  `meta_batches` are this rank's
     block of the single-process batches (shard.shard_range).  Each rank runs the reweighting net on its own batches;
@@ -224,57 +225,3 @@ def gather_to(obj, process_group, dst):
     out = [None] * world if rank == dst else None
     dist.gather_object(obj, out, dst=global_rank(process_group, dst), group=process_group)
     return out
-
-
-def sharded_valid_ap(m, support_batches, image_batches, evaluator, use_07_metric=True, novel_classes=(), fps=None,
-                     process_group=None, dst=0):
-    """valid_batches_ap with this rank's block of the support and query batches (shard.shard_range); collective over
-    `process_group`.  The pools are merged in rank order and scored once on rank `dst`; every rank returns mean_ap's
-    dict, equal to the single-process one.  fps: the per-class result files, open on `dst`, and True on the other
-    ranks (their lines go to `dst`, which writes every rank's lines in rank order: the single-process files); None on
-    every rank for no files."""
-    from .shard import group_info
-    _, rank = group_info(process_group)
-    n_cls = len(evaluator.classes)
-    m.eval()
-    dynamic_weights = sharded_ensemble_dynamic_weights(m, support_batches, n_cls, process_group)
-    dev = next(m.parameters()).device
-    lines = dict((i, []) for i in range(n_cls))
-    for data, imgids, sizes in image_batches:
-        dets = detect(m, data.to(dev), dynamic_weights, n_cls)
-        evaluator.add(dets, imgids, sizes)
-        if fps is not None:
-            for i, l in detection_lines(dets, imgids, sizes, n_cls).items():
-                lines[i].extend(l)
-    if fps is not None:
-        parts = gather_to(lines, process_group, dst)
-        if rank == dst:
-            for part in parts:
-                for i in range(n_cls):
-                    fps[i].writelines(part[i])
-    return evaluator.gather(process_group, dst, use_07_metric=use_07_metric, novel_classes=novel_classes)
-
-
-def sharded_valid_coco(m, support_batches, image_batches, evaluator, novel_classes=(), results_fp=None,
-                       process_group=None, dst=0):
-    """valid_batches_coco sharded as sharded_valid_ap.  results_fp: the results json, open on `dst`, True on the
-    other ranks; None on every rank for no file."""
-    from . import coco_eval
-    from .shard import group_info
-    _, rank = group_info(process_group)
-    n_cls = len(evaluator.classes)
-    m.eval()
-    dynamic_weights = sharded_ensemble_dynamic_weights(m, support_batches, n_cls, process_group)
-    dev = next(m.parameters()).device
-    records = []
-    for data, imgids, sizes in image_batches:
-        dets = detect(m, data.to(dev), dynamic_weights, n_cls)
-        evaluator.add(dets, imgids, sizes)
-        if results_fp is not None:
-            records.extend(coco_eval.detection_records(dets, imgids, sizes, n_cls, evaluator.max_det))
-    if results_fp is not None:
-        parts = gather_to(records, process_group, dst)
-        if rank == dst:
-            ids = dict((n, i) for n, i in zip(evaluator.imagenames, evaluator.image_ids))
-            coco_eval.write_coco_results(results_fp, [r for p in parts for r in p], ids, evaluator.category_ids)
-    return evaluator.gather(process_group, dst, novel_classes=novel_classes)

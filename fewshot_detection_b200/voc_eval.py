@@ -19,6 +19,9 @@ import xml.etree.ElementTree as ET
 
 import numpy as np
 
+from . import eval_pool
+from .eval_pool import DetectionPool, _ptr, check_pool_flags
+
 
 def parse_rec(filename):
     """One VOC annotation file -> list of {'name', 'pose', 'truncated', 'difficult', 'bbox': [xmin, ymin, xmax, ymax]}."""
@@ -165,21 +168,7 @@ def gt_tables(classes, imagenames, recs):
             np.array(diff, dtype=np.uint8))
 
 
-def _call(name, *args):
-    from ._lib import call
-    return call(name, *args)
-
-
-def _ptr(t):
-    return None if t is None else t.data_ptr()
-
-
-def _stream():
-    import torch
-    return torch.cuda.current_stream().cuda_stream
-
-
-class DeviceVocEval(object):
+class DeviceVocEval(DetectionPool):
     """voc_eval / mean_ap over detections that never leave the device.
 
         ev = DeviceVocEval(classes, imagenames, load_annotations(annopath, imagenames, cachedir))
@@ -195,109 +184,34 @@ class DeviceVocEval(object):
 
     Sharded over ranks (shard.py): each rank adds its own contiguous block of batches, then `gather` merges the pools
     in rank order on one rank and scores them there; `merge` does the same for several evaluators on one device."""
-    POOL_KEY, MERGE_FN = 'rank_key', 'fsdet_voc_merge'
+    KEY_DTYPE, MERGE_FN = 'int32', 'fsdet_voc_merge'
 
     def __init__(self, classes, imagenames, recs, device=None, ovthresh=0.5):
         import torch
-        self.classes, self.imagenames = list(classes), list(imagenames)
-        self.index = dict((n, k) for k, n in enumerate(self.imagenames))
-        if len(self.index) != len(self.imagenames):
-            raise ValueError('image names must be distinct')
-        self.device = torch.device(device) if device is not None else torch.device('cuda', torch.cuda.current_device())
+        DetectionPool.__init__(self, classes, imagenames, device)
         self.ovthresh = float(ovthresh)
         ptr, boxes, diff = gt_tables(self.classes, self.imagenames, recs)
         self.n_gt = int(len(diff))
         self.gt_ptr = torch.from_numpy(ptr).to(self.device)
         self.gt_box = torch.from_numpy(boxes).to(self.device)
         self.gt_difficult = torch.from_numpy(diff).to(self.device)
-        self.group_cap = len(self.classes) * len(self.imagenames)
-        self.groups = torch.zeros(max(self.group_cap, 1), 4, dtype=torch.int32, device=self.device)
-        self.counters = torch.zeros(4, dtype=torch.int64, device=self.device)
-        self.pool_cap = 0
-        self.rank_key = self.box = None
-        self._known, self._pending = 0, 0          # records at the last read of counters[0], upper bound added since
-        self._added = set()
-        self.last = None
 
-    @property
-    def POOL_KEY_DTYPE(self):
-        import torch
-        return torch.int32
+    def _gather(self, dets, cap, image_index, image_size):
+        eval_pool._call('fsdet_voc_gather', _ptr(dets.cand), _ptr(dets.keep), _ptr(dets.keep_count), dets.N, cap,
+                        dets.H, dets.W, dets.nC, len(self.classes), _ptr(image_index), _ptr(image_size), _ptr(self.key),
+                        _ptr(self.box), self.pool_cap, _ptr(self.groups), self.group_cap, _ptr(self.counters),
+                        eval_pool._stream())
 
-    def empty_like(self):
-        """A new evaluator over the same classes, image set, ground truth and device, with no detections."""
-        import copy
-        import torch
-        ev = copy.copy(self)
-        ev.groups = torch.zeros_like(self.groups)
-        ev.counters = torch.zeros_like(self.counters)
-        ev.pool_cap, ev.rank_key, ev.box = 0, None, None
-        ev._known, ev._pending, ev._added, ev.last = 0, 0, set(), None
-        return ev
+    def result_file_part(self, dets, imgids, sizes):
+        """The result-file lines of one added batch: valid.detection_lines' {class index: [lines]}."""
+        from .valid import detection_lines
+        return detection_lines(dets, imgids, sizes, len(self.classes))
 
-    @staticmethod
-    def merge(evaluators):
-        """One evaluator with the detections of `evaluators` (same image set, one device) in their order: the pool a
-        single evaluator would hold had it been given their batches in that order."""
-        from .shard import merge_pools
-        return merge_pools(evaluators)
-
-    def gather(self, process_group=None, dst=0, **result_kwargs):
-        """Collective: the pools of every rank of `process_group` merged in rank order on rank `dst`, scored there
-        once with result(**result_kwargs); every rank returns that dict."""
-        from .shard import gather_result
-        return gather_result(self, process_group, dst, **result_kwargs)
-
-    def _reserve(self, bound):
-        """Room for `bound` more records.  Reads the record count (8 bytes) only when the upper bound could overflow."""
-        import torch
-        if self._known + self._pending + bound <= self.pool_cap:
-            self._pending += bound
-            return
-        self._known, self._pending = int(self.counters[0]), 0
-        if self._known + bound > self.pool_cap:
-            cap = max(1 << 20, 2 * self.pool_cap, 8 * bound, self._known + bound)
-            cap = min(cap, 2 ** 31 - 1)
-            if self._known + bound > cap:
-                raise RuntimeError('more than 2^31 - 1 detections')
-            key = torch.empty(cap, dtype=torch.int32, device=self.device)
-            box = torch.empty(cap, 4, dtype=torch.float64, device=self.device)
-            if self._known:
-                key[:self._known].copy_(self.rank_key[:self._known])
-                box[:self._known].copy_(self.box[:self._known])
-            self.rank_key, self.box, self.pool_cap = key, box, cap
-        self._pending = bound
-
-    def add(self, dets, image_indices, sizes):
-        """dets: utils.Detections of one batch after .nms(); image_indices[b]: position in `imagenames` (or the
-        name) of image b; sizes[b] = (width, height)."""
-        import torch
-        n_cls = len(self.classes)
-        if dets.keep is None:
-            raise ValueError('Detections.nms() has not been run')
-        if dets.nC != 1:
-            raise ValueError('rows with %d class scores: only the meta detector (nC = 1) is supported' % dets.nC)
-        if dets.N % n_cls:
-            raise ValueError('%d rows are not images x %d classes' % (dets.N, n_cls))
-        bs = dets.N // n_cls
-        idx = [self.index[i] if isinstance(i, str) else int(i) for i in image_indices]
-        if len(idx) != bs or len(sizes) != bs:
-            raise ValueError('%d images in the batch, %d indices, %d sizes' % (bs, len(idx), len(sizes)))
-        for i in idx:
-            if not 0 <= i < len(self.imagenames):
-                raise IndexError('image index %d outside the image set' % i)
-            if i in self._added:
-                raise ValueError('image %s added twice' % self.imagenames[i])
-            self._added.add(i)
-        if bs == 0:
-            return
-        cap = dets.A * dets.H * dets.W
-        self._reserve(dets.N * cap)
-        idx_t = torch.tensor(idx, dtype=torch.int32).to(self.device)
-        size_t = torch.tensor([[float(w), float(h)] for w, h in sizes], dtype=torch.float64).to(self.device)
-        _call('fsdet_voc_gather', _ptr(dets.cand), _ptr(dets.keep), _ptr(dets.keep_count), dets.N, cap, dets.H, dets.W,
-              dets.nC, n_cls, _ptr(idx_t), _ptr(size_t), _ptr(self.rank_key), _ptr(self.box), self.pool_cap,
-              _ptr(self.groups), self.group_cap, _ptr(self.counters), _stream())
+    def write_result_file(self, fps, parts):
+        """Write result_file_part's batches, in order, to the per-class files `fps` (write_detections' files)."""
+        for i in range(len(self.classes)):
+            for part in parts:
+                fps[i].writelines(part[i])
 
     def result(self, use_07_metric=True, novel_classes=(), curves=False):
         """The dict mean_ap returns; with curves=True also 'rec' / 'prec': {class: float64 array in rank order}.
@@ -306,7 +220,8 @@ class DeviceVocEval(object):
         n_det, n_groups, _, overflow = [int(v) for v in self.counters.cpu()]
         check_pool_flags(overflow)
         n_cls, dev = len(self.classes), self.device
-        ws = torch.empty(max(1, _call_size('fsdet_voc_workspace_bytes', n_det, self.n_gt)), dtype=torch.uint8, device=dev)
+        ws = torch.empty(max(1, eval_pool._call_size('fsdet_voc_workspace_bytes', n_det, self.n_gt)), dtype=torch.uint8,
+                         device=dev)
         out = dict(flags=torch.empty(n_det, dtype=torch.uint8, device=dev),
                    order=torch.empty(n_det, dtype=torch.int32, device=dev),
                    rec=torch.empty(n_det, dtype=torch.float64, device=dev),
@@ -316,12 +231,12 @@ class DeviceVocEval(object):
                    ap07=torch.empty(n_cls, dtype=torch.float64, device=dev),
                    ap_area=torch.empty(n_cls, dtype=torch.float64, device=dev))
         th = np.ascontiguousarray(VOC07_THRESHOLDS, dtype=np.float64)
-        _call('fsdet_voc_evaluate', _ptr(self.rank_key) if n_det else None, _ptr(self.box) if n_det else None, n_det,
-              _ptr(self.groups), n_groups, _ptr(self.gt_ptr), _ptr(self.gt_box) if self.n_gt else None,
-              _ptr(self.gt_difficult) if self.n_gt else None, self.n_gt, n_cls, len(self.imagenames), self.ovthresh,
-              th.ctypes.data, _ptr(ws), ws.numel(), _ptr(out['flags']), _ptr(out['order']), _ptr(out['rec']),
-              _ptr(out['prec']), _ptr(out['cls_count']), _ptr(out['npos']), _ptr(out['ap07']), _ptr(out['ap_area']),
-              _stream())
+        eval_pool._call('fsdet_voc_evaluate', _ptr(self.key) if n_det else None, _ptr(self.box) if n_det else None,
+                        n_det, _ptr(self.groups), n_groups, _ptr(self.gt_ptr), _ptr(self.gt_box) if self.n_gt else None,
+                        _ptr(self.gt_difficult) if self.n_gt else None, self.n_gt, n_cls, len(self.imagenames),
+                        self.ovthresh, th.ctypes.data, _ptr(ws), ws.numel(), _ptr(out['flags']), _ptr(out['order']),
+                        _ptr(out['rec']), _ptr(out['prec']), _ptr(out['cls_count']), _ptr(out['npos']),
+                        _ptr(out['ap07']), _ptr(out['ap_area']), eval_pool._stream())
         self.last = out
         ap = (out['ap07'] if use_07_metric else out['ap_area']).cpu().numpy()
         aps = dict((c, float(ap[i])) for i, c in enumerate(self.classes))
@@ -334,17 +249,3 @@ class DeviceVocEval(object):
             r['prec'] = dict((c, prec[starts[i]:starts[i + 1]]) for i, c in enumerate(self.classes))
         return r
 
-
-def _call_size(name, *args):
-    from ._lib import lib
-    return int(getattr(lib, name)(*args))
-
-
-def check_pool_flags(flags):
-    """Raise on the error bits the gather / merge kernels leave in counters[3]."""
-    if flags & 1:
-        raise RuntimeError('detection pool overflow')
-    if flags & 2:
-        raise RuntimeError('merged pools: an image was evaluated on two ranks')
-    if flags & 4:
-        raise RuntimeError('merged pools: a group outside its pool')

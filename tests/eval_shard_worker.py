@@ -2,7 +2,7 @@
 the backend: nccl with one GPU per rank, or gloo with the ranks sharing the GPUs there are).  On a mini meta model:
   1. valid.sharded_ensemble_dynamic_weights: the reweighting vectors bit-equal on every rank and to one process, also
      when a rank gets no support batch;
-  2. valid.sharded_valid_ap / sharded_valid_coco: the result dicts, the per-class result lines and the COCO results
+  2. valid.score_batches(sharded=True): the result dicts, the per-class result lines and the COCO results
      json equal those of one process, for an image count that is not a multiple of world x batch and for a set where
      a rank gets no batch;
   3. an image evaluated on two ranks raises on every rank (the error of the scoring rank is broadcast).
@@ -95,21 +95,21 @@ def main():
         s0, s1 = shard_range(13, 3, world, rank)
         q0, q1 = shard_range(n_img, bs, world, rank)
         fps1 = [io.StringIO() for _ in classes]
-        one = VA.valid_batches_ap(m, sup, images(0, n_img), V.DeviceVocEval(classes, names, recs), True,
-                                  novel_classes=('cow',), fps=fps1)
+        one = VA.score_batches(m, sup, images(0, n_img), V.DeviceVocEval(classes, names, recs), out=fps1,
+                               use_07_metric=True, novel_classes=('cow',))
         fpsN = [io.StringIO() for _ in classes] if rank == 0 else True
-        got = VA.sharded_valid_ap(m, supports(13, 3, s0, s1), images(q0, q1), V.DeviceVocEval(classes, names, recs),
-                                  True, novel_classes=('cow',), fps=fpsN)
+        got = VA.score_batches(m, supports(13, 3, s0, s1), images(q0, q1), V.DeviceVocEval(classes, names, recs),
+                               out=fpsN, sharded=True, use_07_metric=True, novel_classes=('cow',))
         assert same(got, one), ('sharded VOC result differs', n_img, got, one)
         if rank == 0:
             assert [f.getvalue() for f in fpsN] == [f.getvalue() for f in fps1], 'VOC result lines differ'
             assert sum(len(f.getvalue()) for f in fps1) > 0
         f1 = io.StringIO()
-        one = VA.valid_batches_coco(m, sup, images(0, n_img), C.DeviceCocoEval(classes, names, gt),
-                                    novel_classes=('cow',), results_fp=f1)
+        one = VA.score_batches(m, sup, images(0, n_img), C.DeviceCocoEval(classes, names, gt), out=f1,
+                               novel_classes=('cow',))
         fN = io.StringIO() if rank == 0 else True
-        got = VA.sharded_valid_coco(m, supports(13, 3, s0, s1), images(q0, q1), C.DeviceCocoEval(classes, names, gt),
-                                    novel_classes=('cow',), results_fp=fN)
+        got = VA.score_batches(m, supports(13, 3, s0, s1), images(q0, q1), C.DeviceCocoEval(classes, names, gt),
+                               out=fN, sharded=True, novel_classes=('cow',))
         assert same(got, one), ('sharded COCO result differs', n_img)
         if rank == 0:
             assert fN.getvalue() == f1.getvalue() and len(f1.getvalue()) > 2, 'COCO results json differs'

@@ -245,9 +245,12 @@ def test_pool_and_group_overflow(emul):
     assert counters[3] == 1 and counters[1] == 6 * n_cls
 
 
-def test_device_accumulator_glue_on_emulated_kernels(emul, monkeypatch):
-    """DeviceCocoEval's host side (ground-truth tables, capacity growth, argument lists, summary) with the C-ABI calls
-    routed to the emulated kernels and CPU tensors: the same dict as coco_evaluate."""
+def test_device_pool_glue_and_merge_on_emulated_kernels(emul, monkeypatch):
+    """DeviceCocoEval's host side (ground-truth tables, capacity growth, argument lists, summary, merging) with the
+    C-ABI calls routed to the emulated kernels and CPU tensors: the same dict as coco_evaluate, and the same pool and
+    dict from two evaluators given half the batches each and merged."""
+    import torch
+    from fewshot_detection_b200 import eval_pool
     n_cls = 5
     gt, sizes, rows = synthetic_set(3, n_img=14, n_cls=n_cls)
     names = ['n%d' % i for i in range(14)]
@@ -269,10 +272,16 @@ def test_device_accumulator_glue_on_emulated_kernels(emul, monkeypatch):
             del a[17]                                                         # workspace bytes
             ptrs = (0, 1, 3, 5, 6, 7, 8, 12, 13, 14, 15, 16, 17, 18, 19, 20)
             return emul.emul_coco_evaluate(*[V_(x) if k in ptrs else x for k, x in enumerate(a)])
+        if name == 'fsdet_coco_merge':
+            del a[9]                                                          # workspace bytes
+            a = [V_(x) if k in (1, 2, 3, 5, 8, 9, 10, 12, 14) else x for k, x in enumerate(a)]
+            a[4], a[6], a[11] = ctypes.c_longlong(a[4]), ctypes.c_longlong(a[6]), ctypes.c_longlong(a[11])
+            return emul.emul_coco_merge(*a)
         raise AssertionError(name)
-    monkeypatch.setattr(C, '_call', fake_call)
-    monkeypatch.setattr(C, '_call_size', lambda name, *a: emul.emul_coco_workspace_bytes(*a))
-    monkeypatch.setattr(C, '_stream', lambda: None)
+    emul.emul_eval_merge_workspace_bytes.restype = ctypes.c_size_t
+    monkeypatch.setattr(eval_pool, '_call', fake_call)
+    monkeypatch.setattr(eval_pool, '_call_size', lambda name, *a: getattr(emul, name.replace('fsdet_', 'emul_'))(*a))
+    monkeypatch.setattr(eval_pool, '_stream', lambda *a: None)
     ev = C.DeviceCocoEval(classes, names, gt, device='cpu')
     for images in batches:
         cand, keep, kc = detections(rows, images, n_cls)
@@ -285,3 +294,19 @@ def test_device_accumulator_glue_on_emulated_kernels(emul, monkeypatch):
     want = C.summarize(ref['precision'], ref['recall'], classes, ('c1', 'c4'))
     assert res['all'] == ref['all'] == want['all'] and res['novel'] == want['novel'] and res['ap'] == want['ap']
     assert res['ap']['c4'] == -1.0
+    # the same batches over two evaluators, merged in order
+    halves = [ev.empty_like(), ev.empty_like()]
+    for k, images in enumerate(batches):
+        cand, keep, kc = detections(rows, images, n_cls)
+        halves[2 * k // len(batches)].add(host_detections(cand, keep, kc, n_cls), [names[i] for i in images],
+                                          [sizes[i] for i in images])
+    assert all(int(h.counters[0]) > 0 for h in halves)
+    merged = type(ev).merge(halves)
+    assert calls.count('fsdet_coco_merge') == 1
+    n, g = int(ev.counters[0]), int(ev.counters[1])
+    assert [int(v) for v in merged.counters[[0, 1, 3]]] == [n, g, 0]
+    assert torch.equal(merged.key[:n], ev.key[:n]) and torch.equal(merged.box[:n], ev.box[:n])
+    assert torch.equal(merged.groups[:g], ev.groups[:g])
+    res2 = merged.result(novel_classes=('c1', 'c4'))
+    check_bit_equal(res2, res)
+    assert all(res2[k] == res[k] for k in ('all', 'base', 'novel', 'ap'))

@@ -2,7 +2,7 @@
 
   * the synthetic sets of the host-emulation test: gather and evaluation bit-equal to coco_eval.detection_records and
     coco_eval.coco_evaluate, and the overflow flag;
-  * a mini meta model on a synthetic COCO set: valid.valid_batches_coco equals the results json scored by the host
+  * a mini meta model on a synthetic COCO set: valid.score_batches equals the results json scored by the host
     evaluator, with no per-detection data copied to the host;
   * a minival-sized pass (5,000 images x 80 classes, ~30 survivors per row): precision / recall of 8 random classes
     bit-equal to a host run over those classes alone (classes are evaluated independently)."""
@@ -111,7 +111,7 @@ class _CopyLog(object):
         monkeypatch.setattr(torch.Tensor, 'to', to)
 
 
-def test_mini_meta_model_device_equals_results_json(tmp_path, monkeypatch):
+def test_score_batches_device_equals_results_json(tmp_path, monkeypatch):
     sys.path.insert(0, G)
     from seeding import seeded_init, synth_masks
     from fewshot_detection_b200 import coco_eval as C, netcfg, valid as VA
@@ -158,7 +158,7 @@ def test_mini_meta_model_device_equals_results_json(tmp_path, monkeypatch):
     # device path, host reads logged
     ev = C.DeviceCocoEval(classes, names, gt)
     log = _CopyLog(monkeypatch)
-    dev = VA.valid_batches_coco(m, meta, images, ev, novel_classes=('cow',))
+    dev = VA.score_batches(m, meta, images, ev, novel_classes=('cow',))
     monkeypatch.undo()
     assert max(log.sizes) <= 10 * 101 * n_cls * 4 * 3, log.sizes              # counters, precision, recall, scalars
     n_det = int(ev.counters[0])
@@ -166,7 +166,7 @@ def test_mini_meta_model_device_equals_results_json(tmp_path, monkeypatch):
     # results json of the same detections, scored on the host
     ev2 = C.DeviceCocoEval(classes, names, gt)
     f = io.StringIO()
-    again = VA.valid_batches_coco(m, meta, images, ev2, novel_classes=('cow',), results_fp=f)
+    again = VA.score_batches(m, meta, images, ev2, out=f, novel_classes=('cow',))
     results = json.loads(f.getvalue())
     assert len(results) == n_det
     host = C.coco_evaluate(gt, results, names, classes, novel_classes=('cow',))

@@ -65,7 +65,7 @@ def bits(a):
 
 
 @pytest.mark.parametrize('seed,n_img,n_cls,world', [(0, 24, 6, 2), (1, 24, 6, 3), (9, 300, 12, 4), (2, 24, 6, 16)])
-def test_voc_merge_equals_one_evaluator(seed, n_img, n_cls, world):
+def test_voc_merged_pool_equals_one_evaluator(seed, n_img, n_cls, world):
     from fewshot_detection_b200 import voc_eval as V
     gt, sizes, rows, names, classes, batches = make_set(seed, n_img, n_cls)
     recs = voc_recs(gt, names, classes)
@@ -74,7 +74,7 @@ def test_voc_merge_equals_one_evaluator(seed, n_img, n_cls, world):
     merged = V.DeviceVocEval.merge(parts)
     n = int(one.counters[0])
     assert merged.counters.tolist()[:2] == one.counters.tolist()[:2] and n > 1000
-    assert torch.equal(merged.rank_key[:n], one.rank_key[:n]) and torch.equal(merged.box[:n], one.box[:n])
+    assert torch.equal(merged.key[:n], one.key[:n]) and torch.equal(merged.box[:n], one.box[:n])
     for use07 in (True, False):
         a = merged.result(use07, novel_classes=('c1',), curves=True)
         b = one.result(use07, novel_classes=('c1',), curves=True)

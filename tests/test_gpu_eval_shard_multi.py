@@ -31,7 +31,7 @@ def test_two_gpus_nccl_sharded_equals_one_process():
     assert r.returncode == 0 and r.stdout.count('SHARD_OK') == 2, r.stdout[-4000:]
 
 
-def test_two_processes_gloo_sharded_equals_one_process():
+def test_two_processes_gloo_score_batches_equals_one_process():
     r = torchrun(29637, [WORKER, 'gloo'])
     assert r.returncode == 0 and r.stdout.count('SHARD_OK') == 2, r.stdout[-4000:]
 

@@ -3,7 +3,7 @@
   * '%f' % x -> float() of millions of doubles, bit-exact;
   * tests/golden/voc_eval.npz (the reference's scripts/voc_eval.py): rec / prec equal, VOC07 AP equal, area AP within
     1e-12; synthetic sets with heavy ties against a stable-ranking copy of match_detections;
-  * a mini meta model on a synthetic devkit: valid.valid_batches_ap against valid_batches + voc_eval.mean_ap on the
+  * a mini meta model on a synthetic devkit: valid.score_batches against valid_batches + voc_eval.mean_ap on the
     written files (equal wherever a class has no tied confidences) and against the stable-ranking copy on the same
     lines (equal everywhere), with no per-detection data copied to the host."""
 import os
@@ -128,7 +128,7 @@ class _CopyLog(object):
         monkeypatch.setattr(torch.Tensor, 'to', to)
 
 
-def test_mini_meta_model_device_ap_equals_result_files(tmp_path, monkeypatch):
+def test_score_batches_device_ap_equals_result_files(tmp_path, monkeypatch):
     import sys
     sys.path.insert(0, G)
     from seeding import seeded_init, synth_masks
@@ -186,7 +186,7 @@ def test_mini_meta_model_device_ap_equals_result_files(tmp_path, monkeypatch):
     recs_loaded = V.load_annotations(annopath, names, os.path.join(root, 'cache'))
     ev = V.DeviceVocEval(classes, names, recs_loaded)
     log = _CopyLog(monkeypatch)
-    dev07 = VA.valid_batches_ap(m, meta, images, ev, True, novel_classes=('cow',))
+    dev07 = VA.score_batches(m, meta, images, ev, use_07_metric=True, novel_classes=('cow',))
     monkeypatch.undo()
     assert max(log.sizes) <= max(n_cls, 4), log.sizes          # counters, per-class results, scalars of the ensembling
     # the accumulator alone, from the CUDA trace: its only device-to-host copies are the record count read when the
@@ -225,5 +225,14 @@ def test_mini_meta_model_device_ap_equals_result_files(tmp_path, monkeypatch):
             tied.append(name)
     assert n_lines > 300 and int(ev.counters[0]) == n_lines
     assert 0 < dev07['mean'] < 1 and dev07['mean_novel'] == dev07['ap']['cow']
+    # the result files of the device pass are the files valid_batches writes, byte for byte
+    import io
+    fps = [io.StringIO() for _ in classes]
+    with_files = VA.score_batches(m, meta, images, V.DeviceVocEval(classes, names, recs_loaded), out=fps,
+                                  use_07_metric=True, novel_classes=('cow',))
+    assert with_files == dev07
+    for name, f in zip(classes, fps):
+        with open(detpath.format(name)) as g:
+            assert f.getvalue() == g.read(), name
     print('device AP %s, files AP %s, %d lines, classes with tied confidences: %s'
           % (dev07['ap'], files07['ap'], n_lines, tied))

@@ -359,11 +359,12 @@ def test_gather_equals_result_lines(emul):
     assert counters2.tolist() == [0, 0, 0, 1]
 
 
-def test_device_accumulator_glue_on_emulated_kernels(emul, monkeypatch):
-    """DeviceVocEval's host side (ground-truth tables, capacity growth, argument lists, result dict) with the C-ABI
-    calls routed to the emulated kernels and CPU tensors; same dict as mean_ap on the files write_detections writes."""
+def test_device_pool_glue_and_merge_on_emulated_kernels(emul, monkeypatch):
+    """DeviceVocEval's host side (ground-truth tables, capacity growth, argument lists, result dict, merging) with the
+    C-ABI calls routed to the emulated kernels and CPU tensors; same dict as mean_ap on the files write_detections
+    writes, and the same pool and dict from two evaluators given half the batches each and merged."""
     import torch
-    from fewshot_detection_b200 import utils as U
+    from fewshot_detection_b200 import eval_pool, utils as U
     gold = np.load(os.path.join(G, 'voc_eval.npz'), allow_pickle=False)
     names, recs, classes, per_class = golden_case(gold)
     calls = []
@@ -384,11 +385,18 @@ def test_device_accumulator_glue_on_emulated_kernels(emul, monkeypatch):
             a = [V_(x) if k in ptrs else x for k, x in enumerate(a[:-1])]
             a[11] = ctypes.c_double(a[11])
             return emul.emul_voc_evaluate(*a)
+        if name == 'fsdet_voc_merge':
+            a = list(a[:-1])
+            del a[9]                                                         # workspace bytes
+            a = [V_(x) if k in (1, 2, 3, 5, 8, 9, 10, 12, 14) else x for k, x in enumerate(a)]
+            a[4], a[6], a[11] = ctypes.c_longlong(a[4]), ctypes.c_longlong(a[6]), ctypes.c_longlong(a[11])
+            return emul.emul_voc_merge(*a)
         raise AssertionError(name)
     emul.emul_voc_workspace_bytes.restype = ctypes.c_size_t
-    monkeypatch.setattr(V, '_call', fake_call)
-    monkeypatch.setattr(V, '_call_size', lambda name, *a: emul.emul_voc_workspace_bytes(*a))
-    monkeypatch.setattr(V, '_stream', lambda: None)
+    emul.emul_eval_merge_workspace_bytes.restype = ctypes.c_size_t
+    monkeypatch.setattr(eval_pool, '_call', fake_call)
+    monkeypatch.setattr(eval_pool, '_call_size', lambda name, *a: getattr(emul, name.replace('fsdet_', 'emul_'))(*a))
+    monkeypatch.setattr(eval_pool, '_stream', lambda *a: None)
     ev = V.DeviceVocEval(classes, names, recs, device='cpu')
     # Detections whose kept boxes print exactly as the golden lines: one batch per image, grid 1x1, W = H = 1, A = the
     # most lines of one image and class, det = 1, cls = prob, (xs, ys, ws, hs) chosen so that the corners come back
@@ -399,6 +407,7 @@ def test_device_accumulator_glue_on_emulated_kernels(emul, monkeypatch):
             by_img[l[0]][c].append(l)
     A = max(len(v) for img in by_img.values() for v in img)
     size = (1000, 1000)
+    batches = []
     for n in names:
         rows = by_img[n]
         cand = np.zeros((len(classes), A, 8), dtype=np.float32)
@@ -413,12 +422,13 @@ def test_device_accumulator_glue_on_emulated_kernels(emul, monkeypatch):
         d = U.Detections(torch.from_numpy(cand), torch.from_numpy(kc.copy()), None, len(classes), A, 1, 1, 1, False, True, 0.005)
         d.keep, d.keep_count = torch.from_numpy(keep), torch.from_numpy(kc)
         ev.add(d, [n], [size])
+        batches.append((d, n))
         # what the device computed from these float32 values, as lines: overwrite the host copy with it
         for c, r in enumerate(rows):
             g = ev.groups[int(ev.counters[2]) + c].numpy()
             for s in range(len(r)):
                 k = g[0] + s
-                key = int(ev.rank_key[k]) & 0xffffffff
+                key = int(ev.key[k]) & 0xffffffff
                 r[s] = (n, (KEY_MASK - (key & KEY_MASK)) / 1e6) + tuple(ev.box[k].tolist())
     with pytest.raises(ValueError):
         ev.add(d, [names[-1]], [size])                                      # an image twice
@@ -432,3 +442,20 @@ def test_device_accumulator_glue_on_emulated_kernels(emul, monkeypatch):
         assert np.array_equal(res['rec'][name], rec) and np.array_equal(res['prec'][name], prec)
     assert res['mean_novel'] == res['ap']['cow']
     assert res['mean'] == float(np.mean([res['ap'][c] for c in classes]))
+    # the same batches over two evaluators, merged in order
+    halves = [ev.empty_like(), ev.empty_like()]
+    for k, (d, n) in enumerate(batches):
+        halves[2 * k // len(batches)].add(d, [n], [size])
+    assert all(int(h.counters[0]) > 0 for h in halves)
+    merged = V.DeviceVocEval.merge(halves)
+    assert calls.count('fsdet_voc_merge') == 1
+    n, g = int(ev.counters[0]), int(ev.counters[1])
+    assert [int(v) for v in merged.counters[[0, 1, 3]]] == [n, g, 0]
+    assert torch.equal(merged.key[:n], ev.key[:n]) and torch.equal(merged.box[:n], ev.box[:n])
+    assert torch.equal(merged.groups[:g], ev.groups[:g])
+    res2, res2_area = merged.result(True, novel_classes=('cow',), curves=True), merged.result(False)
+    assert res2_area == res_area
+    assert [res2[k] for k in ('ap', 'mean', 'mean_base', 'mean_novel')] == \
+        [res[k] for k in ('ap', 'mean', 'mean_base', 'mean_novel')]
+    for k in ('rec', 'prec'):
+        assert all(np.array_equal(res2[k][c], res[k][c]) for c in classes)

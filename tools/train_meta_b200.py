@@ -10,7 +10,7 @@ from lists.build_dataset, the support index from lists.support_index, the step f
 replay, one graph per multi-scale input size).  Under torchrun every rank builds the same lists with the same seeds,
 takes its slice of each global batch, and rank 0's parameters are broadcast once before the first step.
 A trained weight file is scored by tools/valid_ensemble_b200.py (valid_ensemble.py + scripts/voc_eval.py).  Opt-in,
-every checkpoint is scored the same way while training runs, sharded over the ranks (valid.sharded_valid_ap):
+every checkpoint is scored the same way while training runs, sharded over the ranks (valid.score_batches):
 
     --eval-devkit DIR [--eval-year Y]      VOC AP on the `valid` list: one line with mean, base and novel AP
     --eval-coco-annotations JSON           COCO box AP on the `valid` list: one line with AP, AP50, AP75
@@ -60,6 +60,7 @@ def checkpoint_evaluator(data_options, devkit, year, coco_annotations, world, ra
     imgids = [os.path.basename(l).split('.')[0] for l in lines]
     if coco_annotations is not None:
         proto = CE.DeviceCocoEval(classes, imgids, CE.load_coco_annotations(coco_annotations, imgids, classes))
+        result_kwargs = dict(novel_classes=novel)
     else:
         voc = os.path.join(devkit, 'VOC' + year)
         names = read_list(os.path.join(voc, 'ImageSets', 'Main', 'test.txt'))
@@ -67,6 +68,7 @@ def checkpoint_evaluator(data_options, devkit, year, coco_annotations, world, ra
                                            os.path.join(devkit, 'annotations_cache'))
         recs = rank0_first(load) if world > 1 else load()  # rank 0 writes the cache, the others read it
         proto = VE.DeviceVocEval(classes, names, recs)
+        result_kwargs = dict(use_07_metric=int(year) < 2010, novel_classes=novel)
     s0, s1 = shard_range(len(inds), support_batch, world, rank)
     q0, q1 = shard_range(len(lines), batch_size, world, rank)
 
@@ -79,15 +81,9 @@ def checkpoint_evaluator(data_options, devkit, year, coco_annotations, world, ra
             for s in range(q0, q1, batch_size):
                 idx = range(s, min(s + batch_size, q1))
                 yield db.batch(idx)[0], [imgids[i] for i in idx], [db._entry(i).size() for i in idx]
-        ev = proto.empty_like()
+        r = VA.score_batches(model, meta, images(), proto.empty_like(), sharded=world > 1, **result_kwargs)
         if coco_annotations is not None:
-            fn = VA.sharded_valid_coco if world > 1 else VA.valid_batches_coco
-            r = fn(model, meta, images(), ev, novel_classes=novel)
             return 'COCO AP %.4f AP50 %.4f AP75 %.4f' % tuple(r['all'][:3])
-        if world > 1:
-            r = VA.sharded_valid_ap(model, meta, images(), ev, int(year) < 2010, novel_classes=novel)
-        else:
-            r = VA.valid_batches_ap(model, meta, images(), ev, int(year) < 2010, novel_classes=novel)
         fmt = lambda v: 'n/a' if v is None else '%.4f' % v
         return 'mAP %s base %s novel %s' % (fmt(r['mean']), fmt(r['mean_base']), fmt(r['mean_novel']))
     return evaluate

@@ -98,7 +98,7 @@ def run(args, world, rank):
     from fewshot_detection_b200.darknet_meta import Darknet
     from fewshot_detection_b200.dataset import DetectionBatcher, MetaBatcher
     from fewshot_detection_b200.shard import rank0_first, shard_range
-    from fewshot_detection_b200 import lists as LS, valid as VA, voc_eval as VE
+    from fewshot_detection_b200 import coco_eval as CE, lists as LS, valid as VA, voc_eval as VE
     sharded, lead = world > 1, rank == 0
     data_options = read_data_cfg(args.datacfg)
     darknetcfg, learnetcfg = parse_cfg(args.darknetcfg), parse_cfg(args.learnetcfg)
@@ -129,24 +129,22 @@ def run(args, world, rank):
             data, _ = db.batch(idx)
             yield data, [imgids[i] for i in idx], [db._entry(i).size() for i in idx]
 
-    fps = None
+    out = None                                        # result files: VOC per class, or the COCO results json
     if args.write_results and not lead:
-        fps = True                                    # this rank's lines go to rank 0
+        out = True                                    # this rank's lines go to rank 0
     elif args.write_results:
         prefix = result_prefix(args.weightfile)
         if not os.path.exists(prefix):
             os.makedirs(prefix)
         logging('saving to: %s' % prefix)
-        fps = [open(os.path.join(prefix, 'comp4_det_test_%s.txt' % c), 'w') for c in classes]
-    if args.coco_annotations is not None:
-        return coco_main(args, m, meta_batches, image_batches(), imgids, classes, novel, sharded, lead)
+        out = [open(os.path.join(prefix, 'comp4_det_test_%s.txt' % c), 'w') for c in classes]
     try:
-        if args.devkit is None:
+        if args.devkit is None and args.coco_annotations is None:
             n_cls = len(classes)
             if not sharded:
                 dw = VA.ensemble_dynamic_weights(m, meta_batches, n_cls)
                 for data, ids, sizes in image_batches():
-                    VA.write_detections(fps, VA.detect(m, data, dw, n_cls), ids, sizes, n_cls)
+                    VA.write_detections(out, VA.detect(m, data, dw, n_cls), ids, sizes, n_cls)
                 return 0
             dw = VA.sharded_ensemble_dynamic_weights(m, meta_batches, n_cls)
             mine = dict((i, []) for i in range(n_cls))
@@ -157,26 +155,32 @@ def run(args, world, rank):
             if lead:
                 for part in parts:
                     for i in range(n_cls):
-                        fps[i].writelines(part[i])
+                        out[i].writelines(part[i])
             return 0
-        voc = os.path.join(args.devkit, 'VOC' + args.year)
-        imagenames = read_list(os.path.join(voc, 'ImageSets', 'Main', 'test.txt'))
-        load = lambda: VE.load_annotations(os.path.join(voc, 'Annotations', '{}.xml'), imagenames,
-                                           os.path.join(args.devkit, 'annotations_cache'))
-        recs = rank0_first(load) if sharded else load()    # rank 0 writes the cache, the others read it
-        use_07 = int(args.year) < 2010
-        ev = VE.DeviceVocEval(classes, imagenames, recs)
-        if sharded:
-            r = VA.sharded_valid_ap(m, meta_batches, image_batches(), ev, use_07, novel_classes=novel, fps=fps)
+        if args.coco_annotations is not None:
+            ev = CE.DeviceCocoEval(classes, imgids, CE.load_coco_annotations(args.coco_annotations, imgids, classes))
+            if args.write_coco_results:
+                out = open(args.write_coco_results, 'w') if lead else True
+            result_kwargs = dict(novel_classes=novel)
         else:
-            r = VA.valid_batches_ap(m, meta_batches, image_batches(), ev, use_07, novel_classes=novel, fps=fps)
+            voc = os.path.join(args.devkit, 'VOC' + args.year)
+            imagenames = read_list(os.path.join(voc, 'ImageSets', 'Main', 'test.txt'))
+            load = lambda: VE.load_annotations(os.path.join(voc, 'Annotations', '{}.xml'), imagenames,
+                                               os.path.join(args.devkit, 'annotations_cache'))
+            recs = rank0_first(load) if sharded else load()    # rank 0 writes the cache, the others read it
+            ev = VE.DeviceVocEval(classes, imagenames, recs)
+            result_kwargs = dict(use_07_metric=int(args.year) < 2010, novel_classes=novel)
+        r = VA.score_batches(m, meta_batches, image_batches(), ev, out, sharded, **result_kwargs)
     finally:
-        if fps is not None and fps is not True:
-            for f in fps:
+        for f in out if isinstance(out, list) else [out]:
+            if f is not None and f is not True:
                 f.close()
     if not lead:
         return 0
-    print('VOC07 metric? ' + ('Yes' if use_07 else 'No'))
+    if args.coco_annotations is not None:
+        print_coco(r, classes, novel)
+        return 0
+    print('VOC07 metric? ' + ('Yes' if result_kwargs['use_07_metric'] else 'No'))
     for c in classes:
         print('AP for {} = {:.4f}{}'.format(c, r['ap'][c], ' (novel)' if c in novel else ''))
     print('Mean AP = {:.4f}'.format(r['mean']))
@@ -187,24 +191,9 @@ def run(args, world, rank):
     return 0
 
 
-def coco_main(args, m, meta_batches, image_batches, imgids, classes, novel, sharded=False, lead=True):
-    """--coco-annotations: the COCO box metric on the device, summary lines as pycocotools prints them."""
-    from fewshot_detection_b200 import coco_eval as CE, valid as VA
-    gt = CE.load_coco_annotations(args.coco_annotations, imgids, classes)
-    ev = CE.DeviceCocoEval(classes, imgids, gt)
-    results_fp = None
-    if args.write_coco_results:
-        results_fp = open(args.write_coco_results, 'w') if lead else True
-    try:
-        if sharded:
-            r = VA.sharded_valid_coco(m, meta_batches, image_batches, ev, novel_classes=novel, results_fp=results_fp)
-        else:
-            r = VA.valid_batches_coco(m, meta_batches, image_batches, ev, novel_classes=novel, results_fp=results_fp)
-    finally:
-        if results_fp is not None and results_fp is not True:
-            results_fp.close()
-    if not lead:
-        return 0
+def print_coco(r, classes, novel):
+    """The summary lines as pycocotools prints them, for all, base and novel classes, then the AP of each class."""
+    from fewshot_detection_b200 import coco_eval as CE
     for title, key in (('all classes', 'all'), ('base classes', 'base'), ('novel classes', 'novel')):
         if r[key] is None:
             continue
@@ -213,7 +202,6 @@ def coco_main(args, m, meta_batches, image_batches, imgids, classes, novel, shar
             print(line)
     for c in classes:
         print('AP for {} = {:.4f}{}'.format(c, r['ap'][c], ' (novel)' if c in novel else ''))
-    return 0
 
 
 if __name__ == '__main__':
