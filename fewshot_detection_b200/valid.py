@@ -14,7 +14,9 @@ or, without the files, scores them where they are (voc_eval.DeviceVocEval, coco_
 
     evaluator.add(dets, imgids, sizes); ...; evaluator.result()          # the dict voc_eval.mean_ap returns
 
-`score_batches` runs that whole pass, in one process or sharded over the ranks of a process group.
+`score_batches` runs that whole pass, in one process or sharded over the ranks of a process group.  Both passes can
+write the ensembled vectors to the reference's vectors file and detect with the base-class rows of a stored one
+(valid_ensemble.py:102-119, `use_baserw`): evaluation_dynamic_weights.
 
 CUDA only (libfsdet.so); no host fallback.
 """
@@ -65,6 +67,70 @@ class ReweightEnsembler(object):
         return [self.enews.view(self.n_cls, self.C, 1, 1)]
 
 
+# ---- stored reweighting vectors (valid_ensemble.py:102-119) ----------------------------------------------------------
+# The file is the reference's: a pickled list with one float32 numpy array [n_cls, C, 1, 1] per dynamic layer, rows in
+# the order of the evaluated class list.  Its `use_baserw` mode replaces the base-class rows of the ensembled vectors
+# with the stored ones, so that after k-shot fine-tuning the base classes keep vectors averaged over a large support set.
+def reweighting_vector_shapes(learnet_blocks, n_cls):
+    """The shapes of the vectors a model with these reweighting-net blocks ensembles for n_cls classes: one layer,
+    [n_cls, C, 1, 1] with C the filters of the net's last convolution (what meta_forward returns per support image)."""
+    convs = [b for b in learnet_blocks if b['type'] == 'convolutional']
+    if not convs:
+        raise ValueError('the reweighting net has no convolution')
+    return [(int(n_cls), int(convs[-1]['filters']), 1, 1)]
+
+
+def save_reweighting_vectors(path, dynamic_weights):
+    """Pickle `[x.cpu().numpy() for x in dynamic_weights]` to `path` (the reference's commented-out writer,
+    valid_ensemble.py:102-106)."""
+    import pickle
+    arrays = [x.detach().to('cpu', torch.float32).contiguous().numpy() for x in dynamic_weights]
+    with open(path, 'wb') as f:
+        pickle.dump(arrays, f)
+
+
+def load_reweighting_vectors(path, shapes=None):
+    """The list save_reweighting_vectors wrote, or a Python 2 pickle of the same list.  `shapes`: the shape of every
+    layer the evaluated model has (reweighting_vector_shapes); anything else raises ValueError, as does anything that
+    is not a list of finite float32 arrays."""
+    import pickle
+    import numpy as np
+    with open(path, 'rb') as f:
+        try:
+            rws = pickle.load(f, encoding='latin1')    # Python 2 pickles hold the array bytes as 8-bit str
+        except Exception as e:
+            raise ValueError('%s: not a pickled list of vectors: %s: %s' % (path, type(e).__name__, e))
+    want = 'float32 arrays of shapes %s' % [tuple(s) for s in shapes] if shapes is not None else \
+        'float32 arrays [n_cls, C, 1, 1]'
+    if not isinstance(rws, list) or not all(isinstance(a, np.ndarray) for a in rws):
+        got = type(rws).__name__ if not isinstance(rws, list) else 'a list of %s' % [type(a).__name__ for a in rws]
+        raise ValueError('%s: expected a list of %s, got %s' % (path, want, got))
+    got = [tuple(a.shape) for a in rws]
+    if shapes is not None and got != [tuple(s) for s in shapes]:
+        raise ValueError('%s: the model needs %s, the file has shapes %s' % (path, want, got))
+    for i, a in enumerate(rws):
+        if a.dtype != np.float32 or a.ndim != 4 or a.shape[2:] != (1, 1):
+            raise ValueError('%s: expected %s, layer %d is %s %s' % (path, want, i, a.dtype, a.shape))
+        if not np.isfinite(a).all():
+            raise ValueError('%s: layer %d %s has non-finite values' % (path, i, a.shape))
+    return rws
+
+
+def substitute_base_rows(dynamic_weights, stored, base_rows):
+    """dynamic_weights[i][base_rows] = stored[i][base_rows] in place, in every layer (valid_ensemble.py:117-119).
+    `stored` is load_reweighting_vectors' list; `base_rows` are the indices of the evaluated classes that are not
+    novel (cfg._real_base_ids for cfg.classes).  The other rows keep their ensembled values."""
+    if len(stored) != len(dynamic_weights):
+        raise ValueError('%d stored layers for %d dynamic layers' % (len(stored), len(dynamic_weights)))
+    rows = torch.as_tensor(list(base_rows), dtype=torch.int64)
+    for dw, rw in zip(dynamic_weights, stored):
+        src = torch.as_tensor(rw)
+        if tuple(src.shape) != tuple(dw.shape):
+            raise ValueError('stored vectors %s do not fit the ensembled %s' % (tuple(src.shape), tuple(dw.shape)))
+        dw[rows.to(dw.device)] = src[rows].to(dw.device, dw.dtype)      # only the base rows go to the device
+    return dynamic_weights
+
+
 def ensemble_dynamic_weights(m, meta_batches, n_cls):
     """valid_ensemble.py:86-100.  `meta_batches` yields (metax [n,3,S,S], mask [n,1,S,S], clsids [n]) like the
     reference's MetaDataset(ensemble=True, with_ids=True) loader."""
@@ -79,6 +145,28 @@ def ensemble_dynamic_weights(m, meta_batches, n_cls):
     if ens is None:
         raise ValueError('no support batches')
     return ens.result()
+
+
+def evaluation_dynamic_weights(m, meta_batches, n_cls, sharded=False, process_group=None, dst=0, base_rw=None,
+                               base_rows=None, save_rw=None):
+    """The vectors an evaluation pass detects with: the ensemble over `meta_batches` (sharded=True: this rank's block,
+    gathered so that every rank holds the single-process vectors), written to the file `save_rw` by one process
+    (rank `dst` when sharded) before any substitution, then with the `base_rows` of the stored `base_rw`
+    (load_reweighting_vectors) substituted on every rank."""
+    if base_rw is not None and base_rows is None:
+        raise ValueError('base_rw needs base_rows: the indices of the evaluated classes that are not novel')
+    if sharded:
+        from .shard import group_info
+        dynamic_weights = sharded_ensemble_dynamic_weights(m, meta_batches, n_cls, process_group)
+        writer = group_info(process_group)[1] == dst
+    else:
+        dynamic_weights = ensemble_dynamic_weights(m, meta_batches, n_cls)
+        writer = True
+    if save_rw is not None and writer:
+        save_reweighting_vectors(save_rw, dynamic_weights)
+    if base_rw is not None:
+        substitute_base_rows(dynamic_weights, base_rw, base_rows)
+    return dynamic_weights
 
 
 def detect(m, data, dynamic_weights, n_cls, conf_thresh=CONF_THRESH, nms_thresh=NMS_THRESH):
@@ -119,12 +207,15 @@ def write_detections(fps, dets, imgids, sizes, n_cls, nms_thresh=NMS_THRESH):
         fps[i].writelines(lines[i])
 
 
-def valid_batches(m, meta_batches, image_batches, class_names, prefix, outfile):
+def valid_batches(m, meta_batches, image_batches, class_names, prefix, outfile, base_rw=None, base_rows=None,
+                  save_rw=None):
     """The body of valid_ensemble.valid() (:86-181) over iterables: `meta_batches` as in ensemble_dynamic_weights,
-    `image_batches` yields (data [b,3,H,W], imgids, sizes).  Writes `<prefix>/<outfile><class>.txt`."""
+    `image_batches` yields (data [b,3,H,W], imgids, sizes).  Writes `<prefix>/<outfile><class>.txt`.
+    base_rw, base_rows, save_rw: the stored-vector mode and the vectors file, as in evaluation_dynamic_weights."""
     n_cls = len(class_names)
     m.eval()
-    dynamic_weights = ensemble_dynamic_weights(m, meta_batches, n_cls)
+    dynamic_weights = evaluation_dynamic_weights(m, meta_batches, n_cls, base_rw=base_rw, base_rows=base_rows,
+                                                 save_rw=save_rw)
     if not os.path.exists(prefix):
         os.makedirs(prefix)
     fps = [open('%s/%s%s.txt' % (prefix, outfile, name), 'w') for name in class_names]
@@ -140,7 +231,7 @@ def valid_batches(m, meta_batches, image_batches, class_names, prefix, outfile):
 
 
 def score_batches(m, support_batches, image_batches, evaluator, out=None, sharded=False, process_group=None, dst=0,
-                  **result_kwargs):
+                  base_rw=None, base_rows=None, save_rw=None, **result_kwargs):
     """valid_batches scored on the device: `evaluator` is a voc_eval.DeviceVocEval or coco_eval.DeviceCocoEval over
     the evaluated image set, `support_batches` are as ensemble_dynamic_weights' meta_batches, `image_batches` yields
     (data, imgids, sizes) with imgids names of that set.  Returns evaluator.result(**result_kwargs): mean_ap's dict
@@ -152,13 +243,14 @@ def score_batches(m, support_batches, image_batches, evaluator, out=None, sharde
     sharded=True: collective over `process_group`, each rank running its own block of the single-process support and
     query batches (shard.shard_range).  The pools are merged in rank order and scored once on rank `dst`; every rank
     returns the single-process dict.  `out` is open on `dst` and True on the other ranks, whose parts go to `dst`,
-    which writes every rank's in rank order: the single-process files.  None on every rank for no files."""
+    which writes every rank's in rank order: the single-process files.  None on every rank for no files.
+
+    base_rw, base_rows, save_rw: the stored-vector mode and the vectors file, as in evaluation_dynamic_weights (the
+    file is written on `dst` when sharded)."""
     n_cls = len(evaluator.classes)
     m.eval()
-    if sharded:
-        dynamic_weights = sharded_ensemble_dynamic_weights(m, support_batches, n_cls, process_group)
-    else:
-        dynamic_weights = ensemble_dynamic_weights(m, support_batches, n_cls)
+    dynamic_weights = evaluation_dynamic_weights(m, support_batches, n_cls, sharded, process_group, dst, base_rw,
+                                                 base_rows, save_rw)
     dev = next(m.parameters()).device
     parts = []
     for data, imgids, sizes in image_batches:

@@ -14,6 +14,8 @@ every checkpoint is scored the same way while training runs, sharded over the ra
 
     --eval-devkit DIR [--eval-year Y]      VOC AP on the `valid` list: one line with mean, base and novel AP
     --eval-coco-annotations JSON           COCO box AP on the `valid` list: one line with AP, AP50, AP75
+    --eval-base-rw PATH                    with either: the base classes detected with the rows of a stored vectors
+                                           file (the evaluation command's --base-rw)
 
 with the support set, batch sizes and thresholds of the evaluation command.
 """
@@ -47,9 +49,11 @@ def broadcast_parameters(model, src=0):
             raise RuntimeError('replicas differ after the parameter broadcast')
 
 
-def checkpoint_evaluator(data_options, devkit, year, coco_annotations, world, rank, batch_size=64, support_batch=64):
+def checkpoint_evaluator(data_options, devkit, year, coco_annotations, world, rank, batch_size=64, support_batch=64,
+                         base_rw=None):
     """evaluate(model, epoch) for MetaTrainer: the evaluation command's pass over `valid`, this rank's shard of it;
-    returns the line rank 0 logs."""
+    returns the line rank 0 logs.  base_rw: stored vectors (valid.load_reweighting_vectors) whose rows replace those
+    of the base classes, cfg._real_base_ids, as the evaluation command's --base-rw does."""
     from fewshot_detection_b200.cfg import cfg
     from fewshot_detection_b200.dataset import DetectionBatcher, MetaBatcher
     from fewshot_detection_b200.shard import rank0_first, shard_range
@@ -71,6 +75,8 @@ def checkpoint_evaluator(data_options, devkit, year, coco_annotations, world, ra
         result_kwargs = dict(use_07_metric=int(year) < 2010, novel_classes=novel)
     s0, s1 = shard_range(len(inds), support_batch, world, rank)
     q0, q1 = shard_range(len(lines), batch_size, world, rank)
+    if base_rw is not None:
+        result_kwargs.update(base_rw=base_rw, base_rows=list(cfg._real_base_ids))
 
     def evaluate(model, epoch):
         mb = MetaBatcher(metalines, inds, classes=classes, train=False, ensemble=True, with_ids=True)
@@ -96,11 +102,19 @@ def main():
     ap.add_argument('--eval-devkit', default=None)
     ap.add_argument('--eval-year', default='2007')
     ap.add_argument('--eval-coco-annotations', default=None)
+    ap.add_argument('--eval-base-rw', default=None)
     opts = ap.parse_args()
-    if len(opts.args) != 4 or (opts.eval_devkit is not None and opts.eval_coco_annotations is not None):
+    scored = opts.eval_devkit is not None or opts.eval_coco_annotations is not None
+    if len(opts.args) != 4 or (opts.eval_devkit is not None and opts.eval_coco_annotations is not None) or \
+            (opts.eval_base_rw is not None and not scored):
+        if opts.eval_base_rw is not None and not scored:
+            print('--eval-base-rw needs --eval-devkit or --eval-coco-annotations')
         print('Usage:')
         print('python tools/train_meta_b200.py datacfg darknetcfg learnetcfg weightfile '
-              '[--eval-devkit DIR [--eval-year Y] | --eval-coco-annotations JSON]')
+              '[--eval-devkit DIR [--eval-year Y] | --eval-coco-annotations JSON] [--eval-base-rw PATH]')
+        return 1
+    if opts.eval_base_rw is not None and not os.path.isfile(opts.eval_base_rw):
+        print('--eval-base-rw: no such file: %s' % opts.eval_base_rw)
         return 1
     argv = [sys.argv[0]] + opts.args
     from fewshot_detection_b200.cfg import cfg, parse_cfg
@@ -129,6 +143,10 @@ def main():
     per_rank = batch_size // world
     steps = [float(s) for s in net_options['steps'].split(',')]
     scales = [float(s) for s in net_options['scales'].split(',')]
+    base_rw = None
+    if opts.eval_base_rw is not None:             # checked against the model before training starts
+        from fewshot_detection_b200 import valid as VA
+        base_rw = VA.load_reweighting_vectors(opts.eval_base_rw, VA.reweighting_vector_shapes(learnetcfg, len(cfg.classes)))
 
     model = Darknet(darknetcfg, learnetcfg)
     if os.path.exists(argv[4]):
@@ -174,7 +192,7 @@ def main():
     if opts.eval_devkit is not None or opts.eval_coco_annotations is not None:
         state = random.getstate(), np.random.get_state()          # the training lists' draws stay as without it
         evaluate = checkpoint_evaluator(data_options, opts.eval_devkit, opts.eval_year, opts.eval_coco_annotations,
-                                        world, rank)
+                                        world, rank, base_rw=base_rw)
         random.setstate(state[0])
         np.random.set_state(state[1])
     tr = T.MetaTrainer(model, optimizer, float(net_options['learning_rate']) / factor, batch_size, steps, scales,

@@ -4,6 +4,7 @@ one run, with the detections scored on the GPU where decode and NMS leave them.
 
     python tools/valid_ensemble_b200.py datacfg darknetcfg learnetcfg weightfile [--devkit DIR] [--write-results]
                                         [--coco-annotations instances_val2014.json] [--write-coco-results PATH]
+                                        [--base-rw PATH] [--save-rw PATH]
 
 The `.data` file is read as tools/train_meta_b200.py reads it: `valid` (image list), `meta` (support dictionary), the
 class list and the `novel` / `novelid` split.  The support images of every class are run through the reweighting net
@@ -21,6 +22,16 @@ reference.
                    lines for all, base and novel classes, and the AP@[.5:.95] of each class.
 --write-coco-results PATH
                    writes the standard COCO results json of the same detections (with --coco-annotations).
+--base-rw PATH     the reference's `use_baserw` mode (valid_ensemble.py:108-119): after the ensemble, the rows of the
+                   base classes (the classes that are not novel) are replaced by those of the stored vectors in PATH,
+                   so that after k-shot fine-tuning the base classes are detected with vectors averaged over a large
+                   support set while the novel classes keep their k-shot ones.  The reference reads
+                   data/rws/voc_novel0_.pkl; here the path is always given.  The file is checked against the model
+                   before the model is built.  Result files go to results/<backup>/ene_<ckpt>.
+--save-rw PATH     writes the ensembled vectors before any substitution, in the reference's format (a pickled list
+                   of one float32 [n_cls, C, 1, 1] numpy array per dynamic layer, rows in class-list order): the file
+                   --base-rw reads, e.g. from a run whose `meta` is the full support dictionary.  Alone, only the
+                   support pass runs.
 
 Ranking differs from the reference's file-based evaluation only for detections whose printed confidences tie: they
 keep result-file order here (voc_eval.DeviceVocEval).
@@ -42,14 +53,25 @@ def read_list(path):
         return [l.rstrip() for l in f.readlines() if l.strip()]
 
 
-def result_prefix(weightfile):
-    """valid_ensemble.py:15-21: results/<directory of the weight file>/ene<weight file stem>."""
+def result_prefix(weightfile, base_rw=False):
+    """valid_ensemble.py:15-22: results/<directory of the weight file>/ene<weight file stem>, ene_<stem> with stored
+    base-class vectors."""
     ckpt = os.path.basename(weightfile).split('.')[0]
     backup = os.path.basename(os.path.dirname(os.path.abspath(weightfile)))
-    return os.path.join('results', backup, 'ene' + ckpt)
+    return os.path.join('results', backup, ('ene_' if base_rw else 'ene') + ckpt)
 
 
-def main(argv=None):
+def load_base_rw(path, datacfg, learnetcfg):
+    """The stored vectors of --base-rw, checked against the class list and reweighting net of the cfgs."""
+    from fewshot_detection_b200.cfg import cfg, parse_cfg
+    from fewshot_detection_b200.utils import read_data_cfg
+    from fewshot_detection_b200 import valid as VA
+    cfg.config_data(read_data_cfg(datacfg))
+    return VA.load_reweighting_vectors(path, VA.reweighting_vector_shapes(parse_cfg(learnetcfg), len(cfg.classes)))
+
+
+def parse_args(argv=None):
+    """The checked arguments and the --base-rw vectors (None without it), before any GPU work."""
     ap = argparse.ArgumentParser(description=__doc__.split('\n')[0])
     ap.add_argument('datacfg')
     ap.add_argument('darknetcfg')
@@ -62,16 +84,32 @@ def main(argv=None):
     ap.add_argument('--write-coco-results', default=None, help='COCO results json to write (with --coco-annotations)')
     ap.add_argument('--batch-size', type=int, default=64, help='query images per forward')
     ap.add_argument('--support-batch', type=int, default=64, help='support images per reweighting-net forward')
+    ap.add_argument('--base-rw', default=None, help='stored vectors file: detect the base classes with its rows')
+    ap.add_argument('--save-rw', default=None, help='write the ensembled vectors to this file')
     args = ap.parse_args(argv)
-    if args.devkit is None and not args.write_results and args.coco_annotations is None:
-        ap.error('nothing to do: give --devkit, --coco-annotations and/or --write-results')
+    if args.devkit is None and not args.write_results and args.coco_annotations is None and args.save_rw is None:
+        ap.error('nothing to do: give --devkit, --coco-annotations, --write-results and/or --save-rw')
     if args.coco_annotations is not None and args.devkit is not None:
         ap.error('--devkit and --coco-annotations score the same detections twice: give one')
     if args.write_coco_results is not None and args.coco_annotations is None:
         ap.error('--write-coco-results needs --coco-annotations (the COCO image and category ids)')
     if args.coco_annotations is not None and args.write_results:
         ap.error('--write-results writes the VOC result files; with --coco-annotations use --write-coco-results')
+    base_rw = None
+    if args.base_rw is not None:                      # a bad file fails here, before the support pass
+        if not os.path.isfile(args.base_rw):
+            ap.error('--base-rw: no such file: %s' % args.base_rw)
+        try:
+            base_rw = load_base_rw(args.base_rw, args.datacfg, args.learnetcfg)
+        except (OSError, ValueError) as e:
+            ap.error('--base-rw: %s' % e)
+    if args.save_rw is not None:
+        os.makedirs(os.path.dirname(os.path.abspath(args.save_rw)), exist_ok=True)
+    return args, base_rw
 
+
+def main(argv=None):
+    args, base_rw = parse_args(argv)
     import torch
 
     world = int(os.environ.get('WORLD_SIZE', '1'))
@@ -82,16 +120,17 @@ def main(argv=None):
         torch.cuda.set_device(local)
         dist.init_process_group('nccl', device_id=torch.device('cuda', local))
         try:
-            return run(args, world, dist.get_rank())
+            return run(args, world, dist.get_rank(), base_rw)
         finally:
             torch.cuda.synchronize()
             dist.destroy_process_group()
     torch.cuda.set_device(0)
-    return run(args, 1, 0)
+    return run(args, 1, 0, base_rw)
 
 
-def run(args, world, rank):
-    """The evaluation on this process's shard (the whole set when world == 1)."""
+def run(args, world, rank, base_rw=None):
+    """The evaluation on this process's shard (the whole set when world == 1); `base_rw` are the stored vectors of
+    --base-rw (load_base_rw)."""
     import torch
     from fewshot_detection_b200.cfg import cfg, parse_cfg
     from fewshot_detection_b200.utils import read_data_cfg, logging
@@ -133,20 +172,22 @@ def run(args, world, rank):
     if args.write_results and not lead:
         out = True                                    # this rank's lines go to rank 0
     elif args.write_results:
-        prefix = result_prefix(args.weightfile)
+        prefix = result_prefix(args.weightfile, base_rw is not None)
         if not os.path.exists(prefix):
             os.makedirs(prefix)
         logging('saving to: %s' % prefix)
         out = [open(os.path.join(prefix, 'comp4_det_test_%s.txt' % c), 'w') for c in classes]
+    rw = dict(base_rw=base_rw, base_rows=list(cfg._real_base_ids) if base_rw is not None else None, save_rw=args.save_rw)
     try:
         if args.devkit is None and args.coco_annotations is None:
             n_cls = len(classes)
+            dw = VA.evaluation_dynamic_weights(m, meta_batches, n_cls, sharded, **rw)
+            if not args.write_results:                # --save-rw alone: the support pass only
+                return 0
             if not sharded:
-                dw = VA.ensemble_dynamic_weights(m, meta_batches, n_cls)
                 for data, ids, sizes in image_batches():
                     VA.write_detections(out, VA.detect(m, data, dw, n_cls), ids, sizes, n_cls)
                 return 0
-            dw = VA.sharded_ensemble_dynamic_weights(m, meta_batches, n_cls)
             mine = dict((i, []) for i in range(n_cls))
             for data, ids, sizes in image_batches():
                 for i, l in VA.detection_lines(VA.detect(m, data, dw, n_cls), ids, sizes, n_cls).items():
@@ -170,7 +211,7 @@ def run(args, world, rank):
             recs = rank0_first(load) if sharded else load()    # rank 0 writes the cache, the others read it
             ev = VE.DeviceVocEval(classes, imagenames, recs)
             result_kwargs = dict(use_07_metric=int(args.year) < 2010, novel_classes=novel)
-        r = VA.score_batches(m, meta_batches, image_batches(), ev, out, sharded, **result_kwargs)
+        r = VA.score_batches(m, meta_batches, image_batches(), ev, out, sharded, **rw, **result_kwargs)
     finally:
         for f in out if isinstance(out, list) else [out]:
             if f is not None and f is not True:
@@ -180,7 +221,13 @@ def run(args, world, rank):
     if args.coco_annotations is not None:
         print_coco(r, classes, novel)
         return 0
-    print('VOC07 metric? ' + ('Yes' if result_kwargs['use_07_metric'] else 'No'))
+    print_voc(r, classes, novel, result_kwargs['use_07_metric'])
+    return 0
+
+
+def print_voc(r, classes, novel, use_07_metric):
+    """scripts/voc_eval.py's lines: the AP of each class, then the mean, base and novel mean AP."""
+    print('VOC07 metric? ' + ('Yes' if use_07_metric else 'No'))
     for c in classes:
         print('AP for {} = {:.4f}{}'.format(c, r['ap'][c], ' (novel)' if c in novel else ''))
     print('Mean AP = {:.4f}'.format(r['mean']))
@@ -188,7 +235,6 @@ def run(args, world, rank):
         print('Mean Base AP = {:.4f}'.format(r['mean_base']))
     if r['mean_novel'] is not None:
         print('Mean Novel AP = {:.4f}'.format(r['mean_novel']))
-    return 0
 
 
 def print_coco(r, classes, novel):
