@@ -73,6 +73,8 @@ SIGNATURES = {
     'fsdet_region_detect': ('ppiiiiiiiidpppp', 'i'),
     'fsdet_nms': ('ppiiiidppp', 'i'),
     'fsdet_nms_boxes64': ('ppiidppp', 'i'),
+    'fsdet_detect_select_workspace_bytes': ('ii', 'z'),
+    'fsdet_detect_select': ('pppiiiiipipzpppppp', 'i'),
     'fsdet_rw_running_mean': ('pppppiiip', 'i'),
     'fsdet_voc_round6': ('pppqp', 'i'),
     'fsdet_voc_gather': ('pppiiiiiippppqpipp', 'i'),

@@ -11,6 +11,7 @@
 // `det_conf * cls_conf > conf_thresh`, the normalisation x/w, the NMS key float32(1 - det_conf) and the NMS IoUs
 // (utils.bbox_iou, utils.py:21-52, operation order kept, no FMA contraction).
 #include "common.cuh"
+#include "eval_sort.cuh"
 
 // tools/host_emul compiles this file with g++ (threads = OS threads) to test the block-level logic without a GPU
 #ifdef FSDET_HOST_EMULATION
@@ -242,6 +243,185 @@ static inline int next_pow2(int v) {
     return p;
 }
 
+// ---- per-image selection of the meta detector's NMS survivors (fsdet_detect_select) ---------------------------------
+// Every survivor of the batch is a record, numbered in row order (image, class) and then NMS rank.  One stable LSD
+// radix sort (eval_sort.cuh) orders the records by ~bits(prob) (low word, then high word), then by image: within an
+// image, prob descending with ties in record order, i.e. class ascending, then NMS rank ascending.  The record count is
+// only known on the device, so the sort's grid covers every candidate slot and its kernels read the count.
+struct SelectWorkspace {
+    int32_t* row_off;                                 // [N + 1] first record of each row
+    long long* n_rec;                                 // [1] records of the batch
+    int32_t* rec;                                     // [N * cap] record -> row * cap + candidate slot
+    uint32_t* keys[2];
+    int32_t* vals[2];
+    unsigned long long* cnt;
+    unsigned long long* part;
+    size_t bytes;
+};
+
+static SelectWorkspace select_workspace_layout(void* base, int N, int cap) {
+    const long long n = (long long)N * cap;
+    const int ntiles = ceil_div(n, kVocTile);
+    const size_t n_cnt = (size_t)256 * ntiles;
+    const size_t n_part = (size_t)ceil_div((long long)n_cnt, kVocTile) + 1;
+    SelectWorkspace w;
+    unsigned char* p = static_cast<unsigned char*>(base);
+    size_t off = 0;
+    auto take = [&](size_t bytes) { unsigned char* q = p ? p + off : nullptr; off += voc_align(bytes); return q; };
+    w.row_off = reinterpret_cast<int32_t*>(take((size_t)(N + 1) * 4));
+    w.n_rec = reinterpret_cast<long long*>(take(8));
+    w.rec = reinterpret_cast<int32_t*>(take((size_t)n * 4));
+    w.keys[0] = reinterpret_cast<uint32_t*>(take((size_t)n * 4));
+    w.keys[1] = reinterpret_cast<uint32_t*>(take((size_t)n * 4));
+    w.vals[0] = reinterpret_cast<int32_t*>(take((size_t)n * 4));
+    w.vals[1] = reinterpret_cast<int32_t*>(take((size_t)n * 4));
+    w.cnt = reinterpret_cast<unsigned long long*>(take(n_cnt * 8));
+    w.part = reinterpret_cast<unsigned long long*>(take(n_part * 8));
+    w.bytes = off;
+    return w;
+}
+
+// One block: the first record of every row (exclusive prefix of keep_count) and the batch's record count.
+__global__ void __launch_bounds__(kDetThreads) select_offsets_kernel(const int32_t* __restrict__ keep_count, int N,
+                                                                     int cap, int32_t* __restrict__ row_off,
+                                                                     long long* __restrict__ n_rec) {
+    __shared__ unsigned long long s[kVocThreads];
+    unsigned long long base = 0;
+    for (int r0 = 0; r0 < N; r0 += kDetThreads) {
+        const int r = r0 + threadIdx.x;
+        const int c = r < N ? min(max(keep_count[r], 0), cap) : 0;
+        unsigned long long chunk;
+        const unsigned long long pre = voc_block_scan((unsigned long long)c, s, chunk);
+        if (r < N) row_off[r] = (int32_t)(base + pre);
+        base += chunk;
+    }
+    if (threadIdx.x == 0) {
+        row_off[N] = (int32_t)base;
+        *n_rec = (long long)base;
+    }
+}
+
+// One block per row: survivor k (NMS rank) becomes record row_off[r] + k.
+__global__ void __launch_bounds__(kDetThreads) select_compact_kernel(const int32_t* __restrict__ keep,
+                                                                     const int32_t* __restrict__ row_off, int cap,
+                                                                     int32_t* __restrict__ rec) {
+    const int r = blockIdx.x;
+    const int o = row_off[r], n = row_off[r + 1] - o;
+    for (int k = threadIdx.x; k < n; k += kDetThreads) rec[o + k] = r * cap + keep[(size_t)r * cap + k];
+}
+
+// valid.detection_lines' prob = det_conf * cls_conf, float64 (exact: a product of two float32 values)
+__device__ __forceinline__ double select_prob(const float* c) { return __dmul_rn((double)c[4], (double)c[5]); }
+
+// Key word `word` of the records taken in the order perm (nullptr: record order): 0 / 1 the low / high half of
+// ~bits(prob) (the bits of a non-negative double order like its value, so ascending ~bits is descending prob),
+// 2 the image.
+__global__ void __launch_bounds__(kDetThreads) select_keys_kernel(const float* __restrict__ cand,
+                                                                  const int32_t* __restrict__ rec,
+                                                                  const int32_t* __restrict__ perm,
+                                                                  const long long* __restrict__ n_rec, int cap,
+                                                                  int n_cls, int word, uint32_t* __restrict__ keys) {
+    const long long n = *n_rec;
+    for (long long j = (long long)blockIdx.x * kDetThreads + threadIdx.x; j < n; j += (long long)gridDim.x * kDetThreads) {
+        const int id = rec[perm ? perm[j] : j];
+        uint32_t k;
+        if (word == 2) {
+            k = (uint32_t)(id / cap / n_cls);
+        } else {
+            const unsigned long long b = ~(unsigned long long)__double_as_longlong(select_prob(cand + (size_t)id * kCandFloats));
+            k = word ? (uint32_t)(b >> 32) : (uint32_t)b;
+        }
+        keys[j] = k;
+    }
+}
+
+// One block per image: its records are the contiguous run [row_off[b * n_cls], row_off[(b + 1) * n_cls]) of the sorted
+// order; the first max_det become the image's result, in pixels with valid.detection_lines' float64 arithmetic.
+// Slots past the count are written as score 0, box 0, class -1.
+__global__ void __launch_bounds__(kDetThreads) select_write_kernel(const float* __restrict__ cand,
+                                                                   const int32_t* __restrict__ rec,
+                                                                   const int32_t* __restrict__ order,
+                                                                   const int32_t* __restrict__ row_off,
+                                                                   const int32_t* __restrict__ sizes, int cap, int n_cls,
+                                                                   int H, int W, int max_det, double* __restrict__ score,
+                                                                   double* __restrict__ box, int32_t* __restrict__ cls,
+                                                                   int32_t* __restrict__ count, int32_t* __restrict__ total) {
+    const int b = blockIdx.x;
+    const int s0 = row_off[b * n_cls], s1 = row_off[(b + 1) * n_cls];
+    const int n = min(s1 - s0, max_det);
+    const double width = (double)sizes[2 * b], height = (double)sizes[2 * b + 1];
+    for (int t = threadIdx.x; t < max_det; t += kDetThreads) {
+        const size_t o = (size_t)b * max_det + t;
+        double4 bx = make_double4(0.0, 0.0, 0.0, 0.0);
+        double sc = 0.0;
+        int c = -1;
+        if (t < n) {
+            const int id = rec[order[s0 + t]];
+            const float* q = cand + (size_t)id * kCandFloats;
+            const double x = __ddiv_rn((double)q[0], (double)W), y = __ddiv_rn((double)q[1], (double)H);
+            const double w2 = __ddiv_rn(__ddiv_rn((double)q[2], (double)W), 2.0);
+            const double h2 = __ddiv_rn(__ddiv_rn((double)q[3], (double)H), 2.0);
+            bx = make_double4(__dmul_rn(__dsub_rn(x, w2), width), __dmul_rn(__dsub_rn(y, h2), height),
+                              __dmul_rn(__dadd_rn(x, w2), width), __dmul_rn(__dadd_rn(y, h2), height));
+            sc = select_prob(q);
+            c = (id / cap) % n_cls;
+        }
+        score[o] = sc;
+        box[o * 4 + 0] = bx.x;
+        box[o * 4 + 1] = bx.y;
+        box[o * 4 + 2] = bx.z;
+        box[o * 4 + 3] = bx.w;
+        cls[o] = c;
+    }
+    if (threadIdx.x == 0) {
+        count[b] = n;
+        total[b] = s1 - s0;
+    }
+}
+
+static int detect_select_impl(const float* cand, const int32_t* keep, const int32_t* keep_count, int N, int cap, int H,
+                              int W, int n_cls, const int32_t* sizes, int max_det, void* workspace, double* score,
+                              double* box, int32_t* cls, int32_t* count, int32_t* total, cudaStream_t st) {
+    (void)st;
+    const SelectWorkspace w = select_workspace_layout(workspace, N, cap);
+    const int B = N / n_cls;
+    const long long n_slots = (long long)N * cap;
+    const int ntiles = ceil_div(n_slots, kVocTile);
+    const int kgrid = ceil_div(n_slots, kDetThreads) < 2048 ? ceil_div(n_slots, kDetThreads) : 2048;
+    VOC_LAUNCH(1, kDetThreads, select_offsets_kernel, keep_count, N, cap, w.row_off, w.n_rec);
+    VOC_CHECK("detect_select_offsets");
+    VOC_LAUNCH(N, kDetThreads, select_compact_kernel, keep, w.row_off, cap, w.rec);
+    VOC_CHECK("detect_select_compact");
+    int img_bits = 0;
+    while ((1 << img_bits) < B) ++img_bits;
+    const int word_passes[3] = {4, 4, (img_bits + 7) / 8};
+    const int32_t* perm = nullptr;                    // record order
+    int cur = 0;
+    for (int word = 0; word < 3; ++word) {
+        if (word_passes[word] == 0) continue;
+        // the word's keys in the current order go to the key buffer the next pass does not write
+        VOC_LAUNCH(kgrid, kDetThreads, select_keys_kernel, cand, w.rec, perm, w.n_rec, cap, n_cls, word, w.keys[cur ^ 1]);
+        VOC_CHECK("detect_select_keys");
+        const uint32_t* kin = w.keys[cur ^ 1];
+        for (int p = 0; p < word_passes[word]; ++p) {
+            VOC_LAUNCH(ntiles, kVocThreads, voc_radix_hist_kernel, kin, (int)n_slots, 8 * p, ntiles, w.cnt, w.n_rec);
+            VOC_CHECK("detect_select_radix_hist");
+            const int rc = voc_scan(w.cnt, (long long)256 * ntiles, w.part, 0, st);
+            if (rc) return rc;
+            VOC_LAUNCH(ntiles, kVocThreads, voc_radix_scatter_kernel, kin, perm, (int)n_slots, 8 * p, ntiles, w.cnt,
+                       w.keys[cur], w.vals[cur], w.n_rec);
+            VOC_CHECK("detect_select_radix_scatter");
+            kin = w.keys[cur];
+            perm = w.vals[cur];
+            cur ^= 1;
+        }
+    }
+    VOC_LAUNCH(B, kDetThreads, select_write_kernel, cand, w.rec, perm, w.row_off, sizes, cap, n_cls, H, W, max_det, score,
+               box, cls, count, total);
+    VOC_CHECK("detect_select_write");
+    return 0;
+}
+
 }  // namespace fsdet
 
 #ifndef FSDET_HOST_EMULATION
@@ -288,6 +468,27 @@ extern "C" int fsdet_nms(const float* cand, const int32_t* count, int N, int cap
 extern "C" int fsdet_nms_boxes64(const double* boxes, const int32_t* count, int N, int cap, double nms_thresh,
                                  int32_t* keep, int32_t* keep_count, void* stream) {
     return launch_nms(nullptr, boxes, count, N, cap, 1, 1, nms_thresh, keep, keep_count, stream);
+}
+
+extern "C" size_t fsdet_detect_select_workspace_bytes(int N, int cap) {
+    if (N < 0 || cap <= 0) return 0;
+    return select_workspace_layout(nullptr, N, cap).bytes;
+}
+
+extern "C" int fsdet_detect_select(const float* cand, const int32_t* keep, const int32_t* keep_count, int N, int cap, int H,
+                                   int W, int n_cls, const int32_t* sizes, int max_det, void* workspace,
+                                   size_t workspace_bytes, double* score, double* box, int32_t* cls, int32_t* count,
+                                   int32_t* total, void* stream) {
+    FSDET_CHECK_ARG(cand && keep && keep_count && sizes && workspace && score && box && cls && count && total,
+                    "detect_select: null pointer");
+    FSDET_CHECK_ARG(n_cls > 0 && N > 0 && N % n_cls == 0, "detect_select: %d rows are not images x %d classes", N, n_cls);
+    FSDET_CHECK_ARG(cap > 0 && H > 0 && W > 0 && max_det > 0, "detect_select: bad shape");
+    FSDET_CHECK_ARG((long long)N * cap < 0x7fffffffll, "detect_select: %d rows x %d candidates do not fit int32", N, cap);
+    FSDET_CHECK_ARG(workspace_bytes >= select_workspace_layout(nullptr, N, cap).bytes,
+                    "detect_select: workspace of %zu bytes, %zu needed", workspace_bytes,
+                    select_workspace_layout(nullptr, N, cap).bytes);
+    return detect_select_impl(cand, keep, keep_count, N, cap, H, W, n_cls, sizes, max_det, workspace, score, box, cls,
+                              count, total, (cudaStream_t)stream);
 }
 
 extern "C" int fsdet_rw_running_mean(float* enews, const int32_t* cnt_in, int32_t* cnt_out, const float* dw,

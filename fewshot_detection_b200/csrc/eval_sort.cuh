@@ -1,5 +1,5 @@
 // Block scan, stable LSD radix sort, uint64 prefix sums, the gather plan and the pool merge shared by the device
-// evaluators (voc_eval.cu, coco_eval.cu), with the launch macros that run them either on the device or under host emulation (tools/host_emul).
+// evaluators (voc_eval.cu, coco_eval.cu) and the per-image selection (detect.cu), with the launch macros that run them either on the device or under host emulation (tools/host_emul).
 // Internal linkage: every evaluator translation unit gets its own copy of the kernels.
 #pragma once
 #include "common.cuh"
@@ -29,9 +29,13 @@ __device__ __forceinline__ unsigned long long voc_block_scan(unsigned long long 
 }
 
 // ---- stable LSD radix sort of (rank_key, record index), 8 bits per pass ----------------------------------------
+// n_live (optional, device): the number of items when only the device knows it; the grid then covers n >= *n_live
+// items and the tiles past *n_live sort nothing.
 __global__ void __launch_bounds__(kVocThreads) voc_radix_hist_kernel(const uint32_t* __restrict__ keys, int n, int shift,
-                                                                     int ntiles, unsigned long long* __restrict__ cnt) {
+                                                                     int ntiles, unsigned long long* __restrict__ cnt,
+                                                                     const long long* __restrict__ n_live = nullptr) {
     __shared__ int h[256];
+    if (n_live && *n_live < n) n = (int)*n_live;
     h[threadIdx.x] = 0;
     __syncthreads();
     const int tile = blockIdx.x;
@@ -50,8 +54,10 @@ __global__ void __launch_bounds__(kVocThreads) voc_radix_scatter_kernel(const ui
                                                                         int shift, int ntiles,
                                                                         const unsigned long long* __restrict__ cnt_scan,
                                                                         uint32_t* __restrict__ keys_out,
-                                                                        int32_t* __restrict__ vals_out) {
+                                                                        int32_t* __restrict__ vals_out,
+                                                                        const long long* __restrict__ n_live = nullptr) {
     __shared__ unsigned long long base[256];
+    if (n_live && *n_live < n) n = (int)*n_live;
     __shared__ int wc[kVocThreads / 32][256];
     __shared__ int tot[256];
     const int tile = blockIdx.x, lane = threadIdx.x & 31, w = threadIdx.x >> 5;

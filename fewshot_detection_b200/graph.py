@@ -1,4 +1,4 @@
-"""CUDA-graph capture of the whole meta-training step.
+"""CUDA-graph capture of the whole meta-training step, and of the detection pass (GraphedDetect, at the end).
 
 The eager step issues ~3,000 kernel launches through ctypes (tens of ms of host time per step at config 2, about
 as long as the GPU work).  `GraphedTrainStep` captures forward + RegionLoss(V2) + backward (+ the gradient
@@ -220,3 +220,83 @@ class GraphedTrainStep(object):
         self._check_and_arm(e.counters)
         self.loss = e.loss
         return e.loss
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+class _DetectEntry(object):
+    __slots__ = ('graph', 'x', 'sizes', 'out')
+
+
+class GraphedDetect(object):
+    """valid.detect_images replayed as one CUDA graph per (batch, side): the query forward (detect_forward), the decode
+    and NMS (fsdet_region_detect, fsdet_nms) and the per-image selection (fsdet_detect_select).
+
+    The model must be in eval mode; its parameters and buffers are only read.  The reweighting vectors are copied
+    once into a static buffer, the anchors are staged on the device once, and every call copies the batch and the
+    image sizes into static buffers and replays.  A batch of fewer than `batch` images is padded to `batch` with zero
+    images whose results are dropped; the forward's tiling depends on the batch size, so its results are those of the
+    eager pass over the padded batch, which can differ in the last bits from an eager pass over the real images
+    alone.  Each (batch, side) is run once eagerly (lazy planning) and then captured; the
+    capture is strict: a host synchronisation or pageable copy inside the pass fails the capture instead of falling
+    back to eager launches.
+
+    `__call__(data, sizes)` returns a utils.ImageDetections over this graph's static result buffer: it is valid until
+    the next call with the same side, so read it (`.lists()`) or copy it first."""
+
+    def __init__(self, model, dynamic_weights, batch, side, n_cls, conf=0.5, nms=0.4, max_det=100):
+        if model.training:
+            raise ValueError('GraphedDetect needs the model in eval mode')
+        self.model, self.batch, self.side = model, int(batch), int(side)
+        self.n_cls, self.conf, self.nms, self.max_det = int(n_cls), float(conf), float(nms), int(max_det)
+        self.device = next(model.parameters()).device
+        dw = dynamic_weights if isinstance(dynamic_weights, (list, tuple)) else [dynamic_weights]
+        self.dw = [t.detach().to(self.device, torch.float32).clone() for t in dw]
+        if self.dw[0].size(0) != self.n_cls:
+            raise ValueError('vectors for %d classes, n_cls = %d' % (self.dw[0].size(0), self.n_cls))
+        self.anchors = torch.tensor([float(a) for a in model.anchors], dtype=torch.float32).to(self.device)
+        self.entries = {}                              # (batch, side) -> _DetectEntry
+        self.pool = None
+        self.captures = 0
+        self._capture((self.batch, self.side))
+
+    def _pass(self, e):
+        from . import valid as VA
+        dets = VA.detect(self.model, e.x, self.dw, self.n_cls, self.conf, self.nms, anchors_dev=self.anchors)
+        dets.select(self.n_cls, e.sizes, self.max_det, out=e.out)
+
+    def _capture(self, key):
+        from .utils import ImageDetections
+        B, side = key
+        e = _DetectEntry()
+        e.x = torch.zeros(B, 3, side, side, dtype=torch.float32, device=self.device)
+        e.sizes = torch.full((B, 2), side, dtype=torch.int32, device=self.device)
+        e.out = ImageDetections.empty(B, self.max_det, self.device)
+        self._pass(e)                                  # eager: the forward's per-shape plans are built here
+        torch.cuda.synchronize()
+        e.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(e.graph, pool=self.pool, capture_error_mode='thread_local'):
+            self._pass(e)
+        if self.pool is None:
+            self.pool = e.graph.pool()
+        self.captures += 1
+        self.entries[key] = e
+        return e
+
+    def __call__(self, data, sizes):
+        """data: float32 [b, 3, side, side] (b <= batch, any device), sizes: b (width, height) pairs."""
+        b = int(data.size(0))
+        if data.dim() != 4 or data.size(1) != 3 or data.size(2) != data.size(3):
+            raise ValueError('data must be [b, 3, side, side], got %s' % (tuple(data.shape),))
+        if not 0 < b <= self.batch or len(sizes) != b:
+            raise ValueError('%d images and %d sizes for a batch of %d' % (b, len(sizes), self.batch))
+        key = (self.batch, int(data.size(2)))
+        e = self.entries.get(key)
+        if e is None:
+            e = self._capture(key)
+        e.x[:b].copy_(data, non_blocking=True)
+        if b < self.batch:
+            e.x[b:].zero_()
+        size_rows = [[int(w), int(h)] for w, h in sizes] + [[key[1], key[1]]] * (self.batch - b)
+        e.sizes.copy_(torch.tensor(size_rows, dtype=torch.int32))   # pageable: the host list is free on return
+        e.graph.replay()
+        return e.out.narrow(b)

@@ -1,4 +1,5 @@
 """Small host helpers of the reference's utils.py that the training driver uses."""
+import struct
 import time
 
 
@@ -19,6 +20,57 @@ def read_data_cfg(datacfg):
 
 def logging(message):
     print('%s %s' % (time.strftime("%Y-%m-%d %H:%M:%S", time.localtime()), message))
+
+
+def load_class_names(namesfile):
+    """utils.py:392-399: one class name per line, trailing whitespace stripped (blank lines included)."""
+    with open(namesfile, 'r') as fp:
+        return [line.rstrip() for line in fp.readlines()]
+
+
+def _image_type(head):
+    """The type `imghdr.what` reports for the first bytes of a file, for the types get_image_size reads."""
+    if head[:8] == b'\x89PNG\r\n\x1a\n':
+        return 'png'
+    if head[:6] in (b'GIF87a', b'GIF89a'):
+        return 'gif'
+    if head[6:10] in (b'JFIF', b'Exif') or head[:4] == b'\xff\xd8\xff\xdb':
+        return 'jpeg'
+    return None
+
+
+def get_image_size(fname):
+    """utils.py:536-569: (width, height) from the header of a PNG, GIF or JPEG file, without decoding it; None for
+    any other file, a file shorter than 24 bytes or a JPEG without a frame header."""
+    with open(fname, 'rb') as fhandle:
+        head = fhandle.read(24)
+        if len(head) != 24:
+            return None
+        kind = _image_type(head)
+        if kind == 'png':
+            if struct.unpack('>i', head[4:8])[0] != 0x0d0a1a0a:
+                return None
+            width, height = struct.unpack('>ii', head[16:24])
+        elif kind == 'gif':
+            width, height = struct.unpack('<HH', head[6:10])
+        elif kind == 'jpeg':
+            try:
+                fhandle.seek(0)                     # walk the segments up to the first SOFn marker
+                size, ftype = 2, 0
+                while not 0xc0 <= ftype <= 0xcf:
+                    fhandle.seek(size, 1)
+                    byte = fhandle.read(1)
+                    while ord(byte) == 0xff:
+                        byte = fhandle.read(1)
+                    ftype = ord(byte)
+                    size = struct.unpack('>H', fhandle.read(2))[0] - 2
+                fhandle.seek(1, 1)                  # the sample precision byte
+                height, width = struct.unpack('>HH', fhandle.read(4))
+            except Exception:
+                return None
+        else:
+            return None
+        return width, height
 
 
 # --------------------------------------------------------------------------------------------------------------------
@@ -141,6 +193,99 @@ class Detections(object):
                 box[4] = 0
         return [row[s] for s in slots]
 
+    # ---- per-image result (meta detector)
+    def select(self, n_cls, sizes, max_det=100, out=None):
+        """The first `max_det` NMS survivors of every image, over all its class rows, ordered by prob = det_conf *
+        cls_conf descending, then class, then NMS rank, with the boxes in pixels (fsdet_detect_select): an
+        ImageDetections, still on the device, of fixed shape.  Rows are (image, class) pairs, image-major, as
+        get_region_boxes_v2 makes them; `.nms()` must have run.  sizes: (width, height) per image, a sequence or an
+        int32 [B, 2] tensor on the device.  out (optional): an ImageDetections of the same B and max_det to write into
+        (a CUDA graph's static result)."""
+        import torch
+        from ._lib import call, lib, ptr
+        if self.keep is None:
+            raise ValueError('select needs the NMS survivors: call .nms(thresh) first')
+        if self.nC != 1:
+            raise ValueError('select takes the meta detector\'s rows (one class channel per row), not nC = %d' % self.nC)
+        n_cls, max_det = int(n_cls), int(max_det)
+        if n_cls <= 0 or self.N % n_cls or self.N == 0:
+            raise ValueError('%d rows are not images x %d classes' % (self.N, n_cls))
+        if max_det <= 0:
+            raise ValueError('max_det must be positive, got %d' % max_det)
+        B, dev = self.N // n_cls, self.cand.device
+        if not torch.is_tensor(sizes):
+            sizes = torch.tensor([[int(w), int(h)] for w, h in sizes], dtype=torch.int32).to(dev)
+        if tuple(sizes.shape) != (B, 2) or sizes.dtype != torch.int32 or sizes.device != dev:
+            raise ValueError('sizes must be int32 [%d, 2] on %s, got %s %s on %s'
+                             % (B, dev, sizes.dtype, tuple(sizes.shape), sizes.device))
+        sizes = sizes.contiguous()
+        if out is None:
+            out = ImageDetections.empty(B, max_det, dev)
+        elif (out.B, out.max_det) != (B, max_det):
+            raise ValueError('out holds %d x %d results, the batch needs %d x %d' % (out.B, out.max_det, B, max_det))
+        cap = self.A * self.H * self.W
+        ws_bytes = int(lib.fsdet_detect_select_workspace_bytes(self.N, cap))
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        call('fsdet_detect_select', ptr(self.cand), ptr(self.keep), ptr(self.keep_count), self.N, cap, self.H, self.W,
+             n_cls, ptr(sizes), max_det, ptr(ws), ws_bytes, ptr(out.score), ptr(out.box), ptr(out.cls), ptr(out.count),
+             ptr(out.total), _stream())
+        return out
+
+
+class ImageDetections(object):
+    """Per-image detections of a batch (Detections.select), device resident, fixed shape:
+    score float64 [B, max_det], box float64 [B, max_det, 4] (x1, y1, x2, y2 in pixels), cls int32 [B, max_det],
+    count int32 [B] (valid slots, best first), total int32 [B] (NMS survivors before the max_det cap).
+    Slots past count hold score 0, box 0, class -1.  All five are views of one device buffer, so `.lists()` costs
+    one device-to-host copy.  `n_images` <= B: the images that are results (a padded batch's real images)."""
+
+    def __init__(self, buf, B, max_det, n_images=None):
+        self.buf, self.B, self.max_det = buf, B, max_det
+        self.n_images = B if n_images is None else n_images
+        self.score, self.box, self.cls, self.count, self.total = self._views(buf, B, max_det)
+
+    @staticmethod
+    def _bytes(B, max_det):
+        return B * max_det * 5 * 8 + B * max_det * 4 + 2 * B * 4
+
+    @staticmethod
+    def _views(buf, B, max_det):
+        import torch
+        K = B * max_det
+        f64 = buf[:K * 40].view(torch.float64) if torch.is_tensor(buf) else buf[:K * 40].view('<f8')
+        i32 = buf[K * 40:].view(torch.int32) if torch.is_tensor(buf) else buf[K * 40:].view('<i4')
+        return (f64[:K].reshape(B, max_det), f64[K:].reshape(B, max_det, 4), i32[:K].reshape(B, max_det),
+                i32[K:K + B], i32[K + B:K + 2 * B])
+
+    @classmethod
+    def empty(cls, B, max_det, device):
+        import torch
+        return cls(torch.empty(cls._bytes(B, max_det), dtype=torch.uint8, device=device), B, max_det)
+
+    def narrow(self, n_images):
+        """The same buffer with only the first n_images images as results."""
+        return ImageDetections(self.buf, self.B, self.max_det, n_images)
+
+    def host(self):
+        """numpy (score, box, cls, count, total) of the result images, one device-to-host copy."""
+        score, box, cls, count, total = self._views(self.buf.cpu().numpy(), self.B, self.max_det)
+        n = self.n_images
+        return score[:n], box[:n], cls[:n], count[:n], total[:n]
+
+    def lists(self, class_names=None):
+        """One list per image of (name, prob, x1, y1, x2, y2), best first; the class index instead of the name when
+        class_names is None."""
+        score, box, cls, count, _ = self.host()
+        out = []
+        for b in range(self.n_images):
+            rows = []
+            for k in range(int(count[b])):
+                c = int(cls[b, k])
+                x1, y1, x2, y2 = (float(v) for v in box[b, k])
+                rows.append((class_names[c] if class_names is not None else c, float(score[b, k]), x1, y1, x2, y2))
+            out.append(rows)
+        return out
+
 
 class _Row(list):
     """A row of get_region_boxes(_v2)'s result that remembers where it came from, so that `nms(row, t)` can use
@@ -155,7 +300,8 @@ class _Row(list):
         return len(self) == self._n0 and all(b[4] == s for b, s in zip(self, self._sig))
 
 
-def _detect(output, n_models, v2, conf_thresh, num_classes, anchors, num_anchors, only_objectness, validation):
+def _detect(output, n_models, v2, conf_thresh, num_classes, anchors, num_anchors, only_objectness, validation,
+            anchors_dev=None):
     import torch
     from ._lib import call, ptr
     if not torch.is_tensor(output) or not output.is_cuda:
@@ -175,18 +321,26 @@ def _detect(output, n_models, v2, conf_thresh, num_classes, anchors, num_anchors
     count = torch.zeros(N, dtype=torch.int32, device=dev)
     want_dense = bool(validation) and not only_objectness and nC > 1
     dense = torch.empty(N * cap, nC, dtype=torch.float32, device=dev) if want_dense else None
-    anc = torch.tensor([float(a) for a in anchors], dtype=torch.float32).to(dev)
+    if anchors_dev is None:
+        anc = torch.tensor([float(a) for a in anchors], dtype=torch.float32).to(dev)
+    else:                                             # staged by the caller: no host-to-device copy here
+        anc = anchors_dev
+        assert anc.dtype == torch.float32 and anc.device == dev and anc.numel() == len(anchors) and anc.is_contiguous()
     call('fsdet_region_detect', ptr(output), ptr(anc), N, A, nC, H, W, int(n_models), int(v2), int(bool(only_objectness)),
          float(conf_thresh), ptr(cand), ptr(count), ptr(dense), _stream())
     return Detections(cand, count, dense, N, A, nC, H, W, bool(only_objectness), bool(validation), float(conf_thresh))
 
 
 def region_detections(output, conf_thresh, num_classes, anchors, num_anchors, only_objectness=1, validation=False,
-                      n_models=None):
-    """Device-resident form of get_region_boxes (n_models=None) / get_region_boxes_v2: returns `Detections`."""
+                      n_models=None, anchors_dev=None):
+    """Device-resident form of get_region_boxes (n_models=None) / get_region_boxes_v2: returns `Detections`.
+    anchors_dev (optional): the anchors as a float32 device tensor, staged once by a caller that captures the decode
+    in a CUDA graph (otherwise they are uploaded from the host on every call)."""
     if n_models is None:
-        return _detect(output, 1, 0, conf_thresh, num_classes, anchors, num_anchors, only_objectness, validation)
-    return _detect(output, n_models, 1, conf_thresh, num_classes, anchors, num_anchors, only_objectness, validation)
+        return _detect(output, 1, 0, conf_thresh, num_classes, anchors, num_anchors, only_objectness, validation,
+                       anchors_dev)
+    return _detect(output, n_models, 1, conf_thresh, num_classes, anchors, num_anchors, only_objectness, validation,
+                   anchors_dev)
 
 
 def get_region_boxes(output, conf_thresh, num_classes, anchors, num_anchors, only_objectness=1, validation=False):

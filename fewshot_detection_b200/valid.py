@@ -10,6 +10,9 @@ same files:
     dets = detect(m, data, dw, n_cls)                                    # Detections, NMS done, still on the device
     write_detections(fps, dets, imgids, sizes, n_cls)                    # 'imgid prob x1 y1 x2 y2' per class file
 
+or, for the boxes of each image rather than the evaluation files, detect_images (per-image top max_det over all
+classes, on the device; graph.GraphedDetect replays the same pass as one CUDA graph).
+
 or, without the files, scores them where they are (voc_eval.DeviceVocEval, coco_eval.DeviceCocoEval):
 
     evaluator.add(dets, imgids, sizes); ...; evaluator.result()          # the dict voc_eval.mean_ap returns
@@ -29,6 +32,9 @@ from .utils import region_detections
 
 CONF_THRESH = 0.005   # valid_ensemble.py:137
 NMS_THRESH = 0.45     # valid_ensemble.py:138
+DETECT_CONF_THRESH = 0.5    # detect.py's do_detect(m, img, 0.5, 0.4)
+DETECT_NMS_THRESH = 0.4
+MAX_DET = 100
 
 
 def _st():
@@ -169,13 +175,24 @@ def evaluation_dynamic_weights(m, meta_batches, n_cls, sharded=False, process_gr
     return dynamic_weights
 
 
-def detect(m, data, dynamic_weights, n_cls, conf_thresh=CONF_THRESH, nms_thresh=NMS_THRESH):
+def detect(m, data, dynamic_weights, n_cls, conf_thresh=CONF_THRESH, nms_thresh=NMS_THRESH, anchors_dev=None):
     """valid_ensemble.py:140-162 for one batch: detect_forward -> get_region_boxes_v2(only_objectness=0,
-    validation=1) -> nms for every (image, class) row.  Returns utils.Detections (device resident)."""
+    validation=1) -> nms for every (image, class) row.  Returns utils.Detections (device resident).
+    anchors_dev: see utils.region_detections."""
     with torch.no_grad():
         output = m.detect_forward(data, dynamic_weights)
-    dets = region_detections(output, conf_thresh, m.num_classes, m.anchors, m.num_anchors, 0, 1, n_models=n_cls)
+    dets = region_detections(output, conf_thresh, m.num_classes, m.anchors, m.num_anchors, 0, 1, n_models=n_cls,
+                             anchors_dev=anchors_dev)
     return dets.nms(nms_thresh)
+
+
+def detect_images(m, data, dynamic_weights, n_cls, sizes, conf_thresh=DETECT_CONF_THRESH, nms_thresh=DETECT_NMS_THRESH,
+                  max_det=MAX_DET):
+    """The boxes of every image of a batch: detect, then Detections.select.  sizes[b] = (width, height) of image b
+    (or an int32 [B, 2] device tensor).  Returns utils.ImageDetections, on the device: per image the first max_det
+    boxes over all classes, by prob descending, in pixels; `.lists(class_names)` brings them to the host.  The
+    thresholds default to those of the reference's single-image detection (do_detect: conf 0.5, NMS 0.4)."""
+    return detect(m, data, dynamic_weights, n_cls, conf_thresh, nms_thresh).select(n_cls, sizes, max_det)
 
 
 def detection_lines(dets, imgids, sizes, n_cls, nms_thresh=NMS_THRESH):

@@ -336,6 +336,21 @@ int fsdet_nms(const float* cand, const int32_t* count, int N, int cap, int H, in
  * which utils.nms (utils.py:85) receives boxes from any caller (e.g. utils.do_detect, utils.py:410-458). */
 int fsdet_nms_boxes64(const double* boxes, const int32_t* count, int N, int cap, double nms_thresh, int32_t* keep,
                       int32_t* keep_count, void* stream);
+/* Per-image detections of the meta detector after fsdet_nms: rows n = b*n_cls + i (image b, class i, nC = 1), cand /
+ * keep / keep_count as fsdet_nms leaves them, cap candidates per row (N*cap < 2^31), H x W the head grid.  For each of
+ * the B = N/n_cls images every NMS survivor of its n_cls rows is ordered by prob = det_conf*cls_max_conf descending,
+ * then class ascending, then NMS rank ascending, at any survivor count (a stable radix sort over the batch), and the
+ * first max_det are written: score float64 [B][max_det] (prob), box float64 [B][max_det][4] (x1, y1, x2, y2 in pixels
+ * of the image size sizes int32 [B][2] = (width, height)), cls int32 [B][max_det], count int32 [B] (written slots)
+ * and total int32 [B] (survivors before the cap).  Arithmetic is valid.detection_lines' own in float64:
+ * x = xs/W, w = ws/W, x1 = (x - w/2.0)*width, ..., so the values equal its result lines before their '%f' print.
+ * Slots count..max_det-1 hold score 0, box 0, class -1; nothing past max_det is written.  Fixed shapes, no
+ * synchronisation, no allocation: the call can be captured in a CUDA graph.  workspace: device memory of at least
+ * fsdet_detect_select_workspace_bytes(N, cap) bytes, 256-byte aligned. */
+size_t fsdet_detect_select_workspace_bytes(int N, int cap);
+int fsdet_detect_select(const float* cand, const int32_t* keep, const int32_t* keep_count, int N, int cap, int H, int W,
+                        int n_cls, const int32_t* sizes, int max_det, void* workspace, size_t workspace_bytes,
+                        double* score, double* box, int32_t* cls, int32_t* count, int32_t* total, void* stream);
 /* Running mean of the support net's reweighting vectors per class, valid_ensemble.py:86-100:
  * for i in 0..n-1: c = ids[i]; enews[c] = enews[c]*cnt[c]/(cnt[c]+1) + dw[i]/(cnt[c]+1); cnt[c] += 1 (float32, the
  * reference's operation order).  enews float32 [n_cls][C] (zero before the first call), dw float32 [n][C];

@@ -32,6 +32,17 @@ extern "C" int emul_nms(const float* cand, const double* boxes64, const int32_t*
     return 0;
 }
 
+extern "C" size_t emul_detect_select_workspace_bytes(int N, int cap) {
+    return select_workspace_layout(nullptr, N, cap).bytes;
+}
+
+extern "C" int emul_detect_select(const float* cand, const int32_t* keep, const int32_t* keep_count, int N, int cap, int H,
+                                  int W, int n_cls, const int32_t* sizes, int max_det, void* workspace, double* score,
+                                  double* box, int32_t* cls, int32_t* count, int32_t* total) {
+    return detect_select_impl(cand, keep, keep_count, N, cap, H, W, n_cls, sizes, max_det, workspace, score, box, cls,
+                              count, total, nullptr);
+}
+
 extern "C" int emul_rw_running_mean(float* enews, const int32_t* cnt_in, int32_t* cnt_out, const float* dw,
                                     const int32_t* ids, int n, int n_cls, int C) {
     emul::launch(dim3(ceil_div(C, 128), n_cls), dim3(128), 0,
