@@ -54,6 +54,7 @@ class GraphedTrainStep(object):
         self.capture_error_mode = 'thread_local'
         self.strict = strict                           # False: fall back to eager launches if a capture fails
         self.capture_failed = None
+        self.stepped = False                           # has this object run a step yet (see __call__)
 
     # ------------------------------------------------------------------ eager (very first step)
     def _eager(self, x, metax, mask, target):
@@ -184,8 +185,12 @@ class GraphedTrainStep(object):
         """One training step. Returns the (static, device) loss tensor.  `target`: the float64 label tensor, on the
         host (the reference's convention) or on the device; with a numeric cfg.neg_ratio the host copy is needed for
         the row sampling - pass it as `target_host` when `target` is a device tensor."""
-        if not any('momentum_buffer' in self.opt.state[p] for g in self.opt.param_groups for p in g['params']):
-            return self._eager(x, metax, mask, target)      # the very first step runs eagerly
+        if not self.stepped:
+            # the first step of this object runs eagerly: it initialises lazily (weight plans, the momentum buffers of
+            # a fresh run).  After a resume the momentum is loaded already, so it is a seasoned step, bit-equal to a
+            # replay; the captures follow from the next call on
+            self.stepped = True
+            return self._eager(x, metax, mask, target)
         if self.capture_failed is not None:
             return self._eager(x, metax, mask, target)
         key = self._key(x, metax, target)

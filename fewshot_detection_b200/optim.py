@@ -75,6 +75,38 @@ class FusedSGD(torch.optim.Optimizer):
                 self._hyper[gi][2] = vals
 
     @torch.no_grad()
+    def load_state_dict(self, state_dict):
+        """torch.optim.Optimizer.load_state_dict (the `state_dict()` layout is torch's), except that momentum is COPIED
+        into the buffers that exist, bits unchanged: the device pointer tables and any captured step graph address those
+        tensors, so swapping them would leave a graph updating freed memory.  A missing buffer is created (like the
+        first step does) and then filled, so loading works before and after a capture.  Refused: a different group or
+        parameter layout, a buffer of another shape or dtype, and a state without momentum for a parameter that already
+        has some (a graph cannot be made to take the first-step path again)."""
+        groups = state_dict['param_groups']
+        if len(groups) != len(self.param_groups) or \
+                any(len(g['params']) != len(s['params']) for g, s in zip(self.param_groups, groups)):
+            raise ValueError('optimizer state of %s parameters per group, this optimizer has %s'
+                             % ([len(s['params']) for s in groups], [len(g['params']) for g in self.param_groups]))
+        pairs = []
+        for group, saved in zip(self.param_groups, groups):
+            for p, idx in zip(group['params'], saved['params']):
+                buf = state_dict['state'].get(idx, {}).get('momentum_buffer')
+                if buf is None:
+                    if 'momentum_buffer' in self.state[p]:
+                        raise ValueError('optimizer state without momentum for parameter %d, which already has a buffer' % idx)
+                    continue
+                if tuple(buf.shape) != tuple(p.shape) or buf.dtype != p.dtype:
+                    raise ValueError('momentum of parameter %d is %s %s, the parameter is %s %s'
+                                     % (idx, buf.dtype, tuple(buf.shape), p.dtype, tuple(p.shape)))
+                pairs.append((p, buf))
+        for p, buf in pairs:
+            if 'momentum_buffer' not in self.state[p]:
+                self.state[p]['momentum_buffer'] = torch.empty_like(p)
+            self.state[p]['momentum_buffer'].copy_(buf)
+        for group, saved in zip(self.param_groups, groups):
+            group.update({k: v for k, v in saved.items() if k != 'params'})
+
+    @torch.no_grad()
     def step(self, closure=None):
         loss = None
         if closure is not None:

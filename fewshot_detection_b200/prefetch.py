@@ -125,21 +125,32 @@ class AsyncLossReader(object):
 class BackgroundPrep(object):
     """Runs the HOST half of the input pipeline one batch ahead in a worker thread (what the reference's DataLoader
     worker processes do, train_meta.py:173-193): `thunks` is an iterable of zero-argument callables, each returning one
-    prepared batch; iteration yields their results in order.  Exceptions of the worker surface at the consumer.  The
-    random draws happen inside the thunks, i.e. in one thread and in order - a seeded run stays reproducible."""
+    prepared batch; iteration yields their results in order.  Exceptions of the worker surface at the consumer.
+
+    The thunks draw from the global random generators, and so does the consumer (neg_filter's one `random()` per empty
+    label row, made when step i is launched).  To keep a seeded run reproducible the draws must come in the serial
+    order - prepare 0, step 0, prepare 1, step 1, ... - whatever the thread timing, so the worker starts thunk i+1 only
+    after the consumer has called `draws_done()` for item i.  The worker therefore prepares batch i+1 while the GPU
+    runs step i, and never runs further ahead."""
 
     def __init__(self, thunks, depth=2):
         import queue
         import threading
         self._q = queue.Queue(maxsize=depth)
         self._done = object()
+        self._go = threading.Semaphore(0)     # one release per item whose consumer-side draws are finished
+        self._closed = False
 
         self.busy_s = 0.0      # time the worker spent preparing (diagnostics)
 
         def work():
             import time as _t
             try:
-                for t in thunks:
+                for i, t in enumerate(thunks):
+                    if i:
+                        self._go.acquire()
+                        if self._closed:
+                            return
                     t0 = _t.time()
                     item = t()
                     self.busy_s += _t.time() - t0
@@ -149,6 +160,16 @@ class BackgroundPrep(object):
                 self._q.put((False, e))
         self._thread = threading.Thread(target=work, daemon=True)
         self._thread.start()
+
+    def draws_done(self):
+        """The consumer has made every random draw that belongs to the item it last received: the worker may start
+        preparing the next one."""
+        self._go.release()
+
+    def close(self):
+        """Stop the worker after its current thunk (a consumer that leaves the loop early)."""
+        self._closed = True
+        self._go.release()
 
     def __iter__(self):
         return self

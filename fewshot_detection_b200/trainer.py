@@ -59,10 +59,31 @@ def epoch_plan(model_seen, nsamples, batch_size, max_batches, tuning=False, max_
     return processed, init_epoch, max_epochs
 
 
+def rng_state():
+    """The states of the generators the input pipeline and neg_filter draw from - Python `random`, numpy, torch CPU -
+    with numpy's key array as an int64 tensor, so resume.write_state can store it."""
+    import random
+    import numpy as np
+    import torch
+    name, keys, pos, has_gauss, cached = np.random.get_state()
+    return dict(python=random.getstate(), numpy=(name, torch.from_numpy(keys.astype(np.int64)), int(pos), int(has_gauss),
+                                                 float(cached)), torch=torch.get_rng_state())
+
+
+def set_rng_state(state):
+    import random
+    import numpy as np
+    import torch
+    random.setstate(state['python'])
+    name, keys, pos, has_gauss, cached = state['numpy']
+    np.random.set_state((name, keys.numpy().astype(np.uint32), pos, has_gauss, cached))
+    torch.set_rng_state(state['torch'])
+
+
 class MetaTrainer(object):
     def __init__(self, model, optimizer, learning_rate, batch_size, steps, scales, make_train_batcher, make_meta_batcher,
                  backupdir=None, save_interval=10, reducer=None, world=1, processed_batches=0, log=print, use_graph=None,
-                 evaluate=None):
+                 evaluate=None, save_state=None):
         """learning_rate: the cfg rate already divided by `lr_factor` (what the driver calls `learning_rate` after
         :136); batch_size: GLOBAL batch; make_train_batcher(seen) / make_meta_batcher(): the epoch's data streams.
         use_graph: replay the step from CUDA graphs (graph.GraphedTrainStep: one graph per input shape, neg_filter
@@ -70,7 +91,9 @@ class MetaTrainer(object):
         evaluate: optional evaluate(model, epoch), run on every rank at the end of each checkpoint epoch (every
         `save_interval` epochs), after the weight file is written where one is written (rank 0 with a backupdir) and
         whether or not one is: every rank takes part in a sharded evaluation.  What it returns is logged
-        (see evaluate_checkpoint)."""
+        (see evaluate_checkpoint).
+        save_state: optional save_state(trainer, epoch), run on every rank at the end of each checkpoint epoch, after
+        the weight file and before `evaluate` (the driver writes the training-state file there, see resume.py)."""
         self.model, self.optimizer = model, optimizer
         self.region_loss = model.loss
         self.learning_rate, self.batch_size = learning_rate, batch_size
@@ -81,7 +104,9 @@ class MetaTrainer(object):
         self.processed_batches = processed_batches
         self.region_loss.seen = model.seen           # train_meta.py:93
         self.log = log
-        self.evaluate = evaluate
+        self.evaluate, self.save_state = evaluate, save_state
+        self.epoch = 0                 # the next epoch to run (after train_epoch(e): e + 1)
+        self.resume_epoch = None       # set by load_state_dict
         self.losses = collections.deque(maxlen=100)   # detached loss tensors of the most recent steps (no host sync)
         import os
         if use_graph is None:
@@ -140,24 +165,32 @@ class MetaTrainer(object):
             stream = ((batcher.finish(q), meta.finish(s)) for q, s in prep)
             self._prep = prep
         else:
+            prep = None
             stream = (((data, target), meta.batch(range(i * n_meta, (i + 1) * n_meta))) for i, (data, target) in enumerate(batcher))
         prof = os.environ.get('FSDET_TRAIN_PROFILE', '0') == '1'
         t_wait = t_step = 0.0
         tp = time.time()
-        for nb, ((data, target), support) in enumerate(stream, 1):
-            metax, mask = support[:2]
-            if prof:
-                t_wait += time.time() - tp
-                tp = time.time()
-            self.adjust_learning_rate(self.processed_batches)
-            self.processed_batches = self.processed_batches + 1
-            loss = self.train_step(data, metax, mask, target)
-            # a graph replay returns its static loss buffer, overwritten by the next replay of that graph (and, being in
-            # the graphs' shared pool, possibly by another graph's scratch): keep a device copy of this step's value
-            self.losses.append(loss.detach().clone() if self.graphed is not None else loss.detach())
-            if prof:
-                t_step += time.time() - tp
-                tp = time.time()
+        try:
+            for nb, ((data, target), support) in enumerate(stream, 1):
+                metax, mask = support[:2]
+                if prof:
+                    t_wait += time.time() - tp
+                    tp = time.time()
+                self.adjust_learning_rate(self.processed_batches)
+                self.processed_batches = self.processed_batches + 1
+                loss = self.train_step(data, metax, mask, target)
+                if prep is not None:
+                    prep.draws_done()         # this step's neg_filter draws are made: batch i+1's may start
+                # a graph replay returns its static loss buffer, overwritten by the next replay of that graph (and, being
+                # in the graphs' shared pool, possibly by another graph's scratch): keep a device copy of this step's value
+                self.losses.append(loss.detach().clone() if self.graphed is not None else loss.detach())
+                if prof:
+                    t_step += time.time() - tp
+                    tp = time.time()
+        except BaseException:
+            if prep is not None:
+                prep.close()
+            raise
         if prof and nb:
             self.log('host time per step: %.1f ms waiting for / finishing the input batch, %.1f ms launching the step, '
                      'background preparation %.1f ms per batch'
@@ -169,7 +202,10 @@ class MetaTrainer(object):
             self.log('save weights to %s' % path)
             self.model.seen = (epoch + 1) * len(batcher) * self.world
             self.model.save_weights(path)
+        self.epoch = epoch + 1
         if (epoch + 1) % self.save_interval == 0:
+            if self.save_state is not None:
+                self.save_state(self, epoch + 1)
             self.evaluate_checkpoint(epoch + 1)
         return nb
 
@@ -198,6 +234,32 @@ class MetaTrainer(object):
             self.log('evaluation at epoch %d: %s' % (epoch, r))
         return r
 
+    def state_dict(self):
+        """What a resumed run needs besides the weight file: the next epoch, `processed_batches` (the schedule
+        position), both `seen` counters (region_loss.seen counts every sample trained on; model.seen is only updated at
+        saves and seeds the next epoch's multi-scale schedule), the optimizer's state with its momentum buffers copied
+        to the host, bits unchanged, and this process's random generators (Python, numpy, torch CPU)."""
+        import torch
+        opt = self.optimizer.state_dict()
+        opt['state'] = {k: {n: (v.detach().to('cpu', copy=True) if torch.is_tensor(v) else v) for n, v in s.items()}
+                        for k, s in opt['state'].items()}
+        return dict(epoch=int(self.epoch), processed_batches=int(self.processed_batches),
+                    region_loss_seen=int(self.region_loss.seen), model_seen=int(self.model.seen), optimizer=opt,
+                    rng=rng_state())
+
+    def load_state_dict(self, state):
+        """Continue where `state` (from state_dict) was taken: fit() then starts at its epoch, whatever init_epoch it
+        is given.  Momentum is copied into the optimizer's buffers (FusedSGD keeps the tensors its pointer tables and
+        step graphs address)."""
+        self.optimizer.load_state_dict(state['optimizer'])
+        self.epoch = self.resume_epoch = int(state['epoch'])
+        self.processed_batches = int(state['processed_batches'])
+        self.region_loss.seen = int(state['region_loss_seen'])
+        self.model.seen = int(state['model_seen'])
+        set_rng_state(state['rng'])
+
     def fit(self, init_epoch, max_epochs):
+        if self.resume_epoch is not None:
+            init_epoch = self.resume_epoch
         for epoch in range(int(init_epoch), int(max_epochs)):
             self.train_epoch(epoch, max_epochs)

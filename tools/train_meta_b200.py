@@ -17,7 +17,15 @@ every checkpoint is scored the same way while training runs, sharded over the ra
     --eval-base-rw PATH                    with either: the base classes detected with the rows of a stored vectors
                                            file (the evaluation command's --base-rw)
 
-with the support set, batch sizes and thresholds of the evaluation command.
+with the support set, batch sizes and thresholds of the evaluation command.  Opt-in as well, resuming exactly
+(fewshot_detection_b200/resume.py):
+
+    --save-state                           every checkpoint also writes backup/%06d.state beside %06d.weights: momentum,
+                                           schedule position, both `seen` counters, every rank's random streams (only the
+                                           newest state file the run wrote is kept)
+    --resume PATH.state                    continue from that state; `weightfile` must be its paired weight file.  Every
+                                           check (file, version, weight checksum, world, batch, cfg, .data, training list)
+                                           is made before any CUDA work
 """
 import os
 import sys
@@ -103,6 +111,8 @@ def main():
     ap.add_argument('--eval-year', default='2007')
     ap.add_argument('--eval-coco-annotations', default=None)
     ap.add_argument('--eval-base-rw', default=None)
+    ap.add_argument('--save-state', action='store_true')
+    ap.add_argument('--resume', default=None)
     opts = ap.parse_args()
     scored = opts.eval_devkit is not None or opts.eval_coco_annotations is not None
     if len(opts.args) != 4 or (opts.eval_devkit is not None and opts.eval_coco_annotations is not None) or \
@@ -111,7 +121,8 @@ def main():
             print('--eval-base-rw needs --eval-devkit or --eval-coco-annotations')
         print('Usage:')
         print('python tools/train_meta_b200.py datacfg darknetcfg learnetcfg weightfile '
-              '[--eval-devkit DIR [--eval-year Y] | --eval-coco-annotations JSON] [--eval-base-rw PATH]')
+              '[--eval-devkit DIR [--eval-year Y] | --eval-coco-annotations JSON] [--eval-base-rw PATH] '
+              '[--save-state] [--resume PATH.state]')
         return 1
     if opts.eval_base_rw is not None and not os.path.isfile(opts.eval_base_rw):
         print('--eval-base-rw: no such file: %s' % opts.eval_base_rw)
@@ -123,15 +134,20 @@ def main():
     from fewshot_detection_b200.optim import FusedSGD
     from fewshot_detection_b200.distributed import GradAllReducer
     from fewshot_detection_b200.dataset import DetectionBatcher, MetaBatcher
-    from fewshot_detection_b200 import trainer as T, lists as LS
+    from fewshot_detection_b200 import trainer as T, lists as LS, resume as R
     import torch.distributed as dist
 
     world = int(os.environ.get('WORLD_SIZE', '1'))
     rank = int(os.environ.get('RANK', '0'))
     local = int(os.environ.get('LOCAL_RANK', '0'))
-    torch.cuda.set_device(local)
-    if world > 1:
-        dist.init_process_group('nccl', device_id=torch.device('cuda', local))
+    resume_state = None
+    if opts.resume is not None:           # every check on the state file is made before any CUDA work
+        try:
+            resume_state = R.read_state(opts.resume)
+            R.check_weights(resume_state, opts.resume, argv[4])
+        except R.StateFileError as e:
+            print('--resume: %s' % e)
+            return 1
 
     data_options = read_data_cfg(argv[1])
     darknetcfg, learnetcfg = parse_cfg(argv[2]), parse_cfg(argv[3])
@@ -147,6 +163,35 @@ def main():
     if opts.eval_base_rw is not None:             # checked against the model before training starts
         from fewshot_detection_b200 import valid as VA
         base_rw = VA.load_reweighting_vectors(opts.eval_base_rw, VA.reweighting_vector_shapes(learnetcfg, len(cfg.classes)))
+    fingerprint = lambda trainlist=None: R.fingerprint(darknetcfg, learnetcfg, data_options, world, batch_size, per_rank,
+                                                       trainlist)
+    if resume_state is not None:
+        try:
+            R.check_fingerprint(resume_state, opts.resume, fingerprint())
+        except R.StateFileError as e:
+            print('--resume: %s' % e)
+            return 1
+
+    if resume_state is not None:
+        seed = int(resume_state['seed'])     # the stored seed rebuilds the training list; the streams are restored below
+    else:
+        seed = int(os.environ.get('FSDET_SEED', str(int.from_bytes(os.urandom(4), 'little')) if world == 1 else '0'))
+    import random
+    random.seed(seed)                 # every rank must build the same lists and draw the same sizes
+    np.random.seed(seed % (2 ** 32))
+    torch.manual_seed(seed)           # train_meta.py:79; unseeded, torch's CPU generator starts from a per-process seed
+    trainlist = LS.build_dataset(data_options)
+    nsamples = len(trainlist)
+    if resume_state is not None:
+        try:
+            R.check_fingerprint(resume_state, opts.resume, fingerprint(trainlist))
+        except R.StateFileError as e:
+            print('--resume: %s' % e)
+            return 1
+
+    torch.cuda.set_device(local)
+    if world > 1:
+        dist.init_process_group('nccl', device_id=torch.device('cuda', local))
 
     model = Darknet(darknetcfg, learnetcfg)
     if os.path.exists(argv[4]):
@@ -163,12 +208,6 @@ def main():
     optimizer = FusedSGD(model.parameters(), **hp)
     reducer = GradAllReducer(model) if world > 1 else None
 
-    seed = int(os.environ.get('FSDET_SEED', str(int.from_bytes(os.urandom(4), 'little')) if world == 1 else '0'))
-    import random
-    random.seed(seed)                 # every rank must build the same lists and draw the same sizes
-    np.random.seed(seed % (2 ** 32))
-    trainlist = LS.build_dataset(data_options)
-    nsamples = len(trainlist)
     processed, init_epoch, max_epochs = T.epoch_plan(model.seen, nsamples, batch_size, int(net_options['max_batches']),
                                                      cfg.tuning, cfg.get('max_epoch'), cfg.repeat)
     backupdir = cfg.get('backup') or data_options.get('backup', 'backup')     # cfg.py:133-145 names it after the run's switches
@@ -198,8 +237,13 @@ def main():
     tr = T.MetaTrainer(model, optimizer, float(net_options['learning_rate']) / factor, batch_size, steps, scales,
                        make_train_batcher, make_meta_batcher, backupdir=backupdir if rank == 0 else None,
                        save_interval=cfg.save_interval, reducer=reducer, world=world, processed_batches=processed,
-                       log=logging if rank == 0 else (lambda *_: None), evaluate=evaluate)
+                       log=logging if rank == 0 else (lambda *_: None), evaluate=evaluate,
+                       save_state=R.state_saver(fingerprint(trainlist), seed, world, rank, logging) if opts.save_state else None)
     model.loss.verbose = rank == 0
+    if resume_state is not None:
+        R.restore(tr, resume_state, rank)    # last: it sets this rank's random generators
+        if rank == 0:
+            logging('resumed from %s at epoch %d, processed %d batches' % (opts.resume, tr.epoch, tr.processed_batches))
     tr.fit(init_epoch, max_epochs)
     if world > 1:
         if tr.graphed is not None:
