@@ -283,7 +283,7 @@ class NetRunner(object):
         self.profile = None     # optional dict name -> [flops, [(start_event, end_event), ...]]
         self.side = None        # second stream for the weight gradients (created by the first backward pass)
         self._side_used = False
-        self._keep = []         # tensors allocated on the main stream that the side stream still reads (until the join)
+        self._keep = []         # tensors allocated on the main stream that the side stream still reads or writes (until the join)
 
     # -- helpers ---------------------------------------------------------
     @staticmethod
@@ -956,11 +956,13 @@ class NetRunner(object):
             if f:
                 f()
         if self._side_ok():
-            # fork behind the apply pass; dz (and the activation planes) were allocated on the main stream: keep them alive
-            # until the join at the end of the backward pass, the allocator only orders their reuse on the main stream
+            # fork behind the apply pass; dz (and the activation planes) and the weight gradient's target (a temporary when
+            # accumulating into an existing .grad, written by the GEMM and added to .grad on the side stream) were allocated
+            # on the main stream: keep them alive until the join at the end of the backward pass, the allocator only orders
+            # their reuse on the main stream
             self.side.wait_stream(self._main)
             self._side_used = True
-            self._keep.append((dz, planes, x))
+            self._keep.append((dz, planes, x, gw))
             with torch.cuda.stream(self.side):
                 weight_grad(self.side.cuda_stream)
         else:
