@@ -54,6 +54,14 @@ SIGNATURES = {
     'fsdet_bn_bwd_rows': ('iii', 'i'),
     'fsdet_bn_bwd_finalize': ('pidpppppppiip', 'i'),
     'fsdet_bn_act_bwd_apply': ('pipipipppppfpippipiiiiip', 'i'),
+    'fsdet_bn_seg_colstats_rows': ('zi', 'i'),
+    'fsdet_bn_seg_colstats': ('piziipp', 'i'),
+    'fsdet_bn_seg_finalize': ('piizppppffppppfppip', 'i'),
+    'fsdet_bn_act_fwd_seg': ('pippfpipippppipiiiiizp', 'i'),
+    'fsdet_bn_seg_bwd_rows': ('iiii', 'i'),
+    'fsdet_bn_act_bwd_reduce_seg': ('pipipippppfpiiiiizp', 'i'),
+    'fsdet_bn_bwd_finalize_seg': ('piizpppppppip', 'i'),
+    'fsdet_bn_act_bwd_apply_seg': ('pipipipppppfpippipiiiiizp', 'i'),
     'fsdet_maxpool_fwd': ('pipiiiiiip', 'i'),
     'fsdet_maxpool_bwd': ('pipipiiiiiip', 'i'),
     'fsdet_reorg_fwd': ('pipiiiiip', 'i'),

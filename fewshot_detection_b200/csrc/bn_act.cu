@@ -4,12 +4,18 @@
 // Replaces nn.BatchNorm2d / nn.LeakyReLU / nn.MaxPool2d of the reference's conv
 // blocks (darknet_meta.py:240-268) and their autograd backward.
 //
-//   forward : conv kernel writes pre-BN z once (+ per-CTA sum / sum-of-squares)
+//   forward : conv kernel writes pre-BN z once (+ per-CTA sum / sum-of-squares; or colstats reads z once more)
 //             bn_finalize  -> mean, invstd, scale = gamma*invstd, shift = beta - mean*scale
 //             bn_act_fwd   -> y = leaky(z*scale+shift) [and/or its 2x2/2 max-pool]
 //   backward: bn_act_bwd_reduce -> sum(du), sum(du*xhat) partials (du = dy through pool+leaky)
 //             bn_bwd_finalize   -> dgamma, dbeta, c1 = dbeta/N, c2 = dgamma/N
 //             bn_act_bwd_apply  -> dz = scale*(du - c1 - xhat*c2)
+//
+// Segments: every pass also runs on a batch split into `nseg` contiguous segments of whole images, each normalised
+// with its own batch statistics (the per-replica BatchNorm of nn.DataParallel).  One launch covers all segments: the
+// segment is a grid dimension, per-segment vectors are [nseg][C] and partial rows never straddle a segment.  The
+// element-wise kernels take a SEG template flag: their one-segment instantiation is the plain pass, instruction for
+// instruction.
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -45,6 +51,58 @@ __device__ __forceinline__ void store_planes4(__half* hi, __half* lo, long long 
 }
 
 
+// ------------------------------------------------------------------ column statistics of z (BN partials)
+// grid (strips per segment, nseg): one CTA per strip of `strip` pixels of segment blockIdx.y (a strip ends at its
+// segment's end); partial[blockIdx.y * gridDim.x + blockIdx.x] = [sum(C) | sum of squares(C) | min(C) | max(C)]
+__global__ void __launch_bounds__(256) colstats_kernel(const float* __restrict__ z, int ld, long long seg_pix, int C, int strip,
+                                                       float* __restrict__ part) {
+    // threads: x = channel vector lane (float4), y = pixel lane
+    const int C4 = C >> 2;
+    const int TC = blockDim.x, TY = blockDim.y;
+    const long long send = (long long)(blockIdx.y + 1) * seg_pix;
+    long long p0 = (long long)blockIdx.y * seg_pix + (long long)blockIdx.x * strip, p1 = p0 + strip < send ? p0 + strip : send;
+    const long long row = (long long)blockIdx.y * gridDim.x + blockIdx.x;
+    FSDET_DYN_SMEM_F64(red_d);
+    float* red = reinterpret_cast<float*>(red_d);  // [TY][TC*16]
+    for (int cv0 = 0; cv0 < C4; cv0 += TC) {
+        int cv = cv0 + threadIdx.x;
+        float s[4] = {0, 0, 0, 0}, q[4] = {0, 0, 0, 0};
+        float mn[4] = {INFINITY, INFINITY, INFINITY, INFINITY}, mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+        if (cv < C4)
+            for (long long p = p0 + threadIdx.y; p < p1; p += 4 * TY) {   // four loads in flight, accumulated in row order
+                float4 v[4];
+#pragma unroll
+                for (int u = 0; u < 4; ++u)
+                    if (p + u * TY < p1) v[u] = ldg4(z + (p + u * TY) * ld + cv * 4);
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    if (p + u * TY >= p1) break;
+                    const float f[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        s[k] += f[k]; q[k] += f[k] * f[k]; mn[k] = fminf(mn[k], f[k]); mx[k] = fmaxf(mx[k], f[k]);
+                    }
+                }
+            }
+        float* mine = red + ((size_t)threadIdx.y * TC + threadIdx.x) * 16;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) { mine[k] = s[k]; mine[4 + k] = q[k]; mine[8 + k] = mn[k]; mine[12 + k] = mx[k]; }
+        __syncthreads();
+        // column j = (channel lane, statistic, component) reduced over the TY pixel lanes in a fixed order, all threads busy
+        for (int j = threadIdx.y * TC + threadIdx.x; j < TC * 16; j += TC * TY) {
+            const int lane = j >> 4, stat = (j >> 2) & 3, comp = j & 3;
+            if (cv0 + lane >= C4) continue;
+            float t = red[j];
+            for (int r = 1; r < TY; ++r) {
+                const float o = red[(size_t)r * TC * 16 + j];
+                t = stat < 2 ? t + o : (stat == 2 ? fminf(t, o) : fmaxf(t, o));
+            }
+            part[row * 4 * C + stat * C + (cv0 + lane) * 4 + comp] = t;
+        }
+        __syncthreads();
+    }
+}
+
 // ------------------------------------------------------------ finalize (fwd)
 // generic double-precision column sums of float partial rows (used by the backward finalize of the bias path)
 __global__ void __launch_bounds__(1024) colsum_double_kernel(const float* __restrict__ part, int nparts, int ncols,
@@ -66,11 +124,16 @@ __global__ void __launch_bounds__(1024) colsum_double_kernel(const float* __rest
 // reduction over the double-precision partial rows of the backward pass: columns [0, nsum) are summed (fixed
 // order), columns [nsum, ncols) hold maxima
 // `zero`: optional device float cleared here (the atomicMax target of the kernel that follows on the same stream - one graph
-// node less than a memset per layer)
+// node less than a memset per layer).  blockIdx.y: segment (its nparts rows -> its row of out)
+template <bool SEG>
 __global__ void __launch_bounds__(1024) colsum_dd_kernel(const double* __restrict__ part, int nparts, int ncols, int nsum,
                                                          double* __restrict__ out, float* __restrict__ zero) {
     __shared__ double red[32][33];
-    if (zero && blockIdx.x == 0 && threadIdx.x == 0 && threadIdx.y == 0) *zero = 0.f;
+    if (zero && blockIdx.x == 0 && (!SEG || blockIdx.y == 0) && threadIdx.x == 0 && threadIdx.y == 0) *zero = 0.f;
+    if (SEG) {
+        part += (long long)blockIdx.y * nparts * ncols;
+        out += (long long)blockIdx.y * ncols;
+    }
     int col = blockIdx.x * 32 + threadIdx.x;
     const bool is_max = col >= nsum;
     double s = 0.0;
@@ -88,13 +151,19 @@ __global__ void __launch_bounds__(1024) colsum_dd_kernel(const double* __restric
     }
 }
 
-// Stage 1: grid (ceil(C/32), S): block (x, y) reduces rows [y*rps, (y+1)*rps) of the conv partial rows
-// [nparts][4C] = (sum | sum of squares | min | max) into red[y][4C] (doubles; sums accumulated in double).
+// Stage 1: grid (ceil(C/32), S, nseg): block (x, y, z) reduces rows [y*rps, (y+1)*rps) of segment z's conv partial
+// rows [nparts][4C] = (sum | sum of squares | min | max) into red[z][y][4C] (doubles; sums accumulated in double).
+template <bool SEG>
 __global__ void __launch_bounds__(1024) bn_stats_reduce_kernel(const float* __restrict__ part, int nparts, int rps, int C,
                                                                double* __restrict__ red, float* __restrict__ zero) {
     __shared__ double rs[32][33], rq[32][33];
     __shared__ float rn[32][33], rx[32][33];
-    if (zero && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0 && threadIdx.y == 0) *zero = 0.f;   // see colsum_dd_kernel
+    if (zero && blockIdx.x == 0 && blockIdx.y == 0 && (!SEG || blockIdx.z == 0) && threadIdx.x == 0 && threadIdx.y == 0)
+        *zero = 0.f;   // see colsum_dd_kernel
+    if (SEG) {
+        part += (long long)blockIdx.z * nparts * 4 * C;
+        red += (long long)blockIdx.z * gridDim.y * 4 * C;
+    }
     const int c = blockIdx.x * 32 + threadIdx.x;
     const int r0 = blockIdx.y * rps;
     const int r1 = min(r0 + rps, nparts);
@@ -125,7 +194,9 @@ __global__ void __launch_bounds__(1024) bn_stats_reduce_kernel(const float* __re
 
 // Stage 2: fold the S reduced rows, derive mean / invstd / scale / shift, update the running statistics and - from
 // the per-channel range of z and the monotonicity of y = leaky(scale*z + shift) in z - the exact absolute maximum
-// of the activation.  One thread per channel.
+// of the activation.  One thread per channel; blockIdx.y: segment (vectors [nseg][C], `count` pixels each).  The
+// running statistics follow segment 0 only (nn.DataParallel keeps replica 0's buffers); amax_y spans all segments.
+template <bool SEG>
 __global__ void __launch_bounds__(128) bn_finalize_kernel(const double* __restrict__ red, int S, double count,
                                                           const float* __restrict__ gamma, const float* __restrict__ beta,
                                                           float* __restrict__ running_mean, float* __restrict__ running_var,
@@ -134,6 +205,16 @@ __global__ void __launch_bounds__(128) bn_finalize_kernel(const double* __restri
                                                           float* __restrict__ shift, float slope, float* __restrict__ amax_y,
                                                           float* __restrict__ xhat_absmax, int C, int training) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (SEG) {
+        const int seg = blockIdx.y;
+        red += (long long)seg * S * 4 * C;
+        if (seg > 0) running_mean = running_var = nullptr;
+        if (mean) mean += seg * C;
+        if (invstd) invstd += seg * C;
+        scale += seg * C;
+        shift += seg * C;
+        if (xhat_absmax) xhat_absmax += seg * C;
+    }
     float ymax = 0.f;
     if (c < C) {
         float m, is;
@@ -195,6 +276,7 @@ struct FwdArgs {
     __half *ph, *pl;     // fp16 hi/lo planes of the pooled output (optional)
     int ldz, ldf, ldp, Cpad;
     int B, H, W, C;
+    int segB;            // images per segment (blockIdx.y = segment; scale / shift are [nseg][C])
     float slope;
 };
 
@@ -207,17 +289,20 @@ __device__ __forceinline__ float4 act4(float4 v, float4 sc, float4 sh, float slo
 }
 
 // no pooling: one thread = one pixel x 4 channels (channel index runs to Cpad: the zero padding of the planes)
+// SEG: segments (blockIdx.y); the one-segment instantiation is the plain pass
+template <bool SEG>
 __global__ void __launch_bounds__(256) bn_act_flat_kernel(const FwdArgs a) {
     const unsigned CP4 = a.Cpad >> 2;
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;   // host guarantees npix * CP4 < 2^31
-    const unsigned npix = (unsigned)a.B * a.H * a.W;
+    const unsigned npix = (unsigned)(SEG ? a.segB : a.B) * a.H * a.W;   // of this segment
     if (i >= npix * CP4) return;
     const unsigned pu = i / CP4;
-    const long long p = pu;
+    const long long p = SEG ? (long long)blockIdx.y * npix + pu : (long long)pu;
     const int c = (int)(i - pu * CP4) * 4;
+    const int vc = SEG ? blockIdx.y * a.C + c : c;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
     if (c < a.C) {
-        v = act4(ldg4(a.z + p * a.ldz + c), ldg4(a.scale + c), ldg4(a.shift + c), a.slope);
+        v = act4(ldg4(a.z + p * a.ldz + c), ldg4(a.scale + vc), ldg4(a.shift + vc), a.slope);
         if (a.yf) *reinterpret_cast<float4*>(a.yf + p * a.ldf + c) = v;
     }
     if (a.fh) store_planes4(a.fh, a.fl, p * a.Cpad + c, v, plane_scale(__ldg(a.amax)));
@@ -226,17 +311,20 @@ __global__ void __launch_bounds__(256) bn_act_flat_kernel(const FwdArgs a) {
 // block (TC channel-vector lanes, TY windows): one thread = one 2x2 window x 4 channels per pass over the channel
 // lanes; windows cover ceil(H/2) x ceil(W/2).  FULL = some full-resolution output is wanted; otherwise only the
 // pooled activation is produced, from max(leaky(y)) == leaky(max(y)) (leaky is monotone).
-template <bool FULL>
+template <bool FULL, bool SEG>
 __global__ void __launch_bounds__(256) bn_act_pool_kernel(const FwdArgs a) {
     const int H = a.H, W = a.W;
     const int H2 = (H + 1) >> 1, W2 = (W + 1) >> 1, Hp = H >> 1, Wp = W >> 1;
     const int CP4 = a.Cpad >> 2;
     const unsigned wi = blockIdx.x * blockDim.y + threadIdx.y;   // host guarantees B*H*W < 2^31
-    if (wi >= (unsigned)a.B * H2 * W2) return;
+    if (wi >= (unsigned)(SEG ? a.segB : a.B) * H2 * W2) return;
     const unsigned t = wi / W2;
     const int w2 = (int)(wi - t * W2);
-    const int b = (int)(t / H2);
-    const int h2 = (int)(t - (unsigned)b * H2);
+    const int bl = (int)(t / H2);
+    const int h2 = (int)(t - (unsigned)bl * H2);
+    const int b = SEG ? blockIdx.y * a.segB + bl : bl;
+    const float* scale = SEG ? a.scale + blockIdx.y * a.C : a.scale;
+    const float* shift = SEG ? a.shift + blockIdx.y * a.C : a.shift;
     const bool whole = h2 < Hp && w2 < Wp;
     if (!FULL && !whole) return;                                 // no pooled output for windows cut by an odd edge
     const float psc = (a.fh || a.ph) ? plane_scale(__ldg(a.amax)) : 1.f;
@@ -247,7 +335,7 @@ __global__ void __launch_bounds__(256) bn_act_pool_kernel(const FwdArgs a) {
         const int c = cv * 4;
         const bool cok = c < a.C;
         float4 sc = make_float4(0, 0, 0, 0), sh = sc;
-        if (cok) { sc = ldg4(a.scale + c); sh = ldg4(a.shift + c); }
+        if (cok) { sc = ldg4(scale + c); sh = ldg4(shift + c); }
         float4 mx;
         if (FULL) {
             mx = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
@@ -302,6 +390,7 @@ struct BwdArgs {
     double* partial;
     int ldz, ld_dyf, ld_dyp, lddz, cpad;
     int B, H, W, C;
+    int segB;            // images per segment (blockIdx.z = segment; vectors [nseg][C], coef [nseg][2C])
     float slope;
     int has_bn;
 };
@@ -337,7 +426,7 @@ __device__ __forceinline__ void bwd_block_reduce(const double* red, double* dst,
 // as a (hi, lo) float pair: a difference of close floats is exact, so nothing is lost to the cancellation.
 // REDUCE writes per CTA row [sum(du) | sum(du*xhat) | max|du|] (3C doubles).
 // APPLY writes dz as fp32 and/or directly as the scaled fp16 (hi, lo) planes the tensor-core GEMMs read.
-template <bool APPLY>
+template <bool APPLY, bool SEG>
 __global__ void __launch_bounds__(256, 3) bn_act_bwd_kernel(const BwdArgs a) {
     const int H2 = (a.H + 1) >> 1, W2 = (a.W + 1) >> 1, Hp = a.H >> 1, Wp = a.W >> 1;
     const int C4 = a.C >> 2;
@@ -345,26 +434,28 @@ __global__ void __launch_bounds__(256, 3) bn_act_bwd_kernel(const BwdArgs a) {
     const int cv = blockIdx.y * TC + threadIdx.x;
     const bool cok = cv < C4;
     const int c = cv * 4;
-    const long long nwin = (long long)a.B * H2 * W2;
+    const int vc = SEG ? blockIdx.z * a.C + c : c;   // per-segment vectors [nseg][C], coef [nseg][2C]
+    const int cc = SEG ? blockIdx.z * a.C : 0;
+    const long long nwin = (long long)(SEG ? a.segB : a.B) * H2 * W2;
 
     float scv[4] = {1, 1, 1, 1}, shv[4] = {0, 0, 0, 0}, muv[4] = {0, 0, 0, 0}, isv[4] = {1, 1, 1, 1};
     float c1h[4] = {0, 0, 0, 0}, c1l[4] = {0, 0, 0, 0}, c2f[4] = {0, 0, 0, 0};
     if (cok) {
-        const float4 sc = ldg4(a.scale + c), sh = ldg4(a.shift + c);
+        const float4 sc = ldg4(a.scale + vc), sh = ldg4(a.shift + vc);
         scv[0] = sc.x; scv[1] = sc.y; scv[2] = sc.z; scv[3] = sc.w;
         shv[0] = sh.x; shv[1] = sh.y; shv[2] = sh.z; shv[3] = sh.w;
         if (a.has_bn) {
-            const float4 mu = ldg4(a.mean + c), is = ldg4(a.invstd + c);
+            const float4 mu = ldg4(a.mean + vc), is = ldg4(a.invstd + vc);
             muv[0] = mu.x; muv[1] = mu.y; muv[2] = mu.z; muv[3] = mu.w;
             isv[0] = is.x; isv[1] = is.y; isv[2] = is.z; isv[3] = is.w;
         }
         if (APPLY && a.has_bn) {
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
-                const double c1 = a.coef[c + k];
+                const double c1 = a.coef[vc + cc + k];
                 c1h[k] = (float)c1;
                 c1l[k] = (float)(c1 - (double)c1h[k]);
-                c2f[k] = (float)a.coef[a.C + c + k];
+                c2f[k] = (float)a.coef[vc + cc + a.C + k];
             }
         }
     }
@@ -375,8 +466,9 @@ __global__ void __launch_bounds__(256, 3) bn_act_bwd_kernel(const BwdArgs a) {
     for (unsigned wi = blockIdx.x * blockDim.y + threadIdx.y; cok && wi < (unsigned)nwin; wi += gridDim.x * blockDim.y) {
         const unsigned t = wi / W2;
         const int w2 = (int)(wi - t * W2);
-        const int b = (int)(t / H2);
-        const int h2 = (int)(t - (unsigned)b * H2);
+        const int bl = (int)(t / H2);
+        const int h2 = (int)(t - (unsigned)bl * H2);
+        const int b = SEG ? blockIdx.z * a.segB + bl : bl;
         float zv[4][4], yv[4][4];
         long long pix[4];
         bool ok[4];
@@ -455,7 +547,7 @@ __global__ void __launch_bounds__(256, 3) bn_act_bwd_kernel(const BwdArgs a) {
             mine[8 + k] = (double)md[k];
         }
         __syncthreads();
-        bwd_block_reduce(red, a.partial + (long long)blockIdx.x * 3 * a.C, a.C, blockIdx.y * TC);
+        bwd_block_reduce(red, a.partial + ((SEG ? (long long)blockIdx.z * gridDim.x : 0ll) + blockIdx.x) * 3 * a.C, a.C, blockIdx.y * TC);
     }
 }
 
@@ -463,7 +555,7 @@ __global__ void __launch_bounds__(256, 3) bn_act_bwd_kernel(const BwdArgs a) {
 // consumer (only dy_pool exists): du is non-zero only at the arg-max pixel of each 2x2 window, so the reduce pass
 // touches one element per window and channel, and the apply pass needs the activation derivative only there.
 // Same arithmetic as the general kernel (the zero terms are dropped), a fraction of the instructions.
-template <bool APPLY>
+template <bool APPLY, bool SEG>
 __global__ void __launch_bounds__(256, 3) bn_act_bwd_pool_kernel(const BwdArgs a) {
     const int H2 = (a.H + 1) >> 1, W2 = (a.W + 1) >> 1, Hp = a.H >> 1, Wp = a.W >> 1;
     const int C4 = a.C >> 2;
@@ -471,12 +563,14 @@ __global__ void __launch_bounds__(256, 3) bn_act_bwd_pool_kernel(const BwdArgs a
     const int cv = blockIdx.y * TC + threadIdx.x;
     const bool cok = cv < C4;
     const int c = cv * 4;
-    const unsigned nwin = (unsigned)a.B * H2 * W2;
+    const int vc = SEG ? blockIdx.z * a.C + c : c;
+    const int cc = SEG ? blockIdx.z * a.C : 0;
+    const unsigned nwin = (unsigned)(SEG ? a.segB : a.B) * H2 * W2;
 
     float scv[4] = {1, 1, 1, 1}, shv[4] = {0, 0, 0, 0}, muv[4] = {0, 0, 0, 0}, isv[4] = {1, 1, 1, 1};
     float c1h[4] = {0, 0, 0, 0}, c1l[4] = {0, 0, 0, 0}, c2f[4] = {0, 0, 0, 0}, t0[4] = {0, 0, 0, 0};
     if (cok) {
-        const float4 sc = ldg4(a.scale + c), sh = ldg4(a.shift + c), mu = ldg4(a.mean + c), is = ldg4(a.invstd + c);
+        const float4 sc = ldg4(a.scale + vc), sh = ldg4(a.shift + vc), mu = ldg4(a.mean + vc), is = ldg4(a.invstd + vc);
         scv[0] = sc.x; scv[1] = sc.y; scv[2] = sc.z; scv[3] = sc.w;
         shv[0] = sh.x; shv[1] = sh.y; shv[2] = sh.z; shv[3] = sh.w;
         muv[0] = mu.x; muv[1] = mu.y; muv[2] = mu.z; muv[3] = mu.w;
@@ -484,10 +578,10 @@ __global__ void __launch_bounds__(256, 3) bn_act_bwd_pool_kernel(const BwdArgs a
         if (APPLY) {
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
-                const double c1 = a.coef[c + k];
+                const double c1 = a.coef[vc + cc + k];
                 c1h[k] = (float)c1;
                 c1l[k] = (float)(c1 - (double)c1h[k]);
-                c2f[k] = (float)a.coef[a.C + c + k];
+                c2f[k] = (float)a.coef[vc + cc + a.C + k];
                 t0[k] = (0.f - c1h[k]) - c1l[k];     // du == 0
             }
         }
@@ -500,8 +594,9 @@ __global__ void __launch_bounds__(256, 3) bn_act_bwd_pool_kernel(const BwdArgs a
     for (unsigned wi = blockIdx.x * blockDim.y + threadIdx.y; cok && wi < nwin; wi += gridDim.x * blockDim.y) {
         const unsigned t = wi / W2;
         const int w2 = (int)(wi - t * W2);
-        const int b = (int)(t / H2);
-        const int h2 = (int)(t - (unsigned)b * H2);
+        const int bl = (int)(t / H2);
+        const int h2 = (int)(t - (unsigned)bl * H2);
+        const int b = SEG ? blockIdx.z * a.segB + bl : bl;
         const bool whole = h2 < Hp && w2 < Wp;       // windows cut by an odd edge have no pooled output
         const unsigned p00 = ((unsigned)b * a.H + 2 * h2) * a.W + 2 * w2;
         float zv[4][4];
@@ -572,28 +667,38 @@ __global__ void __launch_bounds__(256, 3) bn_act_bwd_pool_kernel(const BwdArgs a
             mine[8 + k] = (double)md[k];
         }
         __syncthreads();
-        bwd_block_reduce(red, a.partial + (long long)blockIdx.x * 3 * a.C, a.C, blockIdx.y * TC);
+        bwd_block_reduce(red, a.partial + ((SEG ? (long long)blockIdx.z * gridDim.x : 0ll) + blockIdx.x) * 3 * a.C, a.C, blockIdx.y * TC);
     }
 }
 
-// sums row [3C] -> dgamma, dbeta, the projection coefficients, and an upper bound of max|dz| (the scale of dz's fp16
-// planes): |dz| <= |scale| * (max|du| + |c1| + max|xhat| * |c2|)
+// sums rows [nseg][3C] -> dgamma, dbeta (summed over the segments in order), the projection coefficients of each
+// segment ([nseg][2C]), and an upper bound of max|dz| over all segments (the scale of dz's fp16 planes):
+// |dz| <= |scale| * (max|du| + |c1| + max|xhat| * |c2|).  SEG == false: one segment
+template <bool SEG>
 __global__ void bn_bwd_finalize_kernel(const double* __restrict__ sums, double count, const float* __restrict__ gamma,
                                        const float* __restrict__ invstd, const float* __restrict__ xhat_absmax,
                                        float* __restrict__ dgamma, float* __restrict__ dbeta, double* __restrict__ coef,
-                                       float* __restrict__ amax_bound, int C, int has_bn) {
+                                       float* __restrict__ amax_bound, int C, int has_bn, int nseg) {
     int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= C) return;
-    double sdu = sums[c], sdux = sums[C + c];
-    double bound = sums[2 * C + c];
-    if (dbeta) dbeta[c] = (float)sdu;
-    if (has_bn) {
-        if (dgamma) dgamma[c] = (float)sdux;
-        const double c1 = sdu / count, c2 = sdux / count;
-        coef[c] = c1;
-        coef[C + c] = c2;
-        if (amax_bound) bound = fabs((double)gamma[c] * (double)invstd[c]) * (bound + fabs(c1) + (double)xhat_absmax[c] * fabs(c2));
+    double sdu_all = 0.0, sdux_all = 0.0, bound = 0.0;
+    for (int g = 0; g < (SEG ? nseg : 1); ++g) {
+        const double* sg = sums + (long long)g * 3 * C;
+        const double sdu = sg[c], sdux = sg[C + c];
+        double bg = sg[2 * C + c];
+        sdu_all = g ? sdu_all + sdu : sdu;
+        sdux_all = g ? sdux_all + sdux : sdux;
+        if (has_bn) {
+            const double c1 = sdu / count, c2 = sdux / count;
+            coef[2 * g * C + c] = c1;
+            coef[2 * g * C + C + c] = c2;
+            if (amax_bound)
+                bg = fabs((double)gamma[c] * (double)invstd[g * C + c]) * (bg + fabs(c1) + (double)xhat_absmax[g * C + c] * fabs(c2));
+        }
+        bound = g ? fmax(bound, bg) : bg;
     }
+    if (dbeta) dbeta[c] = (float)sdu_all;
+    if (has_bn && dgamma) dgamma[c] = (float)sdux_all;
     if (amax_bound) {
         const float bf = (float)(bound * 1.0001);
         if (isfinite(bf) && bf > 0.f) atomicMax(reinterpret_cast<int*>(amax_bound), __float_as_int(bf));
@@ -625,6 +730,29 @@ static void stat_split(int nparts, int* S, int* rps) {
     *S = ceil_div(nparts, *rps);
 }
 
+// backward CTA rows per segment: the one-segment rows shared out, so that nseg segments fill the same waves
+static int seg_bwd_rows(int segB, int H, int W, int nseg) {
+    const int r = bwd_rows(segB * nseg, H, W) / nseg;
+    return r < 1 ? 1 : r;
+}
+
+// pixels per partial row of colstats: large tensors use long strips (few partial rows, little reduction work
+// afterwards), small ones short strips so that every SM still gets CTAs
+static int stat_strip(long long npix) {
+    long long s = npix / (8 * kNumSMs) / 32 * 32;
+    return (int)(s < 32 ? 32 : (s > 1024 ? 1024 : s));
+}
+
+// strips per segment of nseg segments of seg_pix pixels (the strip length is that of the whole tensor)
+static int colstats_seg_rows(long long seg_pix, int nseg) { return ceil_div(seg_pix, stat_strip(seg_pix * nseg)); }
+
+// segments of whole images: nseg * seg_pix == B*H*W and seg_pix a multiple of H*W; returns images per segment or 0
+static int seg_images(int B, int H, int W, int nseg, long long seg_pix) {
+    const long long hw = (long long)H * W;
+    if (nseg < 1 || hw <= 0 || seg_pix <= 0 || seg_pix % hw || (long long)nseg * seg_pix != (long long)B * hw) return 0;
+    return (int)(seg_pix / hw);
+}
+
 }  // namespace fsdet
 
 #ifndef FSDET_HOST_EMULATION  // tools/host_emul/bn_act_emul.cpp launches the kernels above on the same geometry
@@ -632,13 +760,40 @@ static void stat_split(int nparts, int* S, int* rps) {
 using namespace fsdet;
 
 extern "C" int fsdet_bn_bwd_rows(int B, int H, int W) { return bwd_rows(B, H, W); }
+extern "C" int fsdet_bn_seg_bwd_rows(int B, int H, int W, int nseg) {
+    return nseg >= 1 && B % nseg == 0 ? seg_bwd_rows(B / nseg, H, W, nseg) : -1;
+}
 
-extern "C" int fsdet_bn_finalize(const float* stat_partial, int nparts, double count, const float* gamma,
-                                 const float* beta, float* running_mean, float* running_var, float momentum, float eps,
-                                 float* mean, float* invstd, float* scale, float* shift, float slope, float* amax_y,
-                                 float* xhat_absmax, int C, int training, void* stream) {
-    FSDET_CHECK_ARG(scale && shift && C > 0, "bn_finalize: bad args");
-    cudaStream_t s = (cudaStream_t)stream;
+extern "C" int fsdet_colstats_rows(size_t npix) { return colstats_seg_rows((long long)npix, 1); }
+extern "C" int fsdet_bn_seg_colstats_rows(size_t seg_pix, int nseg) {
+    return nseg >= 1 ? colstats_seg_rows((long long)seg_pix, nseg) : -1;
+}
+
+static int launch_colstats(const float* z, int ld, long long seg_pix, int nseg, int C, float* partial, cudaStream_t s) {
+    FSDET_CHECK_ARG(z && partial && C % 4 == 0 && ld % 4 == 0 && aligned16(z) && nseg >= 1 && seg_pix >= 0,
+                    "colstats: C=%d ld=%d nseg=%d", C, ld, nseg);
+    if (seg_pix == 0) return 0;
+    const int TCx = chan_lanes(C);
+    const int TY = 256 / TCx;
+    dim3 block(TCx, TY), grid(colstats_seg_rows(seg_pix, nseg), nseg);
+    size_t smem = (size_t)TY * TCx * 16 * sizeof(float);
+    colstats_kernel<<<grid, block, smem, s>>>(z, ld, seg_pix, C, stat_strip(seg_pix * nseg), partial);
+    return launch_status("colstats");
+}
+
+extern "C" int fsdet_colstats(const float* z, int ld, size_t npix, int C, float* partial, void* stream) {
+    return launch_colstats(z, ld, (long long)npix, 1, C, partial, (cudaStream_t)stream);
+}
+
+extern "C" int fsdet_bn_seg_colstats(const float* z, int ld, size_t seg_pix, int nseg, int C, float* partial, void* stream) {
+    return launch_colstats(z, ld, (long long)seg_pix, nseg, C, partial, (cudaStream_t)stream);
+}
+
+static int launch_finalize(const float* stat_partial, int nparts, int nseg, double count, const float* gamma,
+                           const float* beta, float* running_mean, float* running_var, float momentum, float eps,
+                           float* mean, float* invstd, float* scale, float* shift, float slope, float* amax_y,
+                           float* xhat_absmax, int C, int training, cudaStream_t s) {
+    FSDET_CHECK_ARG(scale && shift && C > 0 && nseg >= 1 && (training || nseg == 1), "bn_finalize: bad args");
     if (training) {
         FSDET_CHECK_ARG(stat_partial && nparts > 0, "bn_finalize: training needs the conv partials");
     } else {
@@ -651,79 +806,137 @@ extern "C" int fsdet_bn_finalize(const float* stat_partial, int nparts, double c
     const double* red = nullptr;
     int S = 0;
     if (training) {
-        // scratch for the stage-1 result lives behind the partial rows (fsdet_bn_stat_scratch_rows() extra rows)
+        // scratch for the stage-1 result lives behind the partial rows (nseg * fsdet_bn_stat_scratch_rows() extra rows)
         int rps;
         stat_split(nparts, &S, &rps);
-        double* scratch = reinterpret_cast<double*>(const_cast<float*>(stat_partial) + (size_t)nparts * 4 * C);
-        dim3 block(32, 32), grid(ceil_div(C, 32), S);
-        bn_stats_reduce_kernel<<<grid, block, 0, s>>>(stat_partial, nparts, rps, C, scratch, amax_y);
+        double* scratch = reinterpret_cast<double*>(const_cast<float*>(stat_partial) + (size_t)nseg * nparts * 4 * C);
+        dim3 block(32, 32), grid(ceil_div(C, 32), S, nseg);
+        if (nseg > 1) bn_stats_reduce_kernel<true><<<grid, block, 0, s>>>(stat_partial, nparts, rps, C, scratch, amax_y);
+        else bn_stats_reduce_kernel<false><<<grid, block, 0, s>>>(stat_partial, nparts, rps, C, scratch, amax_y);
         int st = launch_status("bn_finalize/reduce");
         if (st) return st;
         red = scratch;
     }
-    bn_finalize_kernel<<<ceil_div(C, 128), 128, 0, s>>>(red, S, count, gamma, beta, running_mean, running_var, momentum, eps, mean,
-                                                        invstd, scale, shift, slope, amax_y, xhat_absmax, C, training);
+    if (nseg > 1)
+        bn_finalize_kernel<true><<<dim3(ceil_div(C, 128), nseg), 128, 0, s>>>(red, S, count, gamma, beta, running_mean, running_var,
+                                                                               momentum, eps, mean, invstd, scale, shift, slope,
+                                                                               amax_y, xhat_absmax, C, training);
+    else
+        bn_finalize_kernel<false><<<ceil_div(C, 128), 128, 0, s>>>(red, S, count, gamma, beta, running_mean, running_var, momentum,
+                                                                   eps, mean, invstd, scale, shift, slope, amax_y, xhat_absmax,
+                                                                   C, training);
     return launch_status("bn_finalize");
+}
+
+extern "C" int fsdet_bn_finalize(const float* stat_partial, int nparts, double count, const float* gamma,
+                                 const float* beta, float* running_mean, float* running_var, float momentum, float eps,
+                                 float* mean, float* invstd, float* scale, float* shift, float slope, float* amax_y,
+                                 float* xhat_absmax, int C, int training, void* stream) {
+    return launch_finalize(stat_partial, nparts, 1, count, gamma, beta, running_mean, running_var, momentum, eps, mean,
+                           invstd, scale, shift, slope, amax_y, xhat_absmax, C, training, (cudaStream_t)stream);
+}
+
+extern "C" int fsdet_bn_seg_finalize(const float* stat_partial, int nparts, int nseg, size_t seg_pix, const float* gamma,
+                                     const float* beta, float* running_mean, float* running_var, float momentum, float eps,
+                                     float* mean, float* invstd, float* scale, float* shift, float slope, float* amax_y,
+                                     float* xhat_absmax, int C, void* stream) {
+    FSDET_CHECK_ARG(seg_pix > 0, "bn_seg_finalize: empty segments");
+    return launch_finalize(stat_partial, nparts, nseg, (double)seg_pix, gamma, beta, running_mean, running_var, momentum,
+                           eps, mean, invstd, scale, shift, slope, amax_y, xhat_absmax, C, 1, (cudaStream_t)stream);
 }
 
 extern "C" int fsdet_bn_stat_scratch_rows(void) { return 2 * kBnSplits; }  // kBnSplits rows of 4C doubles
 
-extern "C" int fsdet_bn_act_fwd(const float* z, int ldz, const float* scale, const float* shift, float slope, float* y_full,
-                                int ld_full, float* y_pool, int ld_pool, void* full_hi, void* full_lo, void* pool_hi,
-                                void* pool_lo, int Cpad, const float* amax, int B, int H, int W, int C, void* stream) {
+static int launch_act_fwd(const float* z, int ldz, const float* scale, const float* shift, float slope, float* y_full,
+                          int ld_full, float* y_pool, int ld_pool, void* full_hi, void* full_lo, void* pool_hi,
+                          void* pool_lo, int Cpad, const float* amax, int B, int H, int W, int C, int nseg, int segB,
+                          cudaStream_t s) {
     const bool planes = full_hi || pool_hi;
     FSDET_CHECK_ARG(z && scale && shift && (y_full || y_pool || planes), "bn_act_fwd: null pointer");
     FSDET_CHECK_ARG(C % 4 == 0 && ldz % 4 == 0 && (!y_full || ld_full % 4 == 0) && (!y_pool || ld_pool % 4 == 0),
                     "bn_act_fwd: C=%d and leading dims must be multiples of 4", C);
     FSDET_CHECK_ARG(!planes || (amax && Cpad >= C && Cpad % 4 == 0 && (!full_hi || full_lo) && (!pool_hi || pool_lo)),
                     "bn_act_fwd: plane outputs need amax, lo planes and Cpad >= C");
-    cudaStream_t s = (cudaStream_t)stream;
     FwdArgs a;
     a.z = z; a.scale = scale; a.shift = shift; a.amax = amax; a.yf = y_full; a.yp = y_pool;
     a.fh = (__half*)full_hi; a.fl = (__half*)full_lo; a.ph = (__half*)pool_hi; a.pl = (__half*)pool_lo;
     a.ldz = ldz; a.ldf = ld_full; a.ldp = ld_pool; a.Cpad = planes ? Cpad : C; a.B = B; a.H = H; a.W = W; a.C = C; a.slope = slope;
+    a.segB = segB;
     const int CP4 = a.Cpad / 4;
     FSDET_CHECK_ARG((long long)B * H * W * CP4 < (1ll << 31), "bn_act_fwd: tensor too large for 32-bit indexing");
     if (!y_pool && !pool_hi) {
-        long long n = (long long)B * H * W * CP4;
+        long long n = (long long)segB * H * W * CP4;
         if (n == 0) return 0;
-        bn_act_flat_kernel<<<ceil_div(n, 256), 256, 0, s>>>(a);
+        if (nseg > 1) bn_act_flat_kernel<true><<<dim3(ceil_div(n, 256), nseg), 256, 0, s>>>(a);
+        else bn_act_flat_kernel<false><<<ceil_div(n, 256), 256, 0, s>>>(a);
     } else {
-        long long nwin = (long long)B * ((H + 1) / 2) * ((W + 1) / 2);
+        long long nwin = (long long)segB * ((H + 1) / 2) * ((W + 1) / 2);
         if (nwin == 0) return 0;
         // channel-vector lanes sized by the REAL channels: the zero padding of the planes (pitch > C) is written by the
         // same threads in a second trip of their channel loop instead of by threads that never load anything
         const int TC = chan_lanes(C);
         const int TY = 256 / TC;
-        dim3 block(TC, TY), grid((unsigned)ceil_div(nwin, TY));
-        if (a.yf || a.fh) bn_act_pool_kernel<true><<<grid, block, 0, s>>>(a);
-        else bn_act_pool_kernel<false><<<grid, block, 0, s>>>(a);
+        dim3 block(TC, TY), grid((unsigned)ceil_div(nwin, TY), nseg);
+        const bool full = a.yf || a.fh;
+        if (nseg > 1) {
+            if (full) bn_act_pool_kernel<true, true><<<grid, block, 0, s>>>(a);
+            else bn_act_pool_kernel<false, true><<<grid, block, 0, s>>>(a);
+        } else {
+            if (full) bn_act_pool_kernel<true, false><<<grid, block, 0, s>>>(a);
+            else bn_act_pool_kernel<false, false><<<grid, block, 0, s>>>(a);
+        }
     }
     return launch_status("bn_act_fwd");
 }
 
-static int launch_bwd(bool apply, const BwdArgs& a, cudaStream_t s) {
+extern "C" int fsdet_bn_act_fwd(const float* z, int ldz, const float* scale, const float* shift, float slope, float* y_full,
+                                int ld_full, float* y_pool, int ld_pool, void* full_hi, void* full_lo, void* pool_hi,
+                                void* pool_lo, int Cpad, const float* amax, int B, int H, int W, int C, void* stream) {
+    return launch_act_fwd(z, ldz, scale, shift, slope, y_full, ld_full, y_pool, ld_pool, full_hi, full_lo, pool_hi, pool_lo,
+                          Cpad, amax, B, H, W, C, 1, B, (cudaStream_t)stream);
+}
+
+extern "C" int fsdet_bn_act_fwd_seg(const float* z, int ldz, const float* scale, const float* shift, float slope,
+                                    float* y_full, int ld_full, float* y_pool, int ld_pool, void* full_hi, void* full_lo,
+                                    void* pool_hi, void* pool_lo, int Cpad, const float* amax, int B, int H, int W, int C,
+                                    int nseg, size_t seg_pix, void* stream) {
+    const int segB = seg_images(B, H, W, nseg, (long long)seg_pix);
+    FSDET_CHECK_ARG(segB > 0, "bn_act_fwd_seg: %d segments of %zu pixels do not split %d images of %dx%d", nseg, seg_pix, B, H, W);
+    return launch_act_fwd(z, ldz, scale, shift, slope, y_full, ld_full, y_pool, ld_pool, full_hi, full_lo, pool_hi, pool_lo,
+                          Cpad, amax, B, H, W, C, nseg, segB, (cudaStream_t)stream);
+}
+
+static int launch_bwd(bool apply, const BwdArgs& a, int nseg, cudaStream_t s) {
     FSDET_CHECK_ARG((long long)a.B * a.H * a.W < (1ll << 31), "bn_act_bwd: tensor too large for 32-bit pixel indexing");
     int C4 = a.C / 4;
     int TC = chan_lanes(a.C);
     int TY = 256 / TC;
-    dim3 block(TC, TY), grid(bwd_rows(a.B, a.H, a.W), ceil_div(C4, TC));
+    dim3 block(TC, TY), grid(seg_bwd_rows(a.segB, a.H, a.W, nseg), ceil_div(C4, TC), nseg);
     const size_t smem = (size_t)TY * TC * 16 * sizeof(double);  // 32 KB (reduce pass)
     const bool pool_only = !a.dyf && a.dyp && a.has_bn && a.slope >= 0.f && a.slope <= 1.f;
-    if (pool_only) {
-        if (apply) bn_act_bwd_pool_kernel<true><<<grid, block, 0, s>>>(a);
-        else bn_act_bwd_pool_kernel<false><<<grid, block, smem, s>>>(a);
+    if (nseg > 1) {
+        if (pool_only) {
+            if (apply) bn_act_bwd_pool_kernel<true, true><<<grid, block, 0, s>>>(a);
+            else bn_act_bwd_pool_kernel<false, true><<<grid, block, smem, s>>>(a);
+        } else {
+            if (apply) bn_act_bwd_kernel<true, true><<<grid, block, 0, s>>>(a);
+            else bn_act_bwd_kernel<false, true><<<grid, block, smem, s>>>(a);
+        }
     } else {
-        if (apply) bn_act_bwd_kernel<true><<<grid, block, 0, s>>>(a);
-        else bn_act_bwd_kernel<false><<<grid, block, smem, s>>>(a);
+        if (pool_only) {
+            if (apply) bn_act_bwd_pool_kernel<true, false><<<grid, block, 0, s>>>(a);
+            else bn_act_bwd_pool_kernel<false, false><<<grid, block, smem, s>>>(a);
+        } else {
+            if (apply) bn_act_bwd_kernel<true, false><<<grid, block, 0, s>>>(a);
+            else bn_act_bwd_kernel<false, false><<<grid, block, smem, s>>>(a);
+        }
     }
     return launch_status(apply ? "bn_act_bwd_apply" : "bn_act_bwd_reduce");
 }
 
-extern "C" int fsdet_bn_act_bwd_reduce(const float* z, int ldz, const float* dy_full, int ld_dyf, const float* dy_pool,
-                                       int ld_dyp, const float* scale, const float* shift, const float* mean,
-                                       const float* invstd, float slope, double* partial, int B, int H, int W, int C,
-                                       int has_bn, void* stream) {
+static int bwd_reduce(const float* z, int ldz, const float* dy_full, int ld_dyf, const float* dy_pool, int ld_dyp,
+                      const float* scale, const float* shift, const float* mean, const float* invstd, float slope,
+                      double* partial, int B, int H, int W, int C, int has_bn, int nseg, int segB, cudaStream_t s) {
     FSDET_CHECK_ARG(z && scale && shift && partial && (dy_full || dy_pool), "bn_act_bwd_reduce: null pointer");
     FSDET_CHECK_ARG(!has_bn || (mean && invstd), "bn_act_bwd_reduce: BN needs mean/invstd");
     FSDET_CHECK_ARG(C % 4 == 0 && ldz % 4 == 0 && ld_dyf % 4 == 0 && ld_dyp % 4 == 0, "bn_act_bwd_reduce: alignment");
@@ -731,30 +944,67 @@ extern "C" int fsdet_bn_act_bwd_reduce(const float* z, int ldz, const float* dy_
     a.z = z; a.dyf = dy_full; a.dyp = dy_pool; a.scale = scale; a.shift = shift; a.mean = mean; a.invstd = invstd;
     a.coef = nullptr; a.dz = nullptr; a.dh = nullptr; a.dl = nullptr; a.amax = nullptr; a.partial = partial;
     a.ldz = ldz; a.ld_dyf = ld_dyf; a.ld_dyp = ld_dyp; a.lddz = 0; a.cpad = 0;
-    a.B = B; a.H = H; a.W = W; a.C = C; a.slope = slope; a.has_bn = has_bn;
-    return launch_bwd(false, a, (cudaStream_t)stream);
+    a.B = B; a.H = H; a.W = W; a.C = C; a.segB = segB; a.slope = slope; a.has_bn = has_bn;
+    return launch_bwd(false, a, nseg, s);
+}
+
+extern "C" int fsdet_bn_act_bwd_reduce(const float* z, int ldz, const float* dy_full, int ld_dyf, const float* dy_pool,
+                                       int ld_dyp, const float* scale, const float* shift, const float* mean,
+                                       const float* invstd, float slope, double* partial, int B, int H, int W, int C,
+                                       int has_bn, void* stream) {
+    return bwd_reduce(z, ldz, dy_full, ld_dyf, dy_pool, ld_dyp, scale, shift, mean, invstd, slope, partial, B, H, W, C, has_bn,
+                      1, B, (cudaStream_t)stream);
+}
+
+extern "C" int fsdet_bn_act_bwd_reduce_seg(const float* z, int ldz, const float* dy_full, int ld_dyf, const float* dy_pool,
+                                           int ld_dyp, const float* scale, const float* shift, const float* mean,
+                                           const float* invstd, float slope, double* partial, int B, int H, int W, int C,
+                                           int nseg, size_t seg_pix, void* stream) {
+    const int segB = seg_images(B, H, W, nseg, (long long)seg_pix);
+    FSDET_CHECK_ARG(segB > 0, "bn_act_bwd_reduce_seg: %d segments of %zu pixels do not split %d images of %dx%d", nseg, seg_pix, B, H, W);
+    return bwd_reduce(z, ldz, dy_full, ld_dyf, dy_pool, ld_dyp, scale, shift, mean, invstd, slope, partial, B, H, W, C, 1,
+                      nseg, segB, (cudaStream_t)stream);
+}
+
+static int bwd_finalize(const double* partial, int nparts, int nseg, double count, const float* gamma, const float* invstd,
+                        const float* xhat_absmax, float* dgamma, float* dbeta, double* coef, float* amax_bound, int C,
+                        int has_bn, cudaStream_t s) {
+    FSDET_CHECK_ARG(partial && nparts > 0 && C > 0 && nseg >= 1 && (!has_bn || (coef && gamma && invstd)), "bn_bwd_finalize: bad args");
+    FSDET_CHECK_ARG(!(amax_bound && has_bn) || xhat_absmax, "bn_bwd_finalize: the bound of max|dz| needs xhat_absmax");
+    double* sums = const_cast<double*>(partial) + (size_t)nseg * nparts * 3 * C;  // the extra rows
+    dim3 block(32, 32), grid(ceil_div(3 * C, 32), nseg);
+    if (nseg > 1) colsum_dd_kernel<true><<<grid, block, 0, s>>>(partial, nparts, 3 * C, 2 * C, sums, amax_bound);
+    else colsum_dd_kernel<false><<<grid, block, 0, s>>>(partial, nparts, 3 * C, 2 * C, sums, amax_bound);
+    int st = launch_status("bn_bwd_finalize/colsum");
+    if (st) return st;
+    if (nseg > 1)
+        bn_bwd_finalize_kernel<true><<<ceil_div(C, 128), 128, 0, s>>>(sums, count, gamma, invstd, xhat_absmax, dgamma, dbeta, coef,
+                                                                      amax_bound, C, has_bn, nseg);
+    else
+        bn_bwd_finalize_kernel<false><<<ceil_div(C, 128), 128, 0, s>>>(sums, count, gamma, invstd, xhat_absmax, dgamma, dbeta, coef,
+                                                                       amax_bound, C, has_bn, 1);
+    return launch_status("bn_bwd_finalize");
 }
 
 extern "C" int fsdet_bn_bwd_finalize(const double* partial, int nparts, double count, const float* gamma,
                                      const float* invstd, const float* xhat_absmax, float* dgamma, float* dbeta, double* coef,
                                      float* amax_bound, int C, int has_bn, void* stream) {
-    FSDET_CHECK_ARG(partial && nparts > 0 && C > 0 && (!has_bn || (coef && gamma && invstd)), "bn_bwd_finalize: bad args");
-    FSDET_CHECK_ARG(!(amax_bound && has_bn) || xhat_absmax, "bn_bwd_finalize: the bound of max|dz| needs xhat_absmax");
-    cudaStream_t s = (cudaStream_t)stream;
-    double* sums = const_cast<double*>(partial) + (size_t)nparts * 3 * C;  // the extra row
-    dim3 block(32, 32), grid(ceil_div(3 * C, 32));
-    colsum_dd_kernel<<<grid, block, 0, s>>>(partial, nparts, 3 * C, 2 * C, sums, amax_bound);
-    int st = launch_status("bn_bwd_finalize/colsum");
-    if (st) return st;
-    bn_bwd_finalize_kernel<<<ceil_div(C, 128), 128, 0, s>>>(sums, count, gamma, invstd, xhat_absmax, dgamma, dbeta, coef, amax_bound, C, has_bn);
-    return launch_status("bn_bwd_finalize");
+    return bwd_finalize(partial, nparts, 1, count, gamma, invstd, xhat_absmax, dgamma, dbeta, coef, amax_bound, C, has_bn,
+                        (cudaStream_t)stream);
 }
 
-extern "C" int fsdet_bn_act_bwd_apply(const float* z, int ldz, const float* dy_full, int ld_dyf, const float* dy_pool,
-                                      int ld_dyp, const float* scale, const float* shift, const float* mean,
-                                      const float* invstd, const double* coef, float slope, float* dz, int lddz,
-                                      void* dz_hi, void* dz_lo, int cpad, const float* amax, int B, int H, int W, int C,
-                                      int has_bn, void* stream) {
+extern "C" int fsdet_bn_bwd_finalize_seg(const double* partial, int nparts, int nseg, size_t seg_pix, const float* gamma,
+                                         const float* invstd, const float* xhat_absmax, float* dgamma, float* dbeta,
+                                         double* coef, float* amax_bound, int C, void* stream) {
+    FSDET_CHECK_ARG(seg_pix > 0, "bn_bwd_finalize_seg: empty segments");
+    return bwd_finalize(partial, nparts, nseg, (double)seg_pix, gamma, invstd, xhat_absmax, dgamma, dbeta, coef, amax_bound, C, 1,
+                        (cudaStream_t)stream);
+}
+
+static int bwd_apply(const float* z, int ldz, const float* dy_full, int ld_dyf, const float* dy_pool, int ld_dyp,
+                     const float* scale, const float* shift, const float* mean, const float* invstd, const double* coef,
+                     float slope, float* dz, int lddz, void* dz_hi, void* dz_lo, int cpad, const float* amax, int B, int H,
+                     int W, int C, int has_bn, int nseg, int segB, cudaStream_t s) {
     FSDET_CHECK_ARG(z && scale && shift && (dz || dz_hi) && (dy_full || dy_pool), "bn_act_bwd_apply: null pointer");
     FSDET_CHECK_ARG(!has_bn || (mean && invstd && coef), "bn_act_bwd_apply: BN needs mean/invstd/coef");
     FSDET_CHECK_ARG(C % 4 == 0 && ldz % 4 == 0 && ld_dyf % 4 == 0 && ld_dyp % 4 == 0 && lddz % 4 == 0,
@@ -764,8 +1014,28 @@ extern "C" int fsdet_bn_act_bwd_apply(const float* z, int ldz, const float* dy_f
     a.z = z; a.dyf = dy_full; a.dyp = dy_pool; a.scale = scale; a.shift = shift; a.mean = mean; a.invstd = invstd;
     a.coef = coef; a.dz = dz; a.dh = (__half*)dz_hi; a.dl = (__half*)dz_lo; a.amax = amax; a.partial = nullptr;
     a.ldz = ldz; a.ld_dyf = ld_dyf; a.ld_dyp = ld_dyp; a.lddz = lddz; a.cpad = cpad;
-    a.B = B; a.H = H; a.W = W; a.C = C; a.slope = slope; a.has_bn = has_bn;
-    return launch_bwd(true, a, (cudaStream_t)stream);
+    a.B = B; a.H = H; a.W = W; a.C = C; a.segB = segB; a.slope = slope; a.has_bn = has_bn;
+    return launch_bwd(true, a, nseg, s);
+}
+
+extern "C" int fsdet_bn_act_bwd_apply(const float* z, int ldz, const float* dy_full, int ld_dyf, const float* dy_pool,
+                                      int ld_dyp, const float* scale, const float* shift, const float* mean,
+                                      const float* invstd, const double* coef, float slope, float* dz, int lddz,
+                                      void* dz_hi, void* dz_lo, int cpad, const float* amax, int B, int H, int W, int C,
+                                      int has_bn, void* stream) {
+    return bwd_apply(z, ldz, dy_full, ld_dyf, dy_pool, ld_dyp, scale, shift, mean, invstd, coef, slope, dz, lddz, dz_hi, dz_lo,
+                     cpad, amax, B, H, W, C, has_bn, 1, B, (cudaStream_t)stream);
+}
+
+extern "C" int fsdet_bn_act_bwd_apply_seg(const float* z, int ldz, const float* dy_full, int ld_dyf, const float* dy_pool,
+                                          int ld_dyp, const float* scale, const float* shift, const float* mean,
+                                          const float* invstd, const double* coef, float slope, float* dz, int lddz,
+                                          void* dz_hi, void* dz_lo, int cpad, const float* amax, int B, int H, int W, int C,
+                                          int nseg, size_t seg_pix, void* stream) {
+    const int segB = seg_images(B, H, W, nseg, (long long)seg_pix);
+    FSDET_CHECK_ARG(segB > 0, "bn_act_bwd_apply_seg: %d segments of %zu pixels do not split %d images of %dx%d", nseg, seg_pix, B, H, W);
+    return bwd_apply(z, ldz, dy_full, ld_dyf, dy_pool, ld_dyp, scale, shift, mean, invstd, coef, slope, dz, lddz, dz_hi, dz_lo,
+                     cpad, amax, B, H, W, C, 1, nseg, segB, (cudaStream_t)stream);
 }
 
 #endif  // FSDET_HOST_EMULATION

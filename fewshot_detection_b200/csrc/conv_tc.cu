@@ -71,54 +71,6 @@ __global__ void __launch_bounds__(256) split_f16_kernel(const float* __restrict_
     *reinterpret_cast<uint2*>(lo + o) = *reinterpret_cast<uint2*>(l);
 }
 
-// ------------------------------------------------------------------ column statistics of z (BN partials)
-// one CTA per strip of `strip` pixels: partial[blockIdx.x] = [sum(C) | sum of squares(C) | min(C) | max(C)]
-__global__ void __launch_bounds__(256) colstats_kernel(const float* __restrict__ z, int ld, long long npix, int C, int strip,
-                                                       float* __restrict__ part) {
-    // threads: x = channel vector lane (float4), y = pixel lane
-    const int C4 = C >> 2;
-    const int TC = blockDim.x, TY = blockDim.y;
-    long long p0 = (long long)blockIdx.x * strip, p1 = p0 + strip < npix ? p0 + strip : npix;
-    extern __shared__ float red[];  // [TY][TC*16]
-    for (int cv0 = 0; cv0 < C4; cv0 += TC) {
-        int cv = cv0 + threadIdx.x;
-        float s[4] = {0, 0, 0, 0}, q[4] = {0, 0, 0, 0};
-        float mn[4] = {INFINITY, INFINITY, INFINITY, INFINITY}, mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-        if (cv < C4)
-            for (long long p = p0 + threadIdx.y; p < p1; p += 4 * TY) {   // four loads in flight, accumulated in row order
-                float4 v[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u)
-                    if (p + u * TY < p1) v[u] = ldg4(z + (p + u * TY) * ld + cv * 4);
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    if (p + u * TY >= p1) break;
-                    const float f[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        s[k] += f[k]; q[k] += f[k] * f[k]; mn[k] = fminf(mn[k], f[k]); mx[k] = fmaxf(mx[k], f[k]);
-                    }
-                }
-            }
-        float* mine = red + ((size_t)threadIdx.y * TC + threadIdx.x) * 16;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) { mine[k] = s[k]; mine[4 + k] = q[k]; mine[8 + k] = mn[k]; mine[12 + k] = mx[k]; }
-        __syncthreads();
-        // column j = (channel lane, statistic, component) reduced over the TY pixel lanes in a fixed order, all threads busy
-        for (int j = threadIdx.y * TC + threadIdx.x; j < TC * 16; j += TC * TY) {
-            const int lane = j >> 4, stat = (j >> 2) & 3, comp = j & 3;
-            if (cv0 + lane >= C4) continue;
-            float t = red[j];
-            for (int r = 1; r < TY; ++r) {
-                const float o = red[(size_t)r * TC * 16 + j];
-                t = stat < 2 ? t + o : (stat == 2 ? fminf(t, o) : fmaxf(t, o));
-            }
-            part[(long long)blockIdx.x * 4 * C + stat * C + (cv0 + lane) * 4 + comp] = t;
-        }
-        __syncthreads();
-    }
-}
-
 constexpr int TC_BK = 64;                       // halves per 128-byte row (im2col debug tile, weight-gradient tiles)
 constexpr int TC_A_BYTES = 128 * TC_BK * 2;     // 16 KB per plane
 
@@ -493,26 +445,6 @@ extern "C" int fsdet_split_f16(const float* src, int ld, int C, int Cpad, size_t
     split_f16_kernel<<<ceil_div(n, 256), 256, 0, (cudaStream_t)stream>>>(src, ld, C, Cpad / 4, (long long)rows, amax, (__half*)hi,
                                                                          (__half*)lo);
     return launch_status("split_f16");
-}
-
-// pixels per partial row: large tensors use long strips (few partial rows, little reduction work afterwards), small
-// ones short strips so that every SM still gets CTAs
-static int stat_strip(size_t npix) {
-    long long s = (long long)(npix / (8 * kNumSMs)) / 32 * 32;
-    return (int)(s < 32 ? 32 : (s > 1024 ? 1024 : s));
-}
-extern "C" int fsdet_colstats_rows(size_t npix) { return ceil_div((long long)npix, stat_strip(npix)); }
-
-extern "C" int fsdet_colstats(const float* z, int ld, size_t npix, int C, float* partial, void* stream) {
-    FSDET_CHECK_ARG(z && partial && C % 4 == 0 && ld % 4 == 0 && aligned16(z), "colstats: C=%d ld=%d", C, ld);
-    if (npix == 0) return 0;
-    int C4 = C / 4;
-    int TCx = C4 >= 32 ? 32 : (C4 >= 16 ? 16 : (C4 >= 8 ? 8 : (C4 >= 4 ? 4 : (C4 >= 2 ? 2 : 1))));
-    int TY = 256 / TCx;
-    dim3 block(TCx, TY);
-    size_t smem = (size_t)TY * TCx * 16 * sizeof(float);
-    colstats_kernel<<<fsdet_colstats_rows(npix), block, smem, (cudaStream_t)stream>>>(z, ld, (long long)npix, C, stat_strip(npix), partial);
-    return launch_status("colstats");
 }
 
 extern "C" int fsdet_conv_tc_supported(int Cin, int Cout, int ksize) {

@@ -130,8 +130,17 @@ def _copy_blocks(blocks):
 
 
 class Darknet(nn.Module):
-    def __init__(self, darknet_file, learnet_file):
+    """replicas: R, the number of nn.DataParallel replicas one training step of the reference runs (its shipped configs
+    train on 4 GPUs).  A train-mode `forward` then splits the query batch and the support batch into R contiguous
+    chunks: every BatchNorm normalises each chunk by its own statistics (the running statistics follow replica 0),
+    and replica r's query images are reweighted by replica r's vectors.  The output keeps the row order b * n_cls + c.
+    Evaluation and the separate `meta_forward` / `detect_forward` calls are unaffected."""
+
+    def __init__(self, darknet_file, learnet_file, replicas=1):
         super(Darknet, self).__init__()
+        if int(replicas) < 1:
+            raise ValueError('replicas must be >= 1, got %r' % (replicas,))
+        self.replicas = int(replicas)
         self.blocks = darknet_file if isinstance(darknet_file, list) else parse_cfg(darknet_file)
         self.learnet_blocks = learnet_file if isinstance(learnet_file, list) else parse_cfg(learnet_file)
         self.models = create_network(self, self.blocks, RegionLossV2)
@@ -174,8 +183,17 @@ class Darknet(nn.Module):
         return run_network(self._det, [x], dw, self._params(self.models), self.training)
 
     def forward(self, x, metax, mask, ids=None):
-        dynamic_weights = self.meta_forward(metax, mask)
-        return self.detect_forward(x, dynamic_weights)
+        R = self.replicas if self.training else 1
+        if R == 1:
+            dynamic_weights = self.meta_forward(metax, mask)
+            return self.detect_forward(x, dynamic_weights)
+        if x.shape[0] % R or metax.shape[0] % R:
+            raise ValueError('%d replicas need a query batch and a support batch divisible by %d, got x %s and metax %s'
+                             % (R, R, tuple(x.shape), tuple(metax.shape)))
+        inputs = [metax, mask] if cfg.metain_type in [2, 3] else [metax]
+        dw = run_network(self._ler, inputs, None, self._params(self.learnet_models), True, segments=R)
+        self.loss = None
+        return run_network(self._det, [x], dw, self._params(self.models), True, segments=R)
 
     def print_network(self):
         for name, blocks in (('detector', self.blocks), ('reweighting net', self.learnet_blocks)):

@@ -173,7 +173,7 @@ class MetaBatcher(object):
     inds: sequence of (clsid, metaind) like MetaDataset.inds.  `batch(indices)` returns (metax float32 CUDA
     [n, 3, S, S], mask float32 CUDA [n, 1, S, S][, clsids])."""
 
-    def __init__(self, metalines, inds, classes=None, train=False, ensemble=False, with_ids=False, filter=None):
+    def __init__(self, metalines, inds, classes=None, train=False, ensemble=False, with_ids=False, filter=None, replicas=1):
         if cfg.metain_type not in (1, 2):
             raise NotImplementedError('metain_type %r (the cropped-object inputs 3/4 are not used by the shipped cfgs)' % cfg.metain_type)
         self.metalines, self.inds = metalines, list(inds)
@@ -181,7 +181,8 @@ class MetaBatcher(object):
         self.train, self.ensemble, self.with_ids, self.filter = train, ensemble, with_ids, filter
         self.meta_shape = (cfg.meta_width, cfg.meta_height)
         self.mask_shape = (cfg.mask_width, cfg.mask_height)
-        self.batch_size = len(self.classes)      # one support image per class per process (MetaDataset.batch_size / num_gpus)
+        # one support image per class per replica (MetaDataset.batch_size / num_gpus), `replicas` replicas per step
+        self.batch_size = len(self.classes) * replicas
 
     def __len__(self):
         return len(self.inds)

@@ -126,6 +126,17 @@ class Act(object):
     def slice(self, off, C):
         return Act(self.buf, self.off + off, C, self.B, self.H, self.W, self.needs_grad, parent=(self, off))
 
+    def images(self, b0, nb):
+        """Images [b0, b0 + nb) of this activation: a view of the same fp32 buffer and / or fp16 planes (same scale)."""
+        hw = self.H * self.W
+        rows = slice(b0 * hw, (b0 + nb) * hw)
+        a = Act(self.buf[rows] if self.buf is not None else None, self.off, self.C, nb, self.H, self.W, self.needs_grad,
+                dev=self.dev)
+        if self.planes is not None:
+            hi, lo, amax = self.planes
+            a.planes = (hi[rows], lo[rows], amax)
+        return a
+
     def grad_for_write(self):
         """Returns (grad Act, accumulate flag) for a consumer about to write its
         contribution to d(loss)/d(this activation)."""
@@ -266,8 +277,9 @@ def compile_blocks(blocks):
 
 # ------------------------------------------------------------- executor
 class Tape(object):
-    def __init__(self):
+    def __init__(self, segments=1):
         self.records = []
+        self.segments = segments    # replicas of the recorded forward pass (NetRunner.forward)
 
 
 class NetRunner(object):
@@ -283,6 +295,8 @@ class NetRunner(object):
         self.profile = None     # optional dict name -> [flops, [(start_event, end_event), ...]]
         self.side = None        # second stream for the weight gradients (created by the first backward pass)
         self._side_used = False
+        self._nseg = 1          # replicas of the current forward pass (see forward)
+        self._bwd_segments = 1  # replicas of the tape the current backward pass replays
         self._keep = []         # tensors allocated on the main stream that the side stream still reads or writes (until the join)
 
     # -- helpers ---------------------------------------------------------
@@ -393,6 +407,10 @@ class NetRunner(object):
         not include a concurrent kernel's share of the SMs)."""
         if not WGRAD_STREAM or self.profile is not None:
             return False
+        if self._bwd_segments > 1:
+            # replica steps keep every launch on one stream: with the weight gradients on the second stream they gave
+            # non-finite gradients in some runs while another process shared the GPU (never with one stream)
+            return False
         if self.grad_hook is not None and os.environ.get('FSDET_WGRAD_STREAM') != '2':
             # data-parallel runs launch their bucket collectives from the backward pass: keep one compute stream there
             # (the overlap is worth ~0.6 % of a step; FSDET_WGRAD_STREAM=2 forces it for experiments)
@@ -499,15 +517,21 @@ class NetRunner(object):
             self._wp = plan['by_id']
 
     # -- forward -----------------------------------------------------------
-    def forward(self, inputs, extra=None, training=True, record=True):
+    def forward(self, inputs, extra=None, training=True, record=True, segments=1):
         """inputs: list of NCHW tensors concatenated along channels (image[, mask]).
         extra: reweighting vectors [n_cls, K(,1,1)] for a dynamic head.
+        segments: the batch is `segments` replicas of B / segments images (nn.DataParallel's scatter): batch-statistics
+        BatchNorm normalises each replica by its own statistics, and a dynamic head takes `segments` * n_cls vectors,
+        replica r's images reweighted by rows [r * n_cls, (r + 1) * n_cls).
         Returns (output tensor, tape)."""
         x0 = inputs[0]
         dev = x0.device
         B, _, H, W = x0.shape
+        if segments < 1 or B % segments:
+            raise ValueError('a batch of %d images does not split into %d replicas' % (B, segments))
+        self._nseg = segments
         st = _stream()
-        tape = Tape() if record else None
+        tape = Tape(segments) if record else None
         c0 = x0.shape[1]
         c1 = inputs[1].shape[1] if len(inputs) > 1 else 0
         if c0 + c1 != self.in_ch:
@@ -648,20 +672,34 @@ class NetRunner(object):
             assert cout_p == s.cout, 'BatchNorm conv with Cout % 4 != 0 is unsupported'
             z = Act.new(B, H, W, s.cout, dev)
             use_batch_stats = training or not bn.track_running_stats
-            rows_cap = max(_lib.lib.fsdet_conv_stat_rows(npix), _lib.lib.fsdet_colstats_rows(npix), (npix + 127) // 128 + 1, 3 * _lib.lib.fsdet_num_sms())
-            stat = _empty(rows_cap + _lib.lib.fsdet_bn_stat_scratch_rows(), 4 * s.cout, device=dev) if use_batch_stats else None
+            # replicas: the convolution writes z only, and one segmented pass reads it for per-replica statistics
+            nseg = self._nseg if use_batch_stats else 1
             wp = getattr(self, '_wp', {}).get(id(wuse))
-            rows = self._conv('fwd', x, wuse, None, z, stat, cin_p, s.cout, s.k, 0, st, wplanes=wp['fwd'] if wp else None)
-            vec = _empty(5, s.cout, device=dev)  # mean, invstd, scale, shift, max|xhat| (batch statistics only)
-            vec.xh_ok = bool(use_batch_stats)
-            amax_y = _empty(1, device=dev) if use_batch_stats else None
             upd = training and bn.track_running_stats
-            call('fsdet_bn_finalize', ptr(stat), rows, float(npix), ptr(bn.weight), ptr(bn.bias),
-                 ptr(bn.running_mean) if (upd or not use_batch_stats) else None,
-                 ptr(bn.running_var) if (upd or not use_batch_stats) else None,
-                 BN_MOMENTUM if bn.momentum is None else float(bn.momentum), float(bn.eps),
-                 ptr(vec[0]), ptr(vec[1]), ptr(vec[2]), ptr(vec[3]), s.slope, ptr(amax_y), ptr(vec[4]), s.cout,
-                 1 if use_batch_stats else 0, st)
+            momentum = BN_MOMENTUM if bn.momentum is None else float(bn.momentum)
+            amax_y = _empty(1, device=dev) if use_batch_stats else None
+            vec = _empty(5, nseg, s.cout, device=dev)  # mean, invstd, scale, shift, max|xhat| per replica (batch statistics only)
+            vec.xh_ok = bool(use_batch_stats)
+            vec.nseg = nseg
+            if nseg > 1:
+                seg_pix = npix // nseg
+                rows = _lib.lib.fsdet_bn_seg_colstats_rows(seg_pix, nseg)
+                stat = _empty(nseg * (rows + _lib.lib.fsdet_bn_stat_scratch_rows()), 4 * s.cout, device=dev)
+                self._conv('fwd', x, wuse, None, z, None, cin_p, s.cout, s.k, 0, st, wplanes=wp['fwd'] if wp else None)
+                call('fsdet_bn_seg_colstats', z.ptr, z.ld, seg_pix, nseg, s.cout, ptr(stat), st)
+                call('fsdet_bn_seg_finalize', ptr(stat), rows, nseg, seg_pix, ptr(bn.weight), ptr(bn.bias),
+                     ptr(bn.running_mean) if upd else None, ptr(bn.running_var) if upd else None, momentum, float(bn.eps),
+                     ptr(vec[0]), ptr(vec[1]), ptr(vec[2]), ptr(vec[3]), s.slope, ptr(amax_y), ptr(vec[4]), s.cout, st)
+            else:
+                rows_cap = max(_lib.lib.fsdet_conv_stat_rows(npix), _lib.lib.fsdet_colstats_rows(npix), (npix + 127) // 128 + 1, 3 * _lib.lib.fsdet_num_sms())
+                stat = _empty(rows_cap + _lib.lib.fsdet_bn_stat_scratch_rows(), 4 * s.cout, device=dev) if use_batch_stats else None
+                rows = self._conv('fwd', x, wuse, None, z, stat, cin_p, s.cout, s.k, 0, st, wplanes=wp['fwd'] if wp else None)
+                call('fsdet_bn_finalize', ptr(stat), rows, float(npix), ptr(bn.weight), ptr(bn.bias),
+                     ptr(bn.running_mean) if (upd or not use_batch_stats) else None,
+                     ptr(bn.running_var) if (upd or not use_batch_stats) else None,
+                     momentum, float(bn.eps),
+                     ptr(vec[0]), ptr(vec[1]), ptr(vec[2]), ptr(vec[3]), s.slope, ptr(amax_y), ptr(vec[4]), s.cout,
+                     1 if use_batch_stats else 0, st)
             if upd and bn.num_batches_tracked is not None:
                 bn.num_batches_tracked += 1
             # which outputs exist, and in which representation (fp32 and / or fp16 planes)
@@ -694,10 +732,14 @@ class NetRunner(object):
                     pooled.amax = amax_y   # upper bound (max-pool of y): still a valid plane scale
             f32 = full if (full is not None and full.buf is not None) else None
             p32 = pooled if (pooled is not None and pooled.buf is not None) else None
-            call('fsdet_bn_act_fwd', z.ptr, z.ld, ptr(vec[2]), ptr(vec[3]), s.slope,
-                 f32.ptr if f32 else None, f32.ld if f32 else 0, p32.ptr if p32 else None, p32.ld if p32 else 0,
-                 ptr(fpl[0]) if fpl else None, ptr(fpl[1]) if fpl else None, ptr(ppl[0]) if ppl else None,
-                 ptr(ppl[1]) if ppl else None, cp64, ptr(amax_y) if (fpl or ppl) else None, B, H, W, s.cout, st)
+            act_args = (z.ptr, z.ld, ptr(vec[2]), ptr(vec[3]), s.slope,
+                        f32.ptr if f32 else None, f32.ld if f32 else 0, p32.ptr if p32 else None, p32.ld if p32 else 0,
+                        ptr(fpl[0]) if fpl else None, ptr(fpl[1]) if fpl else None, ptr(ppl[0]) if ppl else None,
+                        ptr(ppl[1]) if ppl else None, cp64, ptr(amax_y) if (fpl or ppl) else None, B, H, W, s.cout)
+            if nseg > 1:
+                call('fsdet_bn_act_fwd_seg', *act_args, nseg, npix // nseg, st)
+            else:
+                call('fsdet_bn_act_fwd', *act_args, st)
             rec = ('convbn', s, x, wuse, z, vec, full, pooled, conv, bn)
             return ((full, pooled) if s.fuse_pool else full), rec
         # conv + bias (+ leaky), no BN
@@ -748,16 +790,31 @@ class NetRunner(object):
         n_cls = rw.shape[0]
         if rw.numel() != n_cls * K:
             raise ValueError('dynamic weights must be [n_cls, %d, 1, 1], got %s' % (K, tuple(rw.shape)))
-        rw2 = rw.detach().reshape(n_cls, K).contiguous()
+        R = self._nseg
+        if n_cls % R:
+            raise ValueError('%d reweighting vectors do not split into %d replicas' % (n_cls, R))
+        n_cls //= R
         O = head.cout
         N = n_cls * O
         Npad = _round_up(N, 64)
         W = conv.weight  # [O, K, 1, 1]: OIHW == OHWI storage for 1x1
-        weff = _empty(Npad, K, device=dev)
         beff = _empty(Npad, device=dev)
-        call('fsdet_head_weff', ptr(W), ptr(conv.bias), ptr(rw2), ptr(weff), ptr(beff), n_cls, O, K, Npad, st)
         z = Act.new(x.B, x.H, x.W, Npad, dev)
-        self._conv('head', x, weff, None, z, None, K, Npad, 1, 0, st)
+        if R == 1:
+            rw2 = rw.detach().reshape(n_cls, K).contiguous()
+            weff = _empty(Npad, K, device=dev)
+            call('fsdet_head_weff', ptr(W), ptr(conv.bias), ptr(rw2), ptr(weff), ptr(beff), n_cls, O, K, Npad, st)
+            self._conv('head', x, weff, None, z, None, K, Npad, 1, 0, st)
+        else:
+            # replica r: its images through W (.) rw_r, rw_r = rows [r * n_cls, (r + 1) * n_cls) of the vectors
+            rw2 = rw.detach().reshape(R, n_cls, K).contiguous()
+            weff = _empty(R, Npad, K, device=dev)
+            nb = x.B // R
+            if 'head' in TC_PARTS and self._tc_ok(K, Npad, 1):
+                self._planes(x, st)     # one split (one scale) shared by every replica's GEMMs
+            for r in range(R):
+                call('fsdet_head_weff', ptr(W), ptr(conv.bias), ptr(rw2[r]), ptr(weff[r]), ptr(beff), n_cls, O, K, Npad, st)
+                self._conv('head', x.images(r * nb, nb), weff[r], None, z.images(r * nb, nb), None, K, Npad, 1, 0, st)
         out = _empty(x.B * n_cls, O, x.H, x.W, device=dev)
         call('fsdet_nhwc_to_nchw', z.ptr, z.ld, ptr(beff), ptr(out), x.B, N, x.H * x.W, st)  # + bias[o]
         rec = ('head', s, head, x, rw2, weff, conv, n_cls, O, Npad)
@@ -773,6 +830,7 @@ class NetRunner(object):
         drw = None
         self._side_used = False
         self._main = torch.cuda.current_stream()
+        self._bwd_segments = tape.segments
         try:
             drw = self._backward_records(tape, gout, st)
         finally:
@@ -910,13 +968,19 @@ class NetRunner(object):
                     f()
             self._done(conv.weight, bn.weight, bn.bias)
             return
-        rows = _lib.lib.fsdet_bn_bwd_rows(B, H, W)
-        part = _empty(rows + 1, 3 * s.cout, dtype=torch.float64, device=dev)
-        coef = _empty(2, s.cout, dtype=torch.float64, device=dev)
+        nseg = vec.nseg
+        seg = (nseg, x.npix // nseg)
+        rows = _lib.lib.fsdet_bn_seg_bwd_rows(B, H, W, nseg) if nseg > 1 else _lib.lib.fsdet_bn_bwd_rows(B, H, W)
+        part = _empty(nseg * (rows + 1), 3 * s.cout, dtype=torch.float64, device=dev)
+        coef = _empty(nseg, 2, s.cout, dtype=torch.float64, device=dev)
         a_gf = (gf.ptr, gf.ld) if gf is not None else (None, 0)
         a_gp = (gp.ptr, gp.ld) if gp is not None else (None, 0)
-        call('fsdet_bn_act_bwd_reduce', z.ptr, z.ld, a_gf[0], a_gf[1], a_gp[0], a_gp[1], ptr(vec[2]), ptr(vec[3]),
-             ptr(vec[0]), ptr(vec[1]), s.slope, ptr(part), B, H, W, s.cout, 1, st)
+        if nseg > 1:
+            call('fsdet_bn_act_bwd_reduce_seg', z.ptr, z.ld, a_gf[0], a_gf[1], a_gp[0], a_gp[1], ptr(vec[2]), ptr(vec[3]),
+                 ptr(vec[0]), ptr(vec[1]), s.slope, ptr(part), B, H, W, s.cout, *seg, st)
+        else:
+            call('fsdet_bn_act_bwd_reduce', z.ptr, z.ld, a_gf[0], a_gf[1], a_gp[0], a_gp[1], ptr(vec[2]), ptr(vec[3]),
+                 ptr(vec[0]), ptr(vec[1]), s.slope, ptr(part), B, H, W, s.cout, 1, st)
         # which GEMMs will read dz, and in which form: the tensor-core ones take fp16 planes, written directly by
         # the apply pass (scaled by the bound of max|dz| from the finalize step); fp32 dz only if a SIMT kernel needs it
         cin_p = x.C
@@ -925,8 +989,12 @@ class NetRunner(object):
         want_planes = USE_TC and s.cout % 64 == 0 and (wg_tc or dg_tc) and getattr(vec, 'xh_ok', False)
         want_f32 = (not want_planes) or (not wg_tc) or (x.needs_grad and not dg_tc)
         amax = _empty(1, device=dev) if want_planes else None
-        call('fsdet_bn_bwd_finalize', ptr(part), rows, float(x.npix), ptr(bn.weight), ptr(vec[1]), ptr(vec[4]), ptr(gg), ptr(gb),
-             ptr(coef), ptr(amax), s.cout, 1, st)
+        if nseg > 1:
+            call('fsdet_bn_bwd_finalize_seg', ptr(part), rows, *seg, ptr(bn.weight), ptr(vec[1]), ptr(vec[4]), ptr(gg), ptr(gb),
+                 ptr(coef), ptr(amax), s.cout, st)
+        else:
+            call('fsdet_bn_bwd_finalize', ptr(part), rows, float(x.npix), ptr(bn.weight), ptr(vec[1]), ptr(vec[4]), ptr(gg),
+                 ptr(gb), ptr(coef), ptr(amax), s.cout, 1, st)
         planes = None
         if want_planes:
             planes = (torch.empty(x.npix, s.cout, dtype=torch.float16, device=dev),
@@ -936,9 +1004,13 @@ class NetRunner(object):
             dz.planes = planes
         else:
             dz = Act.planes_only(B, H, W, s.cout, dev, planes)
-        call('fsdet_bn_act_bwd_apply', z.ptr, z.ld, a_gf[0], a_gf[1], a_gp[0], a_gp[1], ptr(vec[2]), ptr(vec[3]),
-             ptr(vec[0]), ptr(vec[1]), ptr(coef), s.slope, dz.ptr if want_f32 else None, dz.ld if want_f32 else 0,
-             ptr(planes[0]) if planes else None, ptr(planes[1]) if planes else None, s.cout, ptr(amax), B, H, W, s.cout, 1, st)
+        apply_args = (z.ptr, z.ld, a_gf[0], a_gf[1], a_gp[0], a_gp[1], ptr(vec[2]), ptr(vec[3]), ptr(vec[0]), ptr(vec[1]),
+                      ptr(coef), s.slope, dz.ptr if want_f32 else None, dz.ld if want_f32 else 0,
+                      ptr(planes[0]) if planes else None, ptr(planes[1]) if planes else None, s.cout, ptr(amax), B, H, W, s.cout)
+        if nseg > 1:
+            call('fsdet_bn_act_bwd_apply_seg', *apply_args, *seg, st)
+        else:
+            call('fsdet_bn_act_bwd_apply', *apply_args, 1, st)
         cin_p = x.C
 
         def weight_grad(sw):
@@ -1035,16 +1107,46 @@ class NetRunner(object):
             nws = _lib.lib.fsdet_head_bias_grad_workspace_floats(x.npix, n_cls, O)
             ws = _empty(max(nws, 1), device=dev)
             call('fsdet_head_bias_grad', dzh.ptr, dzh.ld, ptr(gb), ptr(ws), x.npix, n_cls, O, st)
-        dweff = _empty(Npad, K, device=dev)
-        self._wgrad(x, dzh, dweff, K, Npad, 1, st)
-        drw = _empty(n_cls, K, device=dev)
-        call('fsdet_head_param_grads', ptr(dweff), ptr(conv.weight), ptr(rw2), ptr(gw), ptr(drw), n_cls, O, K, st)
+        if rw2.dim() == 2:
+            dweff = _empty(Npad, K, device=dev)
+            self._wgrad(x, dzh, dweff, K, Npad, 1, st)
+            drw = _empty(n_cls, K, device=dev)
+            call('fsdet_head_param_grads', ptr(dweff), ptr(conv.weight), ptr(rw2), ptr(gw), ptr(drw), n_cls, O, K, st)
+            for f in (fin_w, fin_b):
+                if f:
+                    f()
+            self._done(conv.weight, conv.bias)
+            self._dgrad(x, dzh, weff, K, Npad, 1, st)
+            return drw
+        # replicas: dweff_r over replica r's pixels gives drw_r and dW_r; dW is the sum over the replicas (in order)
+        R = rw2.shape[0]
+        nb = x.B // R
+        if USE_TC:
+            self._planes(dzh, st)   # one split (one scale) shared by every replica's GEMMs
+        dweff = _empty(R, Npad, K, device=dev)
+        drw = _empty(R, n_cls, K, device=dev)
+        dw_r = _empty(O, K, device=dev)
+        for r in range(R):
+            self._wgrad(x.images(r * nb, nb), dzh.images(r * nb, nb), dweff[r], K, Npad, 1, st)
+            call('fsdet_head_param_grads', ptr(dweff[r]), ptr(conv.weight), ptr(rw2[r]), ptr(gw) if r == 0 else ptr(dw_r),
+                 ptr(drw[r]), n_cls, O, K, st)
+            if r:
+                call('fsdet_copy_channels', ptr(dw_r), K, ptr(gw), K, O, K, 1, st)
         for f in (fin_w, fin_b):
             if f:
                 f()
         self._done(conv.weight, conv.bias)
-        self._dgrad(x, dzh, weff, K, Npad, 1, st)
-        return drw
+        if x.needs_grad:
+            g, acc = x.grad_for_write()
+            for r in range(R):
+                self._dgrad_into(dzh.images(r * nb, nb), g.images(r * nb, nb), acc, weff[r], K, Npad, st)
+        return drw.view(R * n_cls, K)
+
+    def _dgrad_into(self, dz, g, acc, w_ohwi, cin_p, cout, st):
+        """dX = dZ x W of a 1x1 convolution, written (or added, acc=1) into gradient view `g`."""
+        wt = _empty(cin_p, 1, cout, device=dz.dev)
+        call('fsdet_weight_flip_transpose', ptr(w_ohwi), ptr(wt), cout, 1, cin_p, st)
+        self._conv('dgrad', dz, wt, None, g, None, cout, cin_p, 1, acc, st)
 
 
 class _NetFunction(torch.autograd.Function):
@@ -1053,10 +1155,10 @@ class _NetFunction(torch.autograd.Function):
     executor (None is returned for them)."""
 
     @staticmethod
-    def forward(ctx, runner, training, n_in, has_extra, *tensors):
+    def forward(ctx, runner, training, segments, n_in, has_extra, *tensors):
         inputs = list(tensors[:n_in])
         extra = tensors[n_in] if has_extra else None
-        out, tape = runner.forward(inputs, extra, training=training, record=True)
+        out, tape = runner.forward(inputs, extra, training=training, record=True, segments=segments)
         ctx.runner = runner
         ctx.tape = tape
         ctx.n_in = n_in
@@ -1073,15 +1175,15 @@ class _NetFunction(torch.autograd.Function):
         grads = [None] * ctx.n_tensors
         if ctx.has_extra and drw is not None:
             grads[ctx.n_in] = drw.view(ctx.extra_shape)
-        return (None, None, None, None) + tuple(grads)
+        return (None, None, None, None, None) + tuple(grads)
 
 
-def run_network(runner, inputs, extra, params, training):
-    """Forward through `runner`; differentiable when grad mode is on."""
+def run_network(runner, inputs, extra, params, training, segments=1):
+    """Forward through `runner`; differentiable when grad mode is on.  segments: see NetRunner.forward."""
     need_grad = torch.is_grad_enabled() and (any(p.requires_grad for p in params) or
                                              (extra is not None and extra.requires_grad))
     if not need_grad:
-        out, _ = runner.forward(list(inputs), extra, training=training, record=False)
+        out, _ = runner.forward(list(inputs), extra, training=training, record=False, segments=segments)
         return out
     tensors = list(inputs) + ([extra] if extra is not None else []) + list(params)
-    return _NetFunction.apply(runner, training, len(inputs), extra is not None, *tensors)
+    return _NetFunction.apply(runner, training, segments, len(inputs), extra is not None, *tensors)

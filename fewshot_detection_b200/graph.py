@@ -71,7 +71,8 @@ class GraphedTrainStep(object):
 
     # ------------------------------------------------------------------ capture
     def _key(self, x, metax, target):
-        return (tuple(x.shape), tuple(metax.shape), tuple(target.shape), self.loss_mod.seen < 12800, str(cfg.neg_ratio))
+        return (tuple(x.shape), tuple(metax.shape), tuple(target.shape), self.loss_mod.seen < 12800, str(cfg.neg_ratio),
+                getattr(self.model, 'replicas', 1))
 
     def _capture(self, key, x, metax, mask, target):
         dev = x.device

@@ -170,6 +170,15 @@ def support_index(metafile, classes, nbatch, ensemble=False, shuffle=False):
     return metalines, inds
 
 
+def rank_support_rows(inds, n_cls, replicas, world, rank):
+    """The support index of `replicas` replicas per global step (built with cfg.num_gpus = replicas, consumed
+    replicas * n_cls entries at a time and scattered in order, replica r taking entries [r * n_cls, (r + 1) * n_cls) of
+    each step) as rank `rank` of `world` sees it: the entries of its replicas replicas / world * rank ... in order."""
+    per = replicas // world * n_cls
+    step = replicas * n_cls
+    return [inds[s + rank * per + j] for s in range(0, len(inds) - step + 1, step) for j in range(per)]
+
+
 def support_batches_per_epoch(train=True):
     """dataset.py:296-309: `nbatch` of MetaDataset - how many support batches one epoch's index holds."""
     if train:

@@ -58,12 +58,14 @@ def _sha(obj):
     return hashlib.sha256(json.dumps(obj, sort_keys=True).encode()).hexdigest()
 
 
-def fingerprint(darknet_blocks, learnet_blocks, data_options, world, batch_size, per_rank, trainlist=None):
+def fingerprint(darknet_blocks, learnet_blocks, data_options, world, batch_size, per_rank, trainlist=None, replicas=None):
     """What a resumed run must share with the run that wrote the state: the parsed darknet and learnet block lists, the
-    `.data` options, the world size, the global and per-rank batch and the built training list (length and hash; left
-    out while trainlist is None, so the other values can be checked before the list is built)."""
+    `.data` options, the world size, the replicas per step (nn.DataParallel replicas, default one per rank), the global
+    and per-rank batch and the built training list (length and hash; left out while trainlist is None, so the other
+    values can be checked before the list is built)."""
     fp = dict(cfg=_sha([[dict(b) for b in darknet_blocks], [dict(b) for b in learnet_blocks]]),
-              data=dict(data_options), world=int(world), batch=int(batch_size), per_rank=int(per_rank))
+              data=dict(data_options), world=int(world), batch=int(batch_size), per_rank=int(per_rank),
+              replicas=int(world if replicas is None else replicas))
     if trainlist is not None:
         fp['trainlist'] = dict(n=len(trainlist), sha256=_sha([str(l) for l in trainlist]))
     return fp
@@ -172,9 +174,10 @@ def check_weights(state, path, weightfile):
 def check_fingerprint(state, path, current):
     """Compare `current` (fingerprint() of this run) with the stored one, key by key in the order world, batches, cfg,
     .data, training list; the first difference is refused with both values."""
-    stored = state['fingerprint']
-    names = dict(world='world size', batch='global batch', per_rank='per-rank batch', cfg='cfg block lists (sha256)',
-                 data='.data options', trainlist='training list')
+    stored = dict(state['fingerprint'])
+    stored.setdefault('replicas', stored.get('world'))     # written before replicas were recorded: one per rank
+    names = dict(world='world size', replicas='replicas per step', batch='global batch', per_rank='per-rank batch',
+                 cfg='cfg block lists (sha256)', data='.data options', trainlist='training list')
     for k in [k for k in names if k in current]:
         if stored[k] != current[k]:
             if k == 'data':

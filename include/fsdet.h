@@ -238,6 +238,49 @@ int fsdet_bn_act_bwd_apply(const float* z, int ldz, const float* dy_full, int ld
                            void* dz_lo, int cpad, const float* amax, int B, int H, int W, int C, int has_bn,
                            void* stream);
 
+/* ---- segmented train-mode BatchNorm (per-replica statistics) -------------
+ * The batch is split into nseg contiguous segments of seg_pix pixels each
+ * (whole images: nseg * seg_pix == B*H*W, seg_pix a multiple of H*W), and each
+ * segment is normalised with its own batch statistics, as every replica of
+ * nn.DataParallel does.  Each pass is one launch for all segments; with one
+ * segment it computes exactly what the plain pass above computes.
+ * Vectors (mean, invstd, scale, shift, xhat_absmax) are [nseg][C]; coef is
+ * [nseg][2*C].
+ * fsdet_bn_seg_colstats: partial rows float [nseg][rows][4*C] with rows =
+ * fsdet_bn_seg_colstats_rows(seg_pix, nseg) (sum | sum of squares | min | max
+ * of strips that never straddle a segment; fixed reduction order), followed by
+ * nseg * fsdet_bn_stat_scratch_rows() rows of scratch for the finalize.
+ * fsdet_bn_seg_finalize (training only): per-segment statistics over seg_pix
+ * pixels; the running statistics are updated from segment 0 alone (unbiased
+ * variance over seg_pix); amax_y spans all segments.
+ * fsdet_bn_act_bwd_reduce_seg: partials double [nseg][fsdet_bn_seg_bwd_rows(B,
+ * H, W, nseg)][3*C] followed by nseg rows for fsdet_bn_bwd_finalize_seg, which
+ * writes the per-segment coefficients, dgamma / dbeta summed over the segments
+ * and one amax_bound over all of them. */
+int fsdet_bn_seg_colstats_rows(size_t seg_pix, int nseg);
+int fsdet_bn_seg_colstats(const float* z, int ld, size_t seg_pix, int nseg, int C, float* partial, void* stream);
+int fsdet_bn_seg_finalize(const float* stat_partial, int nparts, int nseg, size_t seg_pix, const float* gamma,
+                          const float* beta, float* running_mean, float* running_var, float momentum, float eps,
+                          float* mean, float* invstd, float* scale, float* shift, float slope, float* amax_y,
+                          float* xhat_absmax, int C, void* stream);
+int fsdet_bn_act_fwd_seg(const float* z, int ldz, const float* scale, const float* shift, float slope, float* y_full,
+                         int ld_full, float* y_pool, int ld_pool, void* full_hi, void* full_lo, void* pool_hi,
+                         void* pool_lo, int Cpad, const float* amax, int B, int H, int W, int C, int nseg,
+                         size_t seg_pix, void* stream);
+int fsdet_bn_seg_bwd_rows(int B, int H, int W, int nseg);
+int fsdet_bn_act_bwd_reduce_seg(const float* z, int ldz, const float* dy_full, int ld_dyf, const float* dy_pool,
+                                int ld_dyp, const float* scale, const float* shift, const float* mean,
+                                const float* invstd, float slope, double* partial, int B, int H, int W, int C,
+                                int nseg, size_t seg_pix, void* stream);
+int fsdet_bn_bwd_finalize_seg(const double* partial, int nparts, int nseg, size_t seg_pix, const float* gamma,
+                              const float* invstd, const float* xhat_absmax, float* dgamma, float* dbeta,
+                              double* coef, float* amax_bound, int C, void* stream);
+int fsdet_bn_act_bwd_apply_seg(const float* z, int ldz, const float* dy_full, int ld_dyf, const float* dy_pool,
+                               int ld_dyp, const float* scale, const float* shift, const float* mean,
+                               const float* invstd, const double* coef, float slope, float* dz, int lddz, void* dz_hi,
+                               void* dz_lo, int cpad, const float* amax, int B, int H, int W, int C, int nseg,
+                               size_t seg_pix, void* stream);
+
 /* ---- stand-alone pooling / reorg / route (darknet_meta.py:47-74,157-171) */
 /* size 2; stride 2 (floor) or stride 1 with replicate pad right/bottom
  * (MaxPoolStride1, darknet_meta.py:47-53) */

@@ -24,8 +24,16 @@ with the support set, batch sizes and thresholds of the evaluation command.  Opt
                                            schedule position, both `seen` counters, every rank's random streams (only the
                                            newest state file the run wrote is kept)
     --resume PATH.state                    continue from that state; `weightfile` must be its paired weight file.  Every
-                                           check (file, version, weight checksum, world, batch, cfg, .data, training list)
-                                           is made before any CUDA work
+                                           check (file, version, weight checksum, world, replicas, batch, cfg, .data,
+                                           training list) is made before any CUDA work
+
+Opt-in, the reference's own step on any number of GPUs (its configs train 4 nn.DataParallel replicas, `gpus=1,2,3,4`):
+
+    --replicas R                           R replicas per global step, R / world on each rank: BatchNorm statistics per
+                                           replica (batch / R query images, n_cls support images), R support sets per
+                                           step from the support index built for R GPUs, replica r's images reweighted
+                                           by replica r's vectors.  R must be a multiple of the world size and divide
+                                           the global batch.  Without it each rank is one replica.
 """
 import os
 import sys
@@ -113,6 +121,7 @@ def main():
     ap.add_argument('--eval-base-rw', default=None)
     ap.add_argument('--save-state', action='store_true')
     ap.add_argument('--resume', default=None)
+    ap.add_argument('--replicas', type=int, default=None)
     opts = ap.parse_args()
     scored = opts.eval_devkit is not None or opts.eval_coco_annotations is not None
     if len(opts.args) != 4 or (opts.eval_devkit is not None and opts.eval_coco_annotations is not None) or \
@@ -122,7 +131,7 @@ def main():
         print('Usage:')
         print('python tools/train_meta_b200.py datacfg darknetcfg learnetcfg weightfile '
               '[--eval-devkit DIR [--eval-year Y] | --eval-coco-annotations JSON] [--eval-base-rw PATH] '
-              '[--save-state] [--resume PATH.state]')
+              '[--save-state] [--resume PATH.state] [--replicas R]')
         return 1
     if opts.eval_base_rw is not None and not os.path.isfile(opts.eval_base_rw):
         print('--eval-base-rw: no such file: %s' % opts.eval_base_rw)
@@ -140,6 +149,9 @@ def main():
     world = int(os.environ.get('WORLD_SIZE', '1'))
     rank = int(os.environ.get('RANK', '0'))
     local = int(os.environ.get('LOCAL_RANK', '0'))
+    if opts.replicas is not None and (opts.replicas < 1 or opts.replicas % world):
+        print('--replicas %d: the replicas must be a positive multiple of the world size %d' % (opts.replicas, world))
+        return 1
     resume_state = None
     if opts.resume is not None:           # every check on the state file is made before any CUDA work
         try:
@@ -157,6 +169,10 @@ def main():
     cfg.config_net(net_options)
     batch_size = int(net_options['batch'])                      # GLOBAL batch, as in the reference
     per_rank = batch_size // world
+    replicas = world if opts.replicas is None else opts.replicas
+    if batch_size % replicas:
+        print('--replicas %d: the global batch %d does not split into %d replicas' % (replicas, batch_size, replicas))
+        return 1
     steps = [float(s) for s in net_options['steps'].split(',')]
     scales = [float(s) for s in net_options['scales'].split(',')]
     base_rw = None
@@ -164,7 +180,7 @@ def main():
         from fewshot_detection_b200 import valid as VA
         base_rw = VA.load_reweighting_vectors(opts.eval_base_rw, VA.reweighting_vector_shapes(learnetcfg, len(cfg.classes)))
     fingerprint = lambda trainlist=None: R.fingerprint(darknetcfg, learnetcfg, data_options, world, batch_size, per_rank,
-                                                       trainlist)
+                                                       trainlist, replicas)
     if resume_state is not None:
         try:
             R.check_fingerprint(resume_state, opts.resume, fingerprint())
@@ -193,7 +209,10 @@ def main():
     if world > 1:
         dist.init_process_group('nccl', device_id=torch.device('cuda', local))
 
-    model = Darknet(darknetcfg, learnetcfg)
+    model = Darknet(darknetcfg, learnetcfg, replicas=replicas // world)
+    if opts.replicas is not None and rank == 0:
+        logging('%d replicas per step, %d per rank on %d rank(s): %d query images and %d support images per replica'
+                % (replicas, replicas // world, world, batch_size // replicas, len(cfg.base_classes)))
     if os.path.exists(argv[4]):
         model.load_weights(argv[4])
     else:
@@ -222,10 +241,16 @@ def main():
                                 batch_size=per_rank, seen_step=world)
 
     def make_meta_batcher():
-        cfg.num_gpus = 1              # one process per GPU: each rank draws its own n_cls support images per step
+        if opts.replicas is None:
+            cfg.num_gpus = 1          # one process per GPU: each rank draws its own n_cls support images per step
+            metalines, inds = LS.support_index(data_options['meta'], classes, LS.support_batches_per_epoch(train=True),
+                                               shuffle=cfg.randmeta)
+            return MetaBatcher(metalines, inds, classes=classes, train=True)
+        cfg.num_gpus = replicas       # the reference's index for `replicas` GPUs; every rank takes its replicas' rows
         metalines, inds = LS.support_index(data_options['meta'], classes, LS.support_batches_per_epoch(train=True),
                                            shuffle=cfg.randmeta)
-        return MetaBatcher(metalines, inds, classes=classes, train=True)
+        inds = LS.rank_support_rows(inds, len(classes), replicas, world, rank)
+        return MetaBatcher(metalines, inds, classes=classes, train=True, replicas=replicas // world)
 
     evaluate = None
     if opts.eval_devkit is not None or opts.eval_coco_annotations is not None:
