@@ -37,12 +37,13 @@ def _models(side, seed):
     return m.cuda().train(), om
 
 
-def _batch(bs, cs, side, seed, max_gt=5):
+def _batch(bs, cs, side, seed, max_gt=5, replicas=1):
+    """bs query images, `replicas` support sets of cs images each (one per replica), labels for bs x cs rows"""
     from seeding import synth_targets, synth_masks
     g = torch.Generator().manual_seed(seed)
     x = torch.rand(bs, 3, side, side, generator=g)
-    metax = torch.rand(cs, 3, 416, 416, generator=g)
-    mask = torch.from_numpy(synth_masks(cs, 416, seed + 1))
+    metax = torch.rand(replicas * cs, 3, 416, 416, generator=g)
+    mask = torch.from_numpy(synth_masks(replicas * cs, 416, seed + 1))
     tgt = torch.from_numpy(synth_targets(bs, cs, seed + 2, max_gt=max_gt))
     return x, metax, mask, tgt
 

@@ -240,6 +240,10 @@ class StepChecker(object):
         flav = 'halo' if halo else ('im2col-long' if fold else 'im2col-short')
         self.cov.add(flav)
         self.cov.add(kind)
+        if kind == 'fwd':
+            # the epilogue with or without BatchNorm statistics rows: a replica step (and evaluation) runs every forward
+            # without them, its segmented BatchNorm pass reads z once more instead
+            self.cov.add('fwd-stats' if stat else 'fwd-nostats')
         if acc:
             self.cov.add('accumulate')
         self._record(kind, '%dx%dx%dx%d->%d k%d m%d%s' % (B, H, W, Cin, Cout, k, mode, ' acc' if acc else ''), flav, e, r)
@@ -442,19 +446,20 @@ class StepChecker(object):
         self.log.append(dict(kind=kind, shape=shape, flavour=flav, rel=e, ratio=r, extra=extra, full=full))
 
 
-def run_step(side, bs, cs, seed, wrap):
+def run_step(side, bs, cs, seed, wrap, replicas=1):
     """One eager step (forward, RegionLossV2, backward) of the full network with `bs` query images of side x side and
-    `cs` classes (support images at 416x416), while engine.call is replaced by wrap(engine.call).  Returns the head
+    `cs` classes (support images at 416x416), while engine.call is replaced by wrap(engine.call).  With replicas = R
+    the model is Darknet(..., replicas=R) and the support batch R * cs images (R support sets).  Returns the head
     output (detached), the region loss module, the label tensor and the seconds the step took."""
     from fewshot_detection_b200 import engine
     from test_gpu_zz_configs import _batch
     from fewshot_detection_b200 import netcfg
     from fewshot_detection_b200.darknet_meta import Darknet
     from seeding import seeded_init
-    m = Darknet(netcfg.darknet_dynamic_blocks(side, side), netcfg.reweighting_net_blocks())
+    m = Darknet(netcfg.darknet_dynamic_blocks(side, side), netcfg.reweighting_net_blocks(), replicas=replicas)
     seeded_init(m, seed)
     m = m.cuda().train()
-    x, metax, mask, tgt = _batch(bs, cs, side, seed + 1)
+    x, metax, mask, tgt = _batch(bs, cs, side, seed + 1, replicas=replicas)
     L = m.models[len(m.models) - 1]
     L.seen = 20000
     L.verbose = False

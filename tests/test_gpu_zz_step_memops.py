@@ -25,6 +25,14 @@ silently.
                            first-order propagation of the fp32 statistics' measured error and of the sums' bar;
                            planes bit-equal to
                            the split of fp32 dz; amax_bound >= max|dz|; conv + bias (has_bn = 0) dz bit-exact
+  segmented passes         (a replica step: [nseg][C] vectors, [nseg][2C] coefficients, segment k = images
+  (fsdet_*_seg)            [k B/nseg, (k+1) B/nseg)) the plain checks above applied per segment: colstats partial rows
+                           per segment (sums to 1e-5 of the absolute sums, minima and maxima exact); each segment's mean
+                           and invstd against float64 of that segment alone, running statistics from segment 0
+                           (unbiased over its pixels, and bit-unchanged when the other segments' rows change), one
+                           amax_y over all segments, max |mean|/std per segment reported; segment k's scale and shift on
+                           segment k's images; per-segment c1 / c2, dgamma / dbeta summed over segments, dz per segment
+                           including the from-scratch backward over the segment's statistics; one amax_bound >= max|dz|
   data movement            maxpool, reorg, copy_channels, layout conversions, pad_channels, weight_flip_transpose, amax,
                            split_f16, head_weff, globalmax (first maximum in pixel order): bit-exact
   head_param_grads / head_bias_grad   float64, within 1e-6 of the sum of absolute terms
@@ -37,7 +45,7 @@ import time
 import pytest
 import torch
 
-from test_gpu_zz_step_gemms import run_step, scale_from_amax
+from test_gpu_zz_step_gemms import check_stats, run_step, scale_from_amax
 
 pytestmark = pytest.mark.gpu
 
@@ -80,6 +88,17 @@ def act(p, B, H, W, C, ld):
 def chunks(B, H, W, C):
     step = max(1, CHUNK // max(1, H * W * C))
     return [(b, min(B, b + step)) for b in range(0, B, step)]
+
+
+def seg_chunks(B, H, W, C, nseg):
+    """[(segment, b0, b1)]: chunks() of each of nseg segments of B / nseg whole images, none straddling two"""
+    nb = B // nseg
+    return [(k, k * nb + b0, k * nb + b1) for k in range(nseg) for b0, b1 in chunks(nb, H, W, C)]
+
+
+def rows_of_segment(p, ld, seg_pix, k, C):
+    """[seg_pix][C] view of segment k's pixel rows of a buffer with leading dimension ld"""
+    return rows(p + 4 * k * seg_pix * ld, seg_pix, C, ld)
 
 
 def bits(t):
@@ -156,9 +175,12 @@ class MemChecker(object):
         self.unknown = []
         self.failures = []
         self.stat_src = {}      # stat pointer -> (z, ldz, B, H, W, C) of the convolution that filled it
+        self.seg_src = {}       # stat pointer -> (z, ld, seg_pix, nseg, C, rows) of the segmented colstats that filled it
+        self.seg_meanstd = {}   # segment -> worst |mean|/std of its layers (segmented passes only)
+        self.running_before = (None, None)
         self.amax_of = {}       # scale pointer -> amax_y pointer of the same finalize
         self.reduce = {}        # partial pointer -> arguments of the reduce pass
-        self.stats = {}         # (mean pointer) -> (mean64, var64) of z, for the from-scratch backward
+        self.stats = {}         # (mean pointer) -> [(mean64, var64)] of z per segment, for the from-scratch backward
         self.meanstd = []
         self.cancel = []
         self.bound_ratio = []
@@ -197,6 +219,11 @@ class MemChecker(object):
     # ---------------------------------------------------------------- finalize
     def chk_bn_finalize(self, fn, a):
         stat, nparts, count, gamma, beta, rm, rv, mom, eps, mean, invstd, scale, shift, slope, amax_y, xhat, C, training, st = a
+        if training:
+            zp, ldz, B, H, W, zc = self.stat_src[stat]
+            assert zc == C, (zc, C)
+            return self._finalize_train(fn, a, [act(zp, B, H, W, C, ldz)], gamma, beta, rm, rv, mom, eps, mean, invstd,
+                                        scale, shift, slope, amax_y, xhat, C)
         outs = [dev(p, C) for p in (mean, invstd, scale, shift, xhat) if p]
         for o in outs:
             o.fill_(float('nan'))
@@ -208,53 +235,121 @@ class MemChecker(object):
         g = dev(gamma, C).double() if gamma else torch.ones(C, dtype=torch.float64, device='cuda')
         b = dev(beta, C).double() if beta else torch.zeros(C, dtype=torch.float64, device='cuda')
         self.amax_of[scale] = amax_y
-        if not training:
-            return self._finalize_eval(fn, a, rc, m, inv, sc, sh, g, b, rm0, rv0)
-        zp, ldz, B, H, W, zc = self.stat_src[stat]
-        assert zc == C, (zc, C)
-        z = act(zp, B, H, W, C, ldz)
-        s = torch.zeros(C, dtype=torch.float64, device='cuda')
-        N = B * H * W
-        for b0, b1 in chunks(B, H, W, C):
-            s += z[b0:b1].double().sum((0, 1, 2))
-        mu = s / N
-        v = torch.zeros_like(s)
+        return self._finalize_eval(fn, a, rc, m, inv, sc, sh, g, b, rm0, rv0)
+
+    def chk_bn_seg_colstats(self, fn, a):
+        """partial rows of each segment against float64 of that segment alone (sums to 1e-5 of the absolute sums, minima
+        and maxima exact): a strip that straddled two segments moves both segments' minima or maxima"""
+        zp, ld, seg_pix, nseg, C, part, st = a
+        rows = self.lib.fsdet_bn_seg_colstats_rows(seg_pix, nseg)
+        S = dev(part, nseg * rows * 4 * C).view(nseg, rows, 4, C)
+        S.fill_(float('nan'))
+        rc = self.real(fn, *a)
+        torch.cuda.synchronize()
+        for k in range(nseg):
+            check_stats(self.expect, S[k], rows_of_segment(zp, ld, seg_pix, k, C), ('seg_colstats', seg_pix, nseg, C, k))
+        self.seg_src[part] = (zp, ld, seg_pix, nseg, C, rows)
+        self.cov.add('seg-colstats')
+        self._record('bn_seg_colstats', '%dx%dx%d' % (nseg, seg_pix, C), 'seg', 0.0)
+        return rc
+
+    def chk_bn_seg_finalize(self, fn, a):
+        stat, nparts, nseg, seg_pix, gamma, beta, rm, rv, mom, eps, mean, invstd, scale, shift, slope, amax_y, xhat, C, st = a
+        zp, ld, sp, ns, zc, rows = self.seg_src[stat]
+        assert (sp, ns, zc, rows) == (seg_pix, nseg, C, nparts), ((sp, ns, zc, rows), (seg_pix, nseg, C, nparts))
+        zs = [rows_of_segment(zp, ld, seg_pix, k, C).view(seg_pix, 1, 1, C) for k in range(nseg)]
+        rc = self._finalize_train(fn, a, zs, gamma, beta, rm, rv, mom, eps, mean, invstd, scale, shift, slope, amax_y, xhat, C)
+        if rm:
+            # the running statistics come from segment 0 alone: the same finalize with every other segment's partial rows
+            # doubled leaves them bit-unchanged (the reduction order is fixed, so a rerun is bit-reproducible)
+            rm1, rv1 = dev(rm, C).clone(), dev(rv, C).clone()
+            dev(rm, C).copy_(self.running_before[0])
+            dev(rv, C).copy_(self.running_before[1])
+            other = dev(stat, nseg * nparts * 4 * C)[nparts * 4 * C:]
+            keep = other.clone()
+            other.mul_(2.0)
+            probe = torch.full((5 * nseg * C + 1,), float('nan'), device='cuda')
+            P = lambda i: probe.data_ptr() + 4 * i * nseg * C
+            self.real(fn, stat, nparts, nseg, seg_pix, gamma, beta, rm, rv, mom, eps, P(0), P(1), P(2), P(3), slope,
+                      probe.data_ptr() + 4 * 5 * nseg * C, P(4), C, st)
+            torch.cuda.synchronize()
+            same = torch.equal(bits(dev(rm, C)), bits(rm1)) and torch.equal(bits(dev(rv, C)), bits(rv1))
+            moved = not torch.equal(bits(probe[nseg * C:2 * nseg * C]), bits(dev(invstd, nseg * C)))
+            self.expect(same and moved, ('seg_finalize: running statistics depend on segments 1..', C, same, moved))
+            other.copy_(keep)
+            dev(rm, C).copy_(rm1)
+            dev(rv, C).copy_(rv1)
+        self.cov.add('seg-finalize')
+        return rc
+
+    def _finalize_train(self, fn, a, zs, gamma, beta, rm, rv, mom, eps, mean, invstd, scale, shift, slope, amax_y, xhat, C):
+        """Train-mode finalize of len(zs) segments ([nseg][C] vectors, segment k normalised by the statistics of zs[k]):
+        each segment's mean / invstd against float64 of its own z, scale / shift within an ulp, xhat_absmax per segment,
+        running statistics from segment 0 (unbiased over its pixels), one amax_y over every segment."""
+        nseg = len(zs)
+        V = lambda p, k: dev(p + 4 * k * C, C)
+        for p in (mean, invstd, scale, shift, xhat):
+            if p:
+                dev(p, nseg * C).fill_(float('nan'))
+        rm0 = dev(rm, C).clone() if rm else None
+        rv0 = dev(rv, C).clone() if rv else None
+        self.running_before = (rm0, rv0)
+        rc = self.real(fn, *a)
+        torch.cuda.synchronize()
+        g = dev(gamma, C).double() if gamma else torch.ones(C, dtype=torch.float64, device='cuda')
+        b = dev(beta, C).double() if beta else torch.zeros(C, dtype=torch.float64, device='cuda')
+        self.amax_of[scale] = amax_y
         pos = torch.zeros(1, dtype=torch.float64, device='cuda')
         neg = torch.zeros(1, dtype=torch.float64, device='cuda')
-        xmax = torch.zeros(C, device='cuda')
-        for b0, b1 in chunks(B, H, W, C):
-            zz = z[b0:b1]
-            v += ((zz.double() - mu) ** 2).sum((0, 1, 2))
-            y32 = pre_act(zz, sc, sh)
-            u64 = zz.double() * sc.double() + sh.double()
-            pos = torch.maximum(pos, torch.where(y32 > 0, u64, 0.0).max())
-            neg = torch.maximum(neg, torch.where(y32 > 0, 0.0, -u64 * float(slope)).max())
-            xmax = torch.maximum(xmax, ((zz - m) * inv).abs().amax((0, 1, 2)))
-        var = v / N
-        std = torch.sqrt(var + eps)
-        rmean = ((m.double() - mu).abs() / (STAT_BAR * std)).max().item()
-        rinv = ((inv.double() - 1 / std).abs() * std / STAT_BAR).max().item()
-        ms = (mu.abs() / var.sqrt().clamp_min(1e-30)).max().item()
-        self.meanstd.append(ms)
-        self.expect(rmean <= 1 and rinv <= 1, ('bn_finalize mean / invstd', B, H, W, C, rmean, rinv, ms))
-        self.expect((ulps(sc, g * inv.double()) <= 1).all().item(), ('bn_finalize scale', C))
-        self.expect((ulps(sh, b - m.double() * sc.double()) <= 1).all().item(), ('bn_finalize shift', C))
+        stats = []
+        for k, z in enumerate(zs):
+            m, inv, sc, sh = V(mean, k), V(invstd, k), V(scale, k), V(shift, k)
+            B, H, W = z.shape[:3]
+            N = B * H * W
+            s = torch.zeros(C, dtype=torch.float64, device='cuda')
+            for b0, b1 in chunks(B, H, W, C):
+                s += z[b0:b1].double().sum((0, 1, 2))
+            mu = s / N
+            v = torch.zeros_like(s)
+            xmax = torch.zeros(C, device='cuda')
+            for b0, b1 in chunks(B, H, W, C):
+                zz = z[b0:b1]
+                v += ((zz.double() - mu) ** 2).sum((0, 1, 2))
+                y32 = pre_act(zz, sc, sh)
+                u64 = zz.double() * sc.double() + sh.double()
+                pos = torch.maximum(pos, torch.where(y32 > 0, u64, 0.0).max())
+                neg = torch.maximum(neg, torch.where(y32 > 0, 0.0, -u64 * float(slope)).max())
+                xmax = torch.maximum(xmax, ((zz - m) * inv).abs().amax((0, 1, 2)))
+            var = v / N
+            std = torch.sqrt(var + eps)
+            rmean = ((m.double() - mu).abs() / (STAT_BAR * std)).max().item()
+            rinv = ((inv.double() - 1 / std).abs() * std / STAT_BAR).max().item()
+            ms = (mu.abs() / var.sqrt().clamp_min(1e-30)).max().item()
+            self.meanstd.append(ms)
+            if nseg > 1:
+                self.seg_meanstd[k] = max(self.seg_meanstd.get(k, 0.0), ms)
+            self.expect(rmean <= 1 and rinv <= 1, ('bn_finalize mean / invstd', B, H, W, C, k, rmean, rinv, ms))
+            self.expect((ulps(sc, g * inv.double()) <= 1).all().item(), ('bn_finalize scale', C, k))
+            self.expect((ulps(sh, b - m.double() * sc.double()) <= 1).all().item(), ('bn_finalize shift', C, k))
+            if xhat:
+                self.expect(torch.equal(V(xhat, k), xmax), ('bn_finalize xhat_absmax', C, k))
+            if rm and k == 0:
+                want_m = (1 - mom) * rm0.double() + mom * m.double()
+                want_v = (1 - mom) * rv0.double() + mom * var * N / max(N - 1, 1)
+                self.expect(((dev(rm, C).double() - want_m).abs() <= 2.0 ** -22 * (want_m.abs() + m.double().abs())).all().item(),
+                            ('running mean', C))
+                self.expect(((dev(rv, C).double() - want_v).abs() <= 2 * STAT_BAR * mom * var * N / max(N - 1, 1) +
+                             2.0 ** -22 * want_v.abs()).all().item(), ('running var', C))
+            stats.append((mu, var))
+            shape = '%dx%dx%dx%d' % (B, H, W, C) if nseg == 1 else '%d/%dx%dx%d' % (k, nseg, N, C)
+            self._record('bn_finalize', shape, 'train' if nseg == 1 else 'train seg', max(rmean, rinv),
+                         '  |mean|/std %.2f' % ms)
         if amax_y:
             ref = torch.maximum(pos, neg)
             # the negative side is rounded twice (fma, then the slope)
             self.expect(ulps(dev(amax_y, 1), ref).item() <= (1 if pos.item() >= neg.item() else 2), ('bn_finalize amax_y', C))
-        if xhat:
-            self.expect(torch.equal(dev(xhat, C), xmax), ('bn_finalize xhat_absmax', C))
-        if rm:
-            want_m = (1 - mom) * rm0.double() + mom * m.double()
-            want_v = (1 - mom) * rv0.double() + mom * var * N / max(N - 1, 1)
-            self.expect(((dev(rm, C).double() - want_m).abs() <= 2.0 ** -22 * (want_m.abs() + m.double().abs())).all().item(),
-                        ('running mean', C))
-            self.expect(((dev(rv, C).double() - want_v).abs() <= 2 * STAT_BAR * mom * var * N / max(N - 1, 1) +
-                         2.0 ** -22 * want_v.abs()).all().item(), ('running var', C))
-        self.stats[mean] = (mu, var)
+        self.stats[mean] = stats
         self.cov.add('finalize-train')
-        self._record('bn_finalize', '%dx%dx%dx%d' % (B, H, W, C), 'train', max(rmean, rinv), '  |mean|/std %.2f' % ms)
         return rc
 
     def _finalize_eval(self, fn, a, rc, m, inv, sc, sh, g, b, rm0, rv0):
@@ -294,7 +389,16 @@ class MemChecker(object):
 
     # ----------------------------------------------------------------- forward
     def chk_bn_act_fwd(self, fn, a):
-        zp, ldz, scale, shift, slope, yf, ldf, yp, ldp, fh, fl, ph, pl, Cpad, amax, B, H, W, C, st = a
+        return self._act_fwd(fn, a, 1)
+
+    def chk_bn_act_fwd_seg(self, fn, a):
+        B, H, W, C, nseg, seg_pix = a[15:21]
+        assert seg_pix * nseg == B * H * W, (B, H, W, nseg, seg_pix)
+        return self._act_fwd(fn, a, nseg)
+
+    def _act_fwd(self, fn, a, nseg):
+        """the forward check, segment k's scale and shift ([nseg][C]) on segment k's images"""
+        zp, ldz, scale, shift, slope, yf, ldf, yp, ldp, fh, fl, ph, pl, Cpad, amax, B, H, W, C = a[:19]
         Hp, Wp = H // 2, W // 2
         M, Mp = B * H * W, B * Hp * Wp
         YF = act(yf, B, H, W, C, ldf) if yf else None
@@ -310,13 +414,13 @@ class MemChecker(object):
         rc = self.real(fn, *a)
         torch.cuda.synchronize()
         z = act(zp, B, H, W, C, ldz)
-        sc, sh = dev(scale, C), dev(shift, C)
         s = scale_from_amax(dev(amax, 1).item()) if amax else 1.0
         am = self.amax_of.get(scale)
         am = dev(am, 1).item() if am else None
         ok = True
         worst = 0.0
-        for b0, b1 in chunks(B, H, W, C):
+        for k, b0, b1 in seg_chunks(B, H, W, C, nseg):
+            sc, sh = dev(scale + 4 * k * C, C), dev(shift + 4 * k * C, C)
             zz = z[b0:b1]
             y32 = leaky(pre_act(zz, sc, sh), slope)
             u64 = zz.double() * sc.double() + sh.double()
@@ -336,35 +440,37 @@ class MemChecker(object):
                 ok &= not hi[b0:b1, ..., C:].any().item() and not lo[b0:b1, ..., C:].any().item()
             if am is not None:
                 ok &= y32.abs().max().item() <= am
-        self.expect(ok, ('bn_act_fwd', B, H, W, C, Cpad, bool(yf), bool(yp), bool(fh), bool(ph)))
-        self.expect(worst <= 1.0, ('bn_act_fwd: more than two roundings from float64', B, H, W, C, worst))
+        self.expect(ok, ('bn_act_fwd', B, H, W, C, Cpad, nseg, bool(yf), bool(yp), bool(fh), bool(ph)))
+        self.expect(worst <= 1.0, ('bn_act_fwd: more than two roundings from float64', B, H, W, C, nseg, worst))
         pool = bool(yp or ph)
         full = bool(yf or fh)
         flav = 'pool+full' if (pool and full) else ('pool' if pool else 'full')
-        self.cov.add('fwd-' + flav)
+        pre = 'seg-' if nseg > 1 else ''
+        self.cov.add(pre + 'fwd-' + flav)
         if yf or yp:
-            self.cov.add('fwd-f32')
+            self.cov.add(pre + 'fwd-f32')
         if fh or ph:
-            self.cov.add('fwd-planes')
+            self.cov.add(pre + 'fwd-planes')
         if pool and (H % 2 or W % 2):
-            self.cov.add('fwd-odd')
-        self._record('bn_act_fwd', '%dx%dx%dx%d pad%d' % (B, H, W, C, Cpad), flav + (' planes' if (fh or ph) else ''),
-                     worst, '' if ok else '  MISMATCH')
+            self.cov.add(pre + 'fwd-odd')
+        self._record('bn_act_fwd', '%dx%dx%dx%d pad%d' % (B, H, W, C, Cpad) + (' /%d' % nseg if nseg > 1 else ''),
+                     flav + (' planes' if (fh or ph) else '') + (' seg' if nseg > 1 else ''), worst, '' if ok else '  MISMATCH')
         return rc
 
     # ---------------------------------------------------------------- backward
-    def _du(self, r, b0, b1):
-        """float64 du, fp32 du, xhat (kernel statistics) and the fp32 pre-activation of images [b0, b1)"""
-        zp, ldz, dyf, ldf, dyp, ldp, scale, shift, mean, invstd, slope, B, H, W, C, has_bn = r
+    def _du(self, r, b0, b1, k=0):
+        """float64 du, fp32 du, xhat (segment k's kernel statistics) and the fp32 pre-activation of images [b0, b1)"""
+        zp, ldz, dyf, ldf, dyp, ldp, scale, shift, mean, invstd, slope, B, H, W, C, has_bn = r[:16]
         Hp, Wp = H // 2, W // 2
-        sc, sh = dev(scale, C), dev(shift, C)
+        V = lambda p: dev(p + 4 * k * C, C)
+        sc, sh = V(scale), V(shift)
         zz = act(zp, B, H, W, C, ldz)[b0:b1]
         y32 = pre_act(zz, sc, sh)
         a32 = leaky(y32, slope)
         gf = act(dyf, B, H, W, C, ldf)[b0:b1] if dyf else None
         gp = act(dyp, B, Hp, Wp, C, ldp)[b0:b1] if (dyp and Hp * Wp) else None
         du, d32 = route(y32, a32, gf, gp, slope)
-        xh = (zz.double() - dev(mean, C).double()) * dev(invstd, C).double() if has_bn else torch.zeros_like(du)
+        xh = (zz.double() - V(mean).double()) * V(invstd).double() if has_bn else torch.zeros_like(du)
         return du, d32, xh, zz
 
     def chk_bn_act_bwd_reduce(self, fn, a):
@@ -372,49 +478,87 @@ class MemChecker(object):
         nrows = self.lib.fsdet_bn_bwd_rows(B, H, W)
         dev(part, (nrows + 1) * 3 * C, torch.float64).fill_(float('nan'))
         rc = self.real(fn, *a)
-        self.reduce[part] = (zp, ldz, dyf, ldf, dyp, ldp, scale, shift, mean, invstd, slope, B, H, W, C, has_bn)
+        self.reduce[part] = (zp, ldz, dyf, ldf, dyp, ldp, scale, shift, mean, invstd, slope, B, H, W, C, has_bn, 1)
+        return rc
+
+    def chk_bn_act_bwd_reduce_seg(self, fn, a):
+        zp, ldz, dyf, ldf, dyp, ldp, scale, shift, mean, invstd, slope, part, B, H, W, C, nseg, seg_pix, st = a
+        assert seg_pix * nseg == B * H * W, (B, H, W, nseg, seg_pix)
+        nrows = self.lib.fsdet_bn_seg_bwd_rows(B, H, W, nseg)
+        dev(part, nseg * (nrows + 1) * 3 * C, torch.float64).fill_(float('nan'))
+        rc = self.real(fn, *a)
+        self.reduce[part] = (zp, ldz, dyf, ldf, dyp, ldp, scale, shift, mean, invstd, slope, B, H, W, C, 1, nseg)
         return rc
 
     def _sums(self, r):
+        """per segment: float64 sum du, sum du xhat, sum |du|, sum |du xhat| over the segment's images"""
         B, H, W, C = r[11:15]
-        acc = [torch.zeros(C, dtype=torch.float64, device='cuda') for _ in range(4)]
-        for b0, b1 in chunks(B, H, W, C):
-            du, _, xh, _ = self._du(r, b0, b1)
+        acc = [[torch.zeros(C, dtype=torch.float64, device='cuda') for _ in range(4)] for _ in range(r[16])]
+        for k, b0, b1 in seg_chunks(B, H, W, C, r[16]):
+            du, _, xh, _ = self._du(r, b0, b1, k)
             for i, t in enumerate((du, du * xh, du.abs(), (du * xh).abs())):
-                acc[i] += t.sum((0, 1, 2))
+                acc[k][i] += t.sum((0, 1, 2))
         return acc
 
     def chk_bn_bwd_finalize(self, fn, a):
         part, nrows, count, gamma, invstd, xabs, dgamma, dbeta, coef, amax, C, has_bn, st = a
-        for p, n, t in ((dgamma, C, torch.float32), (dbeta, C, torch.float32), (coef, 2 * C, torch.float64)):
+        return self._bwd_finalize(fn, a, part, dgamma, dbeta, coef, C, has_bn)
+
+    def chk_bn_bwd_finalize_seg(self, fn, a):
+        part, nrows, nseg, seg_pix, gamma, invstd, xabs, dgamma, dbeta, coef, amax, C, st = a
+        assert self.reduce[part][16] == nseg, (self.reduce[part][16], nseg)
+        return self._bwd_finalize(fn, a, part, dgamma, dbeta, coef, C, 1)
+
+    def _bwd_finalize(self, fn, a, part, dgamma, dbeta, coef, C, has_bn):
+        """per segment k: c1 = sum du / N_k and c2 = sum du xhat / N_k within 1e-6 of the segment's absolute sums;
+        dgamma, dbeta: the sums over every segment, within 1e-6 of the absolute sums over every segment"""
+        r = self.reduce[part]
+        nseg = r[16]
+        for p, n, t in ((dgamma, C, torch.float32), (dbeta, C, torch.float32), (coef, 2 * C * nseg, torch.float64)):
             if p:
                 dev(p, n, t).fill_(float('nan'))
         rc = self.real(fn, *a)
         torch.cuda.synchronize()
-        r = self.reduce[part]
         B, H, W = r[11:14]
-        N = B * H * W
-        s1, s2, a1, a2 = self._sums(r)
+        N = B * H * W // nseg
+        acc = self._sums(r)
+        s1, s2, a1, a2 = (sum(acc[k][i] for k in range(nseg)) for i in range(4))
         worst = 0.0
         if dbeta:
             e = ((dev(dbeta, C).double() - s1).abs() / (SUM_BAR * a1).clamp_min(1e-300)).max().item()
             worst = max(worst, e)
         if has_bn:
             e2 = ((dev(dgamma, C).double() - s2).abs() / (SUM_BAR * a2).clamp_min(1e-300)).max().item() if dgamma else 0.0
-            cf = dev(coef, 2 * C, torch.float64)
-            e3 = ((cf[:C] - s1 / N).abs() / (SUM_BAR * a1 / N).clamp_min(1e-300)).max().item()
-            e4 = ((cf[C:] - s2 / N).abs() / (SUM_BAR * a2 / N).clamp_min(1e-300)).max().item()
-            worst = max(worst, e2, e3, e4)
+            worst = max(worst, e2)
+            for k in range(nseg):
+                k1, k2, b1, b2 = acc[k]
+                cf = dev(coef + 8 * 2 * C * k, 2 * C, torch.float64)
+                e3 = ((cf[:C] - k1 / N).abs() / (SUM_BAR * b1 / N).clamp_min(1e-300)).max().item()
+                e4 = ((cf[C:] - k2 / N).abs() / (SUM_BAR * b2 / N).clamp_min(1e-300)).max().item()
+                worst = max(worst, e3, e4)
         cancel = (a1 / s1.abs().clamp_min(1e-300)).max().item()
         self.cancel.append(cancel)
-        self.expect(worst <= 1.0, ('bn_bwd_finalize sums', B, H, W, C, has_bn, worst))
-        self._record('bn_bwd_finalize', '%dx%dx%dx%d' % (B, H, W, C), 'bn' if has_bn else 'bias', worst,
-                     '  cancellation %.0f' % cancel)
+        self.expect(worst <= 1.0, ('bn_bwd_finalize sums', B, H, W, C, has_bn, nseg, worst))
+        if nseg > 1:
+            self.cov.add('seg-bwd-finalize')
+        self._record('bn_bwd_finalize', '%dx%dx%dx%d' % (B, H, W, C) + (' /%d' % nseg if nseg > 1 else ''),
+                     ('bn' if has_bn else 'bias') + (' seg' if nseg > 1 else ''), worst, '  cancellation %.0f' % cancel)
         return rc
 
     def chk_bn_act_bwd_apply(self, fn, a):
-        (zp, ldz, dyf, ldf, dyp, ldp, scale, shift, mean, invstd, coef, slope, dzp, lddz, dh, dl, cpad, amax, B, H, W, C,
-         has_bn, st) = a
+        return self._bwd_apply(fn, a, a[22], 1)
+
+    def chk_bn_act_bwd_apply_seg(self, fn, a):
+        B, H, W, C, nseg, seg_pix = a[18:24]
+        assert seg_pix * nseg == B * H * W, (B, H, W, nseg, seg_pix)
+        return self._bwd_apply(fn, a, 1, nseg)
+
+    def _bwd_apply(self, fn, a, has_bn, nseg):
+        """the apply check, segment k's vectors ([nseg][C]) and coefficients ([nseg][2C]) on segment k's images and the
+        from-scratch float64 backward over segment k's statistics; one amax_bound over every segment"""
+        zp, ldz, dyf, ldf, dyp, ldp, scale, shift, mean, invstd, coef, slope, dzp, lddz, dh, dl, cpad, amax, B, H, W, C = a[:22]
+        tail = a[22:-1]         # (has_bn,) or (nseg, seg_pix)
+        st = a[-1]
         M = B * H * W
         DZ = act(dzp, B, H, W, C, lddz) if dzp else None
         DH, DL = [dev(p, M * C, torch.int16).view(B, H, W, C) if p else None for p in (dh, dl)]
@@ -428,51 +572,56 @@ class MemChecker(object):
         if DZ is None:      # planes only: the fp32 dz they were split from (the apply pass only reads its inputs)
             tmp = torch.full((M, C), float('nan'), device='cuda')
             self.real(fn, zp, ldz, dyf, ldf, dyp, ldp, scale, shift, mean, invstd, coef, slope, tmp.data_ptr(), C, None,
-                      None, cpad, amax, B, H, W, C, has_bn, st)
+                      None, cpad, amax, B, H, W, C, *tail, st)
             torch.cuda.synchronize()
             DZ = tmp.view(B, H, W, C)
-        r = (zp, ldz, dyf, ldf, dyp, ldp, scale, shift, mean, invstd, slope, B, H, W, C, has_bn)
-        sc = dev(scale, C).double()
+        r = (zp, ldz, dyf, ldf, dyp, ldp, scale, shift, mean, invstd, slope, B, H, W, C, has_bn, nseg)
+        Ms = M // nseg
         ok = True
         worst = scratch = 0.0
         dzmax = 0.0
+        prop = 0.0
+        seg = []
         if has_bn:
-            cf = dev(coef, 2 * C, torch.float64)
-            c1, c2 = cf[:C], cf[C:]
-            mu, var = self.stats[mean]
-            g = sc / dev(invstd, C).double()
-            # from scratch: float64 statistics of z, float64 xhat, the float64 sums
-            acc = [torch.zeros(C, dtype=torch.float64, device='cuda') for _ in range(4)]
-            for b0, b1 in chunks(B, H, W, C):
-                du, _, _, zz = self._du(r, b0, b1)
+            # from scratch, per segment: float64 statistics of the segment's z, float64 xhat, the float64 sums
+            acc = [[torch.zeros(C, dtype=torch.float64, device='cuda') for _ in range(4)] for _ in range(nseg)]
+            for k, b0, b1 in seg_chunks(B, H, W, C, nseg):
+                mu, var = self.stats[mean][k]
+                du, _, _, zz = self._du(r, b0, b1, k)
                 xs = (zz.double() - mu) / torch.sqrt(var + EPS)
                 for i, t in enumerate((du, du * xs, du.abs(), (du * xs).abs())):
-                    acc[i] += t.sum((0, 1, 2))
-            c1s, c2s = acc[0] / M, acc[1] / M
-            # the kernel's fp32 statistics differ from float64 (within the finalize bars): to first order, a mean error
-            # kappa = (mu - mean) * invstd and an invstd error delta move dz by
-            # |scale| (|delta| |dz| + 2 |delta| |xhat c2| + |kappa| (|c2| + |xhat c1|)); and c1, c2 are exact only to the
-            # backward sums' bar (1e-6 of sum|du| / N and sum|du xhat| / N: c2 cancels, and its products are fp32), which
-            # moves dz by |scale| 1e-6 (sum|du| + |xhat| sum|du xhat|) / N.  That propagation is allowed on top.
-            e1, e2 = SUM_BAR * acc[2] / M, SUM_BAR * acc[3] / M
-            kappa = ((mu - dev(mean, C).double()) * dev(invstd, C).double()).abs()
-            delta = (dev(invstd, C).double() * torch.sqrt(var + EPS) - 1).abs()
-            prop = 0.0
+                    acc[k][i] += t.sum((0, 1, 2))
+            for k in range(nseg):
+                V = lambda p: dev(p + 4 * k * C, C).double()
+                mu, var = self.stats[mean][k]
+                cf = dev(coef + 8 * 2 * C * k, 2 * C, torch.float64)
+                # the kernel's fp32 statistics differ from float64 (within the finalize bars): to first order, a mean
+                # error kappa = (mu - mean) * invstd and an invstd error delta move dz by
+                # |scale| (|delta| |dz| + 2 |delta| |xhat c2| + |kappa| (|c2| + |xhat c1|)); and c1, c2 are exact only to
+                # the backward sums' bar (1e-6 of sum|du| / N and sum|du xhat| / N: c2 cancels, and its products are
+                # fp32), which moves dz by |scale| 1e-6 (sum|du| + |xhat| sum|du xhat|) / N.  That propagation is
+                # allowed on top.
+                seg.append(dict(sc=V(scale), c1=cf[:C], c2=cf[C:], mu=mu, var=var, g=V(scale) / V(invstd),
+                                c1s=acc[k][0] / Ms, c2s=acc[k][1] / Ms, e1=SUM_BAR * acc[k][2] / Ms,
+                                e2=SUM_BAR * acc[k][3] / Ms, kappa=((mu - V(mean)) * V(invstd)).abs(),
+                                delta=(V(invstd) * torch.sqrt(var + EPS) - 1).abs()))
         s = scale_from_amax(dev(amax, 1).item()) if amax else 1.0
-        for b0, b1 in chunks(B, H, W, C):
-            du, d32, xh, zz = self._du(r, b0, b1)
+        for k, b0, b1 in seg_chunks(B, H, W, C, nseg):
+            du, d32, xh, zz = self._du(r, b0, b1, k)
             got = DZ[b0:b1]
             ok &= not torch.isnan(got).any().item()
             dzmax = max(dzmax, got.abs().max().item())
             if has_bn:
+                q = seg[k]
+                sc, c1, c2, c1s, c2s = q['sc'], q['c1'], q['c2'], q['c1s'], q['c2s']
                 ref = sc * (du - c1 - xh * c2)
                 bar = sc.abs() * (du.abs() + c1.abs() + (xh * c2).abs())
                 d = (got.double() - ref).abs()
                 worst = max(worst, torch.where(d == 0, 0.0, d / (SUM_BAR * bar)).max().item())
-                xs = (zz.double() - mu) / torch.sqrt(var + EPS)
-                ref_s = g / torch.sqrt(var + EPS) * (du - c1s - xs * c2s)
-                p = 1.1 * sc.abs() * (delta * ref_s.abs() / sc.abs() + 2 * delta * (xs * c2s).abs() +
-                                      kappa * (c2s.abs() + (xs * c1s).abs()) + e1 + xs.abs() * e2)
+                xs = (zz.double() - q['mu']) / torch.sqrt(q['var'] + EPS)
+                ref_s = q['g'] / torch.sqrt(q['var'] + EPS) * (du - c1s - xs * c2s)
+                p = 1.1 * sc.abs() * (q['delta'] * ref_s.abs() / sc.abs() + 2 * q['delta'] * (xs * c2s).abs() +
+                                      q['kappa'] * (c2s.abs() + (xs * c1s).abs()) + q['e1'] + xs.abs() * q['e2'])
                 prop = max(prop, (p / bar).max().item())
                 d = (got.double() - ref_s).abs()
                 rr = torch.where(d == 0, 0.0, d / (SCRATCH_BAR * bar + p))
@@ -481,8 +630,9 @@ class MemChecker(object):
                     i = rr.flatten().argmax().item()
                     at = lambda t: t.expand(rr.shape).flatten()[i].item()
                     c = i % C
-                    worst_at = dict(du=at(du), c1=c1s[c].item(), xs=at(xs), c2=c2s[c].item(), kappa=kappa[c].item(),
-                                    delta=delta[c].item(), got=at(got), ref=at(ref), ref_s=at(ref_s), bar=at(bar), p=at(p))
+                    worst_at = dict(segment=k, du=at(du), c1=c1s[c].item(), xs=at(xs), c2=c2s[c].item(),
+                                    kappa=q['kappa'][c].item(), delta=q['delta'][c].item(), got=at(got), ref=at(ref),
+                                    ref_s=at(ref_s), bar=at(bar), p=at(p))
             else:
                 ok &= torch.equal(bits(got), bits(d32))
                 d = (got.double() - du).abs()
@@ -494,22 +644,27 @@ class MemChecker(object):
         extra = ''
         if amax and has_bn:
             bound = dev(amax, 1).item()
-            self.expect(bound > dzmax, ('amax_bound below max|dz|', B, H, W, C, bound, dzmax))
+            self.expect(bound > dzmax, ('amax_bound below max|dz|', B, H, W, C, nseg, bound, dzmax))
             self.bound_ratio.append(bound / max(dzmax, 1e-300))
             extra = '  bound/max|dz| %.2f  statistics propagation %.1e of the bound' % (bound / max(dzmax, 1e-300), prop)
-        self.expect(ok, ('bn_act_bwd_apply', B, H, W, C, has_bn, bool(dzp), bool(dh)))
+        self.expect(ok, ('bn_act_bwd_apply', B, H, W, C, has_bn, nseg, bool(dzp), bool(dh)))
         if has_bn and scratch > 1.0:
-            mu2 = sum(act(zp, B, H, W, C, ldz)[b0:b1].double().sum((0, 1, 2)) for b0, b1 in chunks(B, H, W, C)) / M
-            print('  scratch worst element:', worst_at, ' z changed since the forward:', not torch.equal(mu2, mu))
-        self.expect(worst <= 1.0 and scratch <= 1.0, ('bn_act_bwd_apply dz', B, H, W, C, has_bn, worst, scratch))
+            k = worst_at['segment']
+            nb = B // nseg
+            z = act(zp, B, H, W, C, ldz)[k * nb:(k + 1) * nb]
+            mu2 = sum(z[b0:b1].double().sum((0, 1, 2)) for b0, b1 in chunks(nb, H, W, C)) / Ms
+            print('  scratch worst element:', worst_at, ' z changed since the forward:', not torch.equal(mu2, seg[k]['mu']))
+        self.expect(worst <= 1.0 and scratch <= 1.0, ('bn_act_bwd_apply dz', B, H, W, C, has_bn, nseg, worst, scratch))
         pool_only = not dyf and dyp and has_bn and 0.0 <= slope <= 1.0
         flav = 'pool-only' if pool_only else ('general ' + '+'.join(n for n, p in (('full', dyf), ('pool', dyp)) if p))
-        self.cov.add('bwd-' + flav.replace(' ', '-'))
+        pre = 'seg-' if nseg > 1 else ''
+        self.cov.add(pre + 'bwd-' + flav.replace(' ', '-'))
         if not has_bn:
             self.cov.add('bwd-bias')
         if (H % 2 or W % 2) and dyp:
-            self.cov.add('bwd-odd')
-        self._record('bn_act_bwd_apply', '%dx%dx%dx%d' % (B, H, W, C), flav + ('' if has_bn else ' bias'), max(worst, scratch),
+            self.cov.add(pre + 'bwd-odd')
+        self._record('bn_act_bwd_apply', '%dx%dx%dx%d' % (B, H, W, C) + (' /%d' % nseg if nseg > 1 else ''),
+                     flav + ('' if has_bn else ' bias') + (' seg' if nseg > 1 else ''), max(worst, scratch),
                      '  scratch %.3f%s%s' % (scratch, extra, '' if ok else '  MISMATCH'))
         return rc
 
@@ -779,6 +934,8 @@ def report(chk, secs):
     if chk.meanstd:         # a training step (an evaluation pass has no batch statistics and no backward)
         print('worst |mean|/std %.2f, worst cancellation sum|du|/|sum du| %.0f, amax_bound / max|dz| in [%.2f, %.2f]' % (
             max(chk.meanstd), max(chk.cancel), min(chk.bound_ratio), max(chk.bound_ratio)))
+    if chk.seg_meanstd:
+        print('worst |mean|/std per segment:', ', '.join('%d: %.2f' % kv for kv in sorted(chk.seg_meanstd.items())))
     print('coverage:', sorted(chk.cov))
     assert not chk.failures, chk.failures
     return chk

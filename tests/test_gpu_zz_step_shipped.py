@@ -47,11 +47,11 @@ SLEEP_CYCLES = 20000000
 
 
 # ------------------------------------------------------------------------------------------------------------ runner
-def _model(side, seed):
+def _model(side, seed, replicas=1):
     from fewshot_detection_b200 import netcfg
     from fewshot_detection_b200.darknet_meta import Darknet
     from seeding import seeded_init
-    m = Darknet(netcfg.darknet_dynamic_blocks(side, side), netcfg.reweighting_net_blocks())
+    m = Darknet(netcfg.darknet_dynamic_blocks(side, side), netcfg.reweighting_net_blocks(), replicas=replicas)
     seeded_init(m, seed)
     m = m.cuda().train()
     L = m.models[len(m.models) - 1]
@@ -69,19 +69,20 @@ class Run(object):
     gradient and BatchNorm running statistic by name (copied to the host) and the wall time."""
 
 
-def run(side, bs, cs, seed, batch_seeds, wrap=None):
+def run(side, bs, cs, seed, batch_seeds, wrap=None, replicas=1):
     """The seeded full model (configs side x side, `cs` classes, B = `bs`), then forward + RegionLossV2 + backward on
-    each batch of `batch_seeds` without zeroing the gradients in between, while engine.call is wrap(engine.call)."""
+    each batch of `batch_seeds` without zeroing the gradients in between, while engine.call is wrap(engine.call).
+    replicas = R: the R-replica step (Darknet(..., replicas=R), R support sets of `cs` images)."""
     from fewshot_detection_b200 import engine
     from test_gpu_zz_configs import _batch
-    m, L = _model(side, seed)
+    m, L = _model(side, seed, replicas)
     real = engine.call
     if wrap is not None:
         engine.call = wrap(real)
     t0 = time.time()
     try:
         for bseed in batch_seeds:
-            x, metax, mask, tgt = _batch(bs, cs, side, bseed)
+            x, metax, mask, tgt = _batch(bs, cs, side, bseed, replicas=replicas)
             out = m(x.cuda(), metax.cuda(), mask.cuda())
             loss = L(out, tgt)
             loss.backward()
@@ -495,12 +496,12 @@ class LifetimeAudit(object):
         return [(what, self.t0.elapsed_time(end) - self.t0.elapsed_time(done)) for what, done, end in self.windows]
 
 
-def audited_run(batch_seeds, monkeypatch, forget_keep=False):
+def audited_run(batch_seeds, monkeypatch, forget_keep=False, replicas=1):
     from fewshot_detection_b200 import engine
     audit = LifetimeAudit(forget_keep)
     monkeypatch.setattr(engine.NetRunner, '_convbn_bwd', lambda runner, rec, st: audit.convbn(runner, rec, st))
     try:
-        r = run(416, 64, 20, SEED, batch_seeds, audit.wrap)
+        r = run(416, 64, 20, SEED, batch_seeds, audit.wrap, replicas)
     finally:
         monkeypatch.setattr(engine.NetRunner, '_convbn_bwd', audit.real_convbn)
     margins = audit.margins()
