@@ -94,6 +94,12 @@ SIGNATURES = {
     'fsdet_eval_merge_workspace_bytes': ('ii', 'z'),
     'fsdet_voc_merge': ('ipppqpqipzppqpipp', 'i'),
     'fsdet_coco_merge': ('ipppqpqipzppqpipp', 'i'),
+    'fsdet_tta_merge': ('ppiiiiiippipp', 'i'),
+    'fsdet_nms_merged_workspace_bytes': ('ii', 'z'),
+    'fsdet_nms_merged': ('ppiidpzppp', 'i'),
+    'fsdet_detect_select_merged': ('pppiiipipzpppppp', 'i'),
+    'fsdet_voc_gather_merged': ('pppiiippppqpipp', 'i'),
+    'fsdet_coco_gather_merged': ('pppiiippippqpipp', 'i'),
     'fsdet_augment_workspace_bytes':('iiii', 'z'),
     'fsdet_augment_batch': ('pppiiiiipzpppp', 'i'),
     'fsdet_box_masks': ('piiipp', 'i'),

@@ -338,6 +338,12 @@ class DeviceCocoEval(DetectionPool):
         return min(cap, self.max_det)
 
     def _gather(self, dets, cap, image_index, image_size):
+        if eval_pool._is_merged(dets):
+            eval_pool._call('fsdet_coco_gather_merged', _ptr(dets.merged), _ptr(dets.keep), _ptr(dets.keep_count),
+                            dets.N, cap, len(self.classes), _ptr(image_index), _ptr(image_size), self.max_det,
+                            _ptr(self.key), _ptr(self.box), self.pool_cap, _ptr(self.groups), self.group_cap,
+                            _ptr(self.counters), eval_pool._stream())
+            return
         eval_pool._call('fsdet_coco_gather', _ptr(dets.cand), _ptr(dets.keep), _ptr(dets.keep_count), dets.N, cap,
                         dets.H, dets.W, dets.nC, len(self.classes), _ptr(image_index), _ptr(image_size), self.max_det,
                         _ptr(self.key), _ptr(self.box), self.pool_cap, _ptr(self.groups), self.group_cap,

@@ -18,6 +18,7 @@
 //   4. Accumulate: one block per (class, area, maxDets) scans the class's ranked records for the 10 thresholds at once.
 //      A record contributes (rc, pr) = (tp / npig, tp / (tp + fp + eps)) at its TP or FP; the precision at recall
 //      threshold r is the largest pr with rc >= recThrs[r], or 0: pycocotools' envelope read at searchsorted(rc, r).
+#include "detect_records.cuh"
 #include "eval_sort.cuh"
 
 namespace fsdet {
@@ -37,19 +38,21 @@ struct CocoParams {
 // ---- gather: one batch of Detections (after NMS) -> records + group descriptors ---------------------------------
 // eval_gather_plan_kernel (eval_sort.cuh) lays out the batch's groups and counters, each row cut to max_det records;
 // coco_gather_rows_kernel fills the records.
-__device__ __forceinline__ double coco_score(const float* __restrict__ cand, const int32_t* __restrict__ keep, int r,
-                                             int cap, int j) {
-    const float* v = cand + ((size_t)r * cap + keep[(size_t)r * cap + j]) * 8;
-    return __dmul_rn((double)v[4], (double)v[5]);
+template <class Rows>
+__device__ __forceinline__ double coco_score(const Rows& rows, const int32_t* __restrict__ keep, int r, int cap, int j) {
+    const size_t id = (size_t)r * cap + keep[(size_t)r * cap + j];
+    return __dmul_rn((double)rows.det(id), (double)rows.cls(id));
 }
 
 // One block per row: survivor t goes to rank (# survivors with a higher score, or an equal one earlier), kept if the
 // rank is below max_det.  Box as coco_eval.detection_records computes it: box = [xs/W, ys/H, ws/W, hs/H] (float64 of
 // the float32 candidate), x1 = (box[0] - box[2]/2.0) * width, x2 = (box[0] + box[2]/2.0) * width, w = x2 - x1.
-__global__ void __launch_bounds__(kVocThreads) coco_gather_rows_kernel(const float* __restrict__ cand,
+// Rows: a reader of detect_records.cuh (the candidates of one pass, or the merged records of several).
+template <class Rows>
+__global__ void __launch_bounds__(kVocThreads) coco_gather_rows_kernel(const Rows rows,
                                                                        const int32_t* __restrict__ keep,
                                                                        const int32_t* __restrict__ keep_count, int cap,
-                                                                       int H, int W, int n_cls, int max_det,
+                                                                       int n_cls, int max_det,
                                                                        const double* __restrict__ image_size,
                                                                        const int32_t* __restrict__ groups,
                                                                        const long long* __restrict__ counters,
@@ -61,16 +64,15 @@ __global__ void __launch_bounds__(kVocThreads) coco_gather_rows_kernel(const flo
     const int count = max(keep_count[r], 0);
     const double width = image_size[(r / n_cls) * 2], height = image_size[(r / n_cls) * 2 + 1];
     for (int t = threadIdx.x; t < count; t += kVocThreads) {
-        const double s = coco_score(cand, keep, r, cap, t);
+        const double s = coco_score(rows, keep, r, cap, t);
         int rank = 0;
         for (int j = 0; j < count && rank < max_det; ++j) {
-            const double o = coco_score(cand, keep, r, cap, j);
+            const double o = coco_score(rows, keep, r, cap, j);
             rank += (o > s || (o == s && j < t)) ? 1 : 0;
         }
         if (rank >= max_det) continue;
-        const float* v = cand + ((size_t)r * cap + keep[(size_t)r * cap + t]) * 8;
-        const double bx = __ddiv_rn((double)v[0], (double)W), by = __ddiv_rn((double)v[1], (double)H);
-        const double bw = __ddiv_rn((double)v[2], (double)W), bh = __ddiv_rn((double)v[3], (double)H);
+        const double4 b = rows.box((size_t)r * cap + keep[(size_t)r * cap + t]);
+        const double bx = b.x, by = b.y, bw = b.z, bh = b.w;
         const double hw = __ddiv_rn(bw, 2.0), hh = __ddiv_rn(bh, 2.0);
         const double x1 = __dmul_rn(__dsub_rn(bx, hw), width), y1 = __dmul_rn(__dsub_rn(by, hh), height);
         const double x2 = __dmul_rn(__dadd_rn(bx, hw), width), y2 = __dmul_rn(__dadd_rn(by, hh), height);
@@ -375,15 +377,16 @@ static CocoWorkspace coco_workspace_layout(void* base, int n_det, int n_gt, int 
     return w;
 }
 
-static int coco_gather_impl(const float* cand, const int32_t* keep, const int32_t* keep_count, int N, int cap, int H,
-                            int W, int n_cls, const int32_t* image_index, const double* image_size, int max_det,
-                            double* score, double* box, long long pool_cap, int32_t* groups, int group_cap,
-                            long long* counters, cudaStream_t st) {
+template <class Rows>
+static int coco_gather_impl(const Rows& rows, const int32_t* keep, const int32_t* keep_count, int N, int cap, int n_cls,
+                            const int32_t* image_index, const double* image_size, int max_det, double* score,
+                            double* box, long long pool_cap, int32_t* groups, int group_cap, long long* counters,
+                            cudaStream_t st) {
     (void)st;
     VOC_LAUNCH(1, kVocThreads, eval_gather_plan_kernel, keep_count, N, n_cls, image_index, max_det, pool_cap, groups,
                group_cap, counters);
     VOC_CHECK("coco_gather_plan");
-    VOC_LAUNCH(N, kVocThreads, coco_gather_rows_kernel, cand, keep, keep_count, cap, H, W, n_cls, max_det, image_size,
+    VOC_LAUNCH(N, kVocThreads, coco_gather_rows_kernel<Rows>, rows, keep, keep_count, cap, n_cls, max_det, image_size,
                groups, counters, score, box);
     VOC_CHECK("coco_gather_rows");
     return 0;
@@ -476,8 +479,25 @@ extern "C" int fsdet_coco_gather(const float* cand, const int32_t* keep, const i
     FSDET_CHECK_ARG(cap > 0 && H > 0 && W > 0 && pool_cap >= 0 && pool_cap <= 0x7fffffffll && group_cap >= 0,
                     "coco_gather: bad shape");
     if (N == 0) return 0;
-    return coco_gather_impl(cand, keep, keep_count, N, cap, H, W, n_cls, image_index, image_size, max_det, score, box,
-                            pool_cap, groups, group_cap, counters, (cudaStream_t)stream);
+    return coco_gather_impl(CandRows{cand, H, W}, keep, keep_count, N, cap, n_cls, image_index, image_size, max_det,
+                            score, box, pool_cap, groups, group_cap, counters, (cudaStream_t)stream);
+}
+
+extern "C" int fsdet_coco_gather_merged(const void* merged, const int32_t* keep, const int32_t* keep_count, int N,
+                                        int cap, int n_cls, const int32_t* image_index, const double* image_size,
+                                        int max_det, double* score, double* box, long long pool_cap, int32_t* groups,
+                                        int group_cap, long long* counters, void* stream) {
+    FSDET_CHECK_ARG(merged && keep && keep_count && image_index && image_size && score && box && groups && counters,
+                    "coco_gather_merged: null pointer");
+    FSDET_CHECK_ARG(n_cls > 0 && n_cls < kCocoMaxClasses && N >= 0 && N % n_cls == 0,
+                    "coco_gather_merged: %d rows are not images x %d classes (1..%d)", N, n_cls, kCocoMaxClasses - 1);
+    FSDET_CHECK_ARG(max_det > 0 && max_det <= 255, "coco_gather_merged: max_det %d outside 1..255", max_det);
+    FSDET_CHECK_ARG(cap > 0 && pool_cap >= 0 && pool_cap <= 0x7fffffffll && group_cap >= 0,
+                    "coco_gather_merged: bad shape");
+    if (N == 0) return 0;
+    return coco_gather_impl(MergedRows{static_cast<const TtaRecord*>(merged)}, keep, keep_count, N, cap, n_cls,
+                            image_index, image_size, max_det, score, box, pool_cap, groups, group_cap, counters,
+                            (cudaStream_t)stream);
 }
 
 extern "C" int fsdet_coco_merge(int n_src, const long long* src_counters, const double* src_score, const double* src_box,

@@ -11,6 +11,7 @@
 // `det_conf * cls_conf > conf_thresh`, the normalisation x/w, the NMS key float32(1 - det_conf) and the NMS IoUs
 // (utils.bbox_iou, utils.py:21-52, operation order kept, no FMA contraction).
 #include "common.cuh"
+#include "detect_records.cuh"
 #include "eval_sort.cuh"
 
 // tools/host_emul compiles this file with g++ (threads = OS threads) to test the block-level logic without a GPU
@@ -311,12 +312,16 @@ __global__ void __launch_bounds__(kDetThreads) select_compact_kernel(const int32
 }
 
 // valid.detection_lines' prob = det_conf * cls_conf, float64 (exact: a product of two float32 values)
-__device__ __forceinline__ double select_prob(const float* c) { return __dmul_rn((double)c[4], (double)c[5]); }
+template <class Rows>
+__device__ __forceinline__ double select_prob(const Rows& rows, size_t id) {
+    return __dmul_rn((double)rows.det(id), (double)rows.cls(id));
+}
 
 // Key word `word` of the records taken in the order perm (nullptr: record order): 0 / 1 the low / high half of
 // ~bits(prob) (the bits of a non-negative double order like its value, so ascending ~bits is descending prob),
-// 2 the image.
-__global__ void __launch_bounds__(kDetThreads) select_keys_kernel(const float* __restrict__ cand,
+// 2 the image.  Rows: a reader of detect_records.cuh.
+template <class Rows>
+__global__ void __launch_bounds__(kDetThreads) select_keys_kernel(const Rows rows,
                                                                   const int32_t* __restrict__ rec,
                                                                   const int32_t* __restrict__ perm,
                                                                   const long long* __restrict__ n_rec, int cap,
@@ -328,7 +333,7 @@ __global__ void __launch_bounds__(kDetThreads) select_keys_kernel(const float* _
         if (word == 2) {
             k = (uint32_t)(id / cap / n_cls);
         } else {
-            const unsigned long long b = ~(unsigned long long)__double_as_longlong(select_prob(cand + (size_t)id * kCandFloats));
+            const unsigned long long b = ~(unsigned long long)__double_as_longlong(select_prob(rows, (size_t)id));
             k = word ? (uint32_t)(b >> 32) : (uint32_t)b;
         }
         keys[j] = k;
@@ -338,12 +343,13 @@ __global__ void __launch_bounds__(kDetThreads) select_keys_kernel(const float* _
 // One block per image: its records are the contiguous run [row_off[b * n_cls], row_off[(b + 1) * n_cls]) of the sorted
 // order; the first max_det become the image's result, in pixels with valid.detection_lines' float64 arithmetic.
 // Slots past the count are written as score 0, box 0, class -1.
-__global__ void __launch_bounds__(kDetThreads) select_write_kernel(const float* __restrict__ cand,
+template <class Rows>
+__global__ void __launch_bounds__(kDetThreads) select_write_kernel(const Rows rows,
                                                                    const int32_t* __restrict__ rec,
                                                                    const int32_t* __restrict__ order,
                                                                    const int32_t* __restrict__ row_off,
                                                                    const int32_t* __restrict__ sizes, int cap, int n_cls,
-                                                                   int H, int W, int max_det, double* __restrict__ score,
+                                                                   int max_det, double* __restrict__ score,
                                                                    double* __restrict__ box, int32_t* __restrict__ cls,
                                                                    int32_t* __restrict__ count, int32_t* __restrict__ total) {
     const int b = blockIdx.x;
@@ -357,13 +363,13 @@ __global__ void __launch_bounds__(kDetThreads) select_write_kernel(const float* 
         int c = -1;
         if (t < n) {
             const int id = rec[order[s0 + t]];
-            const float* q = cand + (size_t)id * kCandFloats;
-            const double x = __ddiv_rn((double)q[0], (double)W), y = __ddiv_rn((double)q[1], (double)H);
-            const double w2 = __ddiv_rn(__ddiv_rn((double)q[2], (double)W), 2.0);
-            const double h2 = __ddiv_rn(__ddiv_rn((double)q[3], (double)H), 2.0);
+            const double4 q = rows.box((size_t)id);
+            const double x = q.x, y = q.y;
+            const double w2 = __ddiv_rn(q.z, 2.0);
+            const double h2 = __ddiv_rn(q.w, 2.0);
             bx = make_double4(__dmul_rn(__dsub_rn(x, w2), width), __dmul_rn(__dsub_rn(y, h2), height),
                               __dmul_rn(__dadd_rn(x, w2), width), __dmul_rn(__dadd_rn(y, h2), height));
-            sc = select_prob(q);
+            sc = select_prob(rows, (size_t)id);
             c = (id / cap) % n_cls;
         }
         score[o] = sc;
@@ -379,9 +385,10 @@ __global__ void __launch_bounds__(kDetThreads) select_write_kernel(const float* 
     }
 }
 
-static int detect_select_impl(const float* cand, const int32_t* keep, const int32_t* keep_count, int N, int cap, int H,
-                              int W, int n_cls, const int32_t* sizes, int max_det, void* workspace, double* score,
-                              double* box, int32_t* cls, int32_t* count, int32_t* total, cudaStream_t st) {
+template <class Rows>
+static int detect_select_impl(const Rows& rows, const int32_t* keep, const int32_t* keep_count, int N, int cap,
+                              int n_cls, const int32_t* sizes, int max_det, void* workspace, double* score, double* box,
+                              int32_t* cls, int32_t* count, int32_t* total, cudaStream_t st) {
     (void)st;
     const SelectWorkspace w = select_workspace_layout(workspace, N, cap);
     const int B = N / n_cls;
@@ -400,7 +407,8 @@ static int detect_select_impl(const float* cand, const int32_t* keep, const int3
     for (int word = 0; word < 3; ++word) {
         if (word_passes[word] == 0) continue;
         // the word's keys in the current order go to the key buffer the next pass does not write
-        VOC_LAUNCH(kgrid, kDetThreads, select_keys_kernel, cand, w.rec, perm, w.n_rec, cap, n_cls, word, w.keys[cur ^ 1]);
+        VOC_LAUNCH(kgrid, kDetThreads, select_keys_kernel<Rows>, rows, w.rec, perm, w.n_rec, cap, n_cls, word,
+                   w.keys[cur ^ 1]);
         VOC_CHECK("detect_select_keys");
         const uint32_t* kin = w.keys[cur ^ 1];
         for (int p = 0; p < word_passes[word]; ++p) {
@@ -416,9 +424,177 @@ static int detect_select_impl(const float* cand, const int32_t* keep, const int3
             cur ^= 1;
         }
     }
-    VOC_LAUNCH(B, kDetThreads, select_write_kernel, cand, w.rec, perm, w.row_off, sizes, cap, n_cls, H, W, max_det, score,
-               box, cls, count, total);
+    VOC_LAUNCH(B, kDetThreads, select_write_kernel<Rows>, rows, w.rec, perm, w.row_off, sizes, cap, n_cls, max_det,
+               score, box, cls, count, total);
     VOC_CHECK("detect_select_write");
+    return 0;
+}
+
+// ---- test-time augmentation: the candidates of several passes in one table per row (fsdet_tta_merge) ----------------
+// One CTA per row, one launch per pass: the pass's candidates of row r go to merged[r][merged_count[r] ...) in slot
+// order, as the reference's box lists of the pass would be appended to the row's list, with the box normalised to the
+// image in float64 (x = xs / W, ..., utils.py:270) and mirrored (x = 1.0 - x) for a flipped pass.  A row whose pass does
+// not fit in merged_cap records takes none of it and sets *overflow.
+__global__ void __launch_bounds__(kDetThreads) tta_merge_kernel(const float* __restrict__ cand,
+                                                                const int32_t* __restrict__ count, int cap, int H, int W,
+                                                                int flip, int pass, TtaRecord* __restrict__ merged,
+                                                                int32_t* __restrict__ merged_count, int merged_cap,
+                                                                int32_t* __restrict__ overflow) {
+    const int r = blockIdx.x;
+    const int n = min(max(count[r], 0), cap);
+    const int off = merged_count[r];
+    __syncthreads();                                  // every thread has read the offset before it moves
+    if (off < 0 || (long long)off + n > merged_cap) {
+        if (threadIdx.x == 0) *overflow = 1;
+        return;
+    }
+    for (int t = threadIdx.x; t < n; t += kDetThreads) {
+        const float* v = cand + ((size_t)r * cap + t) * kCandFloats;
+        TtaRecord q;
+        const double x = __ddiv_rn((double)v[0], (double)W);
+        q.x = flip ? __dsub_rn(1.0, x) : x;
+        q.y = __ddiv_rn((double)v[1], (double)H);
+        q.w = __ddiv_rn((double)v[2], (double)W);
+        q.h = __ddiv_rn((double)v[3], (double)H);
+        q.det = v[4];
+        q.cls = v[5];
+        q.cid = __float_as_int(v[6]);
+        q.src = (pass << kTtaSlotBits) | t;
+        merged[(size_t)r * merged_cap + off + t] = q;
+    }
+    if (threadIdx.x == 0) merged_count[r] = off + n;
+}
+
+// ---- NMS over merged rows of any length (fsdet_nms_merged) ------------------------------------------------------------
+// utils.nms on every row: a stable sort on float32(1 - det_conf), then greedy suppression with the float64 IoU.
+// 1. Every candidate of the batch is a record (row order, then slot); one stable LSD radix sort (eval_sort.cuh) orders
+//    them by the key, then by row: per row, key ascending with ties in merged order.  The workspace is the per-image
+//    selection's (SelectWorkspace).
+// 2. One CTA per row streams its sorted boxes through shared memory kNmsChunk at a time.  A box is kept iff its
+//    det_conf > 0 and no kept box before it overlaps it by more than the threshold, so each chunk is first tested
+//    against every box the earlier chunks kept (in parallel, no order needed), then suppressed greedily within itself,
+//    exactly as fsdet_nms does for a whole row.
+constexpr int kNmsChunk = 1024;
+constexpr int kNmsMergedMaxCap = 1 << 16;
+
+__global__ void __launch_bounds__(kDetThreads) nms_merged_compact_kernel(const int32_t* __restrict__ row_off, int cap,
+                                                                         int32_t* __restrict__ rec) {
+    const int r = blockIdx.x;
+    const int o = row_off[r], n = row_off[r + 1] - o;
+    for (int k = threadIdx.x; k < n; k += kDetThreads) rec[o + k] = r * cap + k;
+}
+
+// The bits of a float ordered like its value (so ascending key = ascending float32(1 - det_conf)).
+__device__ __forceinline__ uint32_t nms_key_bits(float f) {
+    const uint32_t u = __float_as_uint(f);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// word 0: the NMS key of the records taken in the order perm (nullptr: record order); 1: the row.
+__global__ void __launch_bounds__(kDetThreads) nms_merged_keys_kernel(const TtaRecord* __restrict__ merged,
+                                                                      const int32_t* __restrict__ rec,
+                                                                      const int32_t* __restrict__ perm,
+                                                                      const long long* __restrict__ n_rec, int cap,
+                                                                      int word, uint32_t* __restrict__ keys) {
+    const long long n = *n_rec;
+    for (long long j = (long long)blockIdx.x * kDetThreads + threadIdx.x; j < n; j += (long long)gridDim.x * kDetThreads) {
+        const int id = rec[perm ? perm[j] : j];
+        keys[j] = word ? (uint32_t)(id / cap)
+                       : nms_key_bits((float)__dsub_rn(1.0, (double)merged[id].det));   // det_confs[i] = 1 - boxes[i][4]
+    }
+}
+
+__global__ void __launch_bounds__(kDetThreads) nms_merged_suppress_kernel(const TtaRecord* __restrict__ merged,
+                                                                          const int32_t* __restrict__ rec,
+                                                                          const int32_t* __restrict__ order,
+                                                                          const int32_t* __restrict__ row_off, int cap,
+                                                                          double thresh, int32_t* __restrict__ keep,
+                                                                          int32_t* __restrict__ keep_count) {
+    __shared__ double4 s_box[kNmsChunk];
+    __shared__ double4 s_kept[kDetThreads];
+    __shared__ unsigned char s_alive[kNmsChunk];
+    __shared__ int s_warp[kDetThreads / 32];
+    const int r = blockIdx.x;
+    const int s0 = row_off[r], n = row_off[r + 1] - s0;
+    const TtaRecord* row = merged + (size_t)r * cap;
+    int32_t* krow = keep + (size_t)r * cap;
+    int n_kept = 0;
+    for (int c0 = 0; c0 < n; c0 += kNmsChunk) {
+        const int m = min(kNmsChunk, n - c0);
+        for (int t = threadIdx.x; t < m; t += kDetThreads) {
+            const TtaRecord& q = merged[rec[order[s0 + c0 + t]]];
+            s_box[t] = make_double4(q.x, q.y, q.w, q.h);
+            s_alive[t] = q.det > 0.f ? 1 : 0;
+        }
+        // Suppressors: the boxes the earlier chunks kept, staged kDetThreads at a time, then the chunk's own boxes in
+        // order.  One sweep per suppressor (one IoU call site: ptxas keeps the float64 division's slow path unspilled).
+        for (int k0 = 0;; k0 += kDetThreads) {
+            const bool kept = k0 < n_kept;           // block-uniform
+            __syncthreads();                          // s_box / s_alive written; s_kept free
+            if (kept && k0 + (int)threadIdx.x < n_kept) {
+                const TtaRecord& q = row[krow[k0 + threadIdx.x]];
+                s_kept[threadIdx.x] = make_double4(q.x, q.y, q.w, q.h);
+            }
+            if (kept) __syncthreads();
+            const int ns = kept ? min(kDetThreads, n_kept - k0) : m;
+            for (int v = 0; v < ns; ++v) {
+                if (!kept && !s_alive[v]) continue;   // block-uniform: alive[v] was last written before a barrier
+                const double4 bi = kept ? s_kept[v] : s_box[v];
+                for (int j = (kept ? 0 : v + 1) + threadIdx.x; j < m; j += kDetThreads)
+                    if (s_alive[j] && nms_iou(bi, s_box[j]) > thresh) s_alive[j] = 0;
+                if (!kept) __syncthreads();
+            }
+            if (!kept) break;
+        }
+        for (int t0 = 0; t0 < m; t0 += kDetThreads) {
+            const int t = t0 + threadIdx.x;
+            const bool f = t < m && s_alive[t];
+            int total;
+            const int pos = n_kept + block_flag_scan(f, s_warp, total);
+            if (f) krow[pos] = rec[order[s0 + c0 + t]] - r * cap;
+            n_kept += total;
+        }
+        __syncthreads();                              // krow of this chunk visible to the block; s_box free
+    }
+    if (threadIdx.x == 0) keep_count[r] = n_kept;
+}
+
+static int nms_merged_impl(const TtaRecord* merged, const int32_t* count, int N, int cap, double thresh, void* workspace,
+                           int32_t* keep, int32_t* keep_count, cudaStream_t st) {
+    (void)st;
+    const SelectWorkspace w = select_workspace_layout(workspace, N, cap);
+    const long long n_slots = (long long)N * cap;
+    const int ntiles = ceil_div(n_slots, kVocTile);
+    const int kgrid = ceil_div(n_slots, kDetThreads) < 2048 ? ceil_div(n_slots, kDetThreads) : 2048;
+    VOC_LAUNCH(1, kDetThreads, select_offsets_kernel, count, N, cap, w.row_off, w.n_rec);
+    VOC_CHECK("nms_merged_offsets");
+    VOC_LAUNCH(N, kDetThreads, nms_merged_compact_kernel, w.row_off, cap, w.rec);
+    VOC_CHECK("nms_merged_compact");
+    int row_bits = 0;
+    while ((1 << row_bits) < N) ++row_bits;
+    const int word_passes[2] = {4, (row_bits + 7) / 8};
+    const int32_t* perm = nullptr;                    // record order
+    int cur = 0;
+    for (int word = 0; word < 2; ++word) {
+        if (word_passes[word] == 0) continue;
+        VOC_LAUNCH(kgrid, kDetThreads, nms_merged_keys_kernel, merged, w.rec, perm, w.n_rec, cap, word, w.keys[cur ^ 1]);
+        VOC_CHECK("nms_merged_keys");
+        const uint32_t* kin = w.keys[cur ^ 1];
+        for (int p = 0; p < word_passes[word]; ++p) {
+            VOC_LAUNCH(ntiles, kVocThreads, voc_radix_hist_kernel, kin, (int)n_slots, 8 * p, ntiles, w.cnt, w.n_rec);
+            VOC_CHECK("nms_merged_radix_hist");
+            const int rc = voc_scan(w.cnt, (long long)256 * ntiles, w.part, 0, st);
+            if (rc) return rc;
+            VOC_LAUNCH(ntiles, kVocThreads, voc_radix_scatter_kernel, kin, perm, (int)n_slots, 8 * p, ntiles, w.cnt,
+                       w.keys[cur], w.vals[cur], w.n_rec);
+            VOC_CHECK("nms_merged_radix_scatter");
+            kin = w.keys[cur];
+            perm = w.vals[cur];
+            cur ^= 1;
+        }
+    }
+    VOC_LAUNCH(N, kDetThreads, nms_merged_suppress_kernel, merged, w.rec, perm, w.row_off, cap, thresh, keep, keep_count);
+    VOC_CHECK("nms_merged_suppress");
     return 0;
 }
 
@@ -487,8 +663,61 @@ extern "C" int fsdet_detect_select(const float* cand, const int32_t* keep, const
     FSDET_CHECK_ARG(workspace_bytes >= select_workspace_layout(nullptr, N, cap).bytes,
                     "detect_select: workspace of %zu bytes, %zu needed", workspace_bytes,
                     select_workspace_layout(nullptr, N, cap).bytes);
-    return detect_select_impl(cand, keep, keep_count, N, cap, H, W, n_cls, sizes, max_det, workspace, score, box, cls,
-                              count, total, (cudaStream_t)stream);
+    return detect_select_impl(CandRows{cand, H, W}, keep, keep_count, N, cap, n_cls, sizes, max_det, workspace, score,
+                              box, cls, count, total, (cudaStream_t)stream);
+}
+
+extern "C" int fsdet_detect_select_merged(const void* merged, const int32_t* keep, const int32_t* keep_count, int N,
+                                          int cap, int n_cls, const int32_t* sizes, int max_det, void* workspace,
+                                          size_t workspace_bytes, double* score, double* box, int32_t* cls,
+                                          int32_t* count, int32_t* total, void* stream) {
+    FSDET_CHECK_ARG(merged && keep && keep_count && sizes && workspace && score && box && cls && count && total,
+                    "detect_select_merged: null pointer");
+    FSDET_CHECK_ARG(n_cls > 0 && N > 0 && N % n_cls == 0, "detect_select_merged: %d rows are not images x %d classes", N,
+                    n_cls);
+    FSDET_CHECK_ARG(cap > 0 && max_det > 0, "detect_select_merged: bad shape");
+    FSDET_CHECK_ARG((long long)N * cap < 0x7fffffffll, "detect_select_merged: %d rows x %d candidates do not fit int32",
+                    N, cap);
+    FSDET_CHECK_ARG(workspace_bytes >= select_workspace_layout(nullptr, N, cap).bytes,
+                    "detect_select_merged: workspace of %zu bytes, %zu needed", workspace_bytes,
+                    select_workspace_layout(nullptr, N, cap).bytes);
+    return detect_select_impl(MergedRows{static_cast<const TtaRecord*>(merged)}, keep, keep_count, N, cap, n_cls, sizes,
+                              max_det, workspace, score, box, cls, count, total, (cudaStream_t)stream);
+}
+
+extern "C" int fsdet_tta_merge(const float* cand, const int32_t* count, int N, int cap, int H, int W, int flip,
+                               int pass, void* merged, int32_t* merged_count, int merged_cap, int32_t* overflow,
+                               void* stream) {
+    FSDET_CHECK_ARG(cand && count && merged && merged_count && overflow, "tta_merge: null pointer");
+    FSDET_CHECK_ARG(N >= 0 && cap > 0 && cap <= (1 << kTtaSlotBits) && H > 0 && W > 0 && merged_cap > 0,
+                    "tta_merge: bad shape (at most %d candidates per row of a pass)", 1 << kTtaSlotBits);
+    FSDET_CHECK_ARG(pass >= 0 && pass < kTtaMaxPasses, "tta_merge: pass %d outside 0..%d", pass, kTtaMaxPasses - 1);
+    FSDET_CHECK_ARG(flip == 0 || flip == 1, "tta_merge: flip must be 0 or 1");
+    if (N == 0) return 0;
+    tta_merge_kernel<<<N, kDetThreads, 0, (cudaStream_t)stream>>>(cand, count, cap, H, W, flip, pass,
+                                                                   static_cast<TtaRecord*>(merged), merged_count,
+                                                                   merged_cap, overflow);
+    return launch_status("tta_merge");
+}
+
+extern "C" size_t fsdet_nms_merged_workspace_bytes(int N, int cap) {
+    if (N < 0 || cap <= 0) return 0;
+    return select_workspace_layout(nullptr, N, cap).bytes;
+}
+
+extern "C" int fsdet_nms_merged(const void* merged, const int32_t* count, int N, int cap, double nms_thresh,
+                                void* workspace, size_t workspace_bytes, int32_t* keep, int32_t* keep_count,
+                                void* stream) {
+    FSDET_CHECK_ARG(merged && count && workspace && keep && keep_count, "nms_merged: null pointer");
+    FSDET_CHECK_ARG(N >= 0 && cap > 0 && cap <= kNmsMergedMaxCap, "nms_merged: %d candidates per row (1..%d)", cap,
+                    kNmsMergedMaxCap);
+    FSDET_CHECK_ARG((long long)N * cap < 0x7fffffffll, "nms_merged: %d rows x %d candidates do not fit int32", N, cap);
+    FSDET_CHECK_ARG(workspace_bytes >= select_workspace_layout(nullptr, N, cap).bytes,
+                    "nms_merged: workspace of %zu bytes, %zu needed", workspace_bytes,
+                    select_workspace_layout(nullptr, N, cap).bytes);
+    if (N == 0) return 0;
+    return nms_merged_impl(static_cast<const TtaRecord*>(merged), count, N, cap, nms_thresh, workspace, keep, keep_count,
+                           (cudaStream_t)stream);
 }
 
 extern "C" int fsdet_rw_running_mean(float* enews, const int32_t* cnt_in, int32_t* cnt_out, const float* dw,

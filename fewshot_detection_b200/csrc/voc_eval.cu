@@ -18,6 +18,7 @@
 // order for every class at once (class-major).
 //
 // Arithmetic follows voc_eval.py in float64 with its operation order and no FMA contraction; see each kernel.
+#include "detect_records.cuh"
 #include "eval_sort.cuh"
 
 namespace fsdet {
@@ -66,9 +67,10 @@ __global__ void voc_round6_kernel(const double* __restrict__ x, double* __restri
 // One block per row: the kept boxes of row r in survivor order, as valid.detection_lines computes and prints them:
 // box = [xs/W, ys/H, ws/W, hs/H, det, cls] (float64 of the float32 candidate), x1 = (box[0] - box[2]/2.0) * width, ...,
 // prob = det * cls; every value through '%f' -> float().
-__global__ void __launch_bounds__(kVocThreads) voc_gather_rows_kernel(const float* __restrict__ cand,
-                                                                      const int32_t* __restrict__ keep, int cap, int H,
-                                                                      int W, int n_cls, const double* __restrict__ image_size,
+// Rows: a reader of detect_records.cuh (the candidates of one pass, or the merged records of several).
+template <class Rows>
+__global__ void __launch_bounds__(kVocThreads) voc_gather_rows_kernel(const Rows rows, const int32_t* __restrict__ keep,
+                                                                      int cap, int n_cls, const double* __restrict__ image_size,
                                                                       const int32_t* __restrict__ groups,
                                                                       const long long* __restrict__ counters,
                                                                       uint32_t* __restrict__ rank_key,
@@ -81,17 +83,16 @@ __global__ void __launch_bounds__(kVocThreads) voc_gather_rows_kernel(const floa
     const int cls = r % n_cls;
     const double width = image_size[(r / n_cls) * 2], height = image_size[(r / n_cls) * 2 + 1];
     for (int t = threadIdx.x; t < count; t += kVocThreads) {
-        const int slot = keep[(size_t)r * cap + t];
-        const float* v = cand + ((size_t)r * cap + slot) * 8;
-        const double bx = __ddiv_rn((double)v[0], (double)W), by = __ddiv_rn((double)v[1], (double)H);
-        const double bw = __ddiv_rn((double)v[2], (double)W), bh = __ddiv_rn((double)v[3], (double)H);
+        const size_t id = (size_t)r * cap + keep[(size_t)r * cap + t];
+        const double4 b = rows.box(id);
+        const double bx = b.x, by = b.y, bw = b.z, bh = b.w;
         const double hw = __ddiv_rn(bw, 2.0), hh = __ddiv_rn(bh, 2.0);
         double n;
         const double x1 = voc_round6(__dmul_rn(__dsub_rn(bx, hw), width), &n);
         const double y1 = voc_round6(__dmul_rn(__dsub_rn(by, hh), height), &n);
         const double x2 = voc_round6(__dmul_rn(__dadd_rn(bx, hw), width), &n);
         const double y2 = voc_round6(__dmul_rn(__dadd_rn(by, hh), height), &n);
-        voc_round6(__dmul_rn((double)v[4], (double)v[5]), &n);
+        voc_round6(__dmul_rn((double)rows.det(id), (double)rows.cls(id)), &n);
         const uint32_t key = (uint32_t)fmin(fmax(n, 0.0), (double)kVocKeyMask);
         const long long d = start + t;
         rank_key[d] = ((uint32_t)cls << kVocKeyBits) | (kVocKeyMask - key);
@@ -319,15 +320,15 @@ static VocWorkspace voc_workspace_layout(void* base, int n_det, int n_gt) {
     return w;
 }
 
-static int voc_gather_impl(const float* cand, const int32_t* keep, const int32_t* keep_count, int N, int cap, int H, int W,
-                           int n_cls, const int32_t* image_index, const double* image_size, uint32_t* rank_key,
-                           double* box, long long pool_cap, int32_t* groups, int group_cap, long long* counters,
-                           cudaStream_t st) {
+template <class Rows>
+static int voc_gather_impl(const Rows& rows, const int32_t* keep, const int32_t* keep_count, int N, int cap, int n_cls,
+                           const int32_t* image_index, const double* image_size, uint32_t* rank_key, double* box,
+                           long long pool_cap, int32_t* groups, int group_cap, long long* counters, cudaStream_t st) {
     (void)st;
     VOC_LAUNCH(1, kVocThreads, eval_gather_plan_kernel, keep_count, N, n_cls, image_index, cap, pool_cap, groups,
                group_cap, counters);                  // a row keeps at most cap boxes: the limit never binds
     VOC_CHECK("voc_gather_plan");
-    VOC_LAUNCH(N, kVocThreads, voc_gather_rows_kernel, cand, keep, cap, H, W, n_cls, image_size, groups, counters,
+    VOC_LAUNCH(N, kVocThreads, voc_gather_rows_kernel<Rows>, rows, keep, cap, n_cls, image_size, groups, counters,
                rank_key, box);
     VOC_CHECK("voc_gather_rows");
     return 0;
@@ -403,8 +404,24 @@ extern "C" int fsdet_voc_gather(const float* cand, const int32_t* keep, const in
     FSDET_CHECK_ARG(cap > 0 && H > 0 && W > 0 && pool_cap >= 0 && pool_cap <= 0x7fffffffll && group_cap >= 0,
                     "voc_gather: bad shape");
     if (N == 0) return 0;
-    return voc_gather_impl(cand, keep, keep_count, N, cap, H, W, n_cls, image_index, image_size, rank_key, box, pool_cap,
-                           groups, group_cap, counters, (cudaStream_t)stream);
+    return voc_gather_impl(CandRows{cand, H, W}, keep, keep_count, N, cap, n_cls, image_index, image_size, rank_key, box,
+                           pool_cap, groups, group_cap, counters, (cudaStream_t)stream);
+}
+
+extern "C" int fsdet_voc_gather_merged(const void* merged, const int32_t* keep, const int32_t* keep_count, int N, int cap,
+                                       int n_cls, const int32_t* image_index, const double* image_size,
+                                       uint32_t* rank_key, double* box, long long pool_cap, int32_t* groups,
+                                       int group_cap, long long* counters, void* stream) {
+    FSDET_CHECK_ARG(merged && keep && keep_count && image_index && image_size && rank_key && box && groups && counters,
+                    "voc_gather_merged: null pointer");
+    FSDET_CHECK_ARG(n_cls > 0 && n_cls <= kVocMaxClasses && N >= 0 && N % n_cls == 0,
+                    "voc_gather_merged: %d rows are not images x %d classes (1..%d)", N, n_cls, kVocMaxClasses);
+    FSDET_CHECK_ARG(cap > 0 && pool_cap >= 0 && pool_cap <= 0x7fffffffll && group_cap >= 0,
+                    "voc_gather_merged: bad shape");
+    if (N == 0) return 0;
+    return voc_gather_impl(MergedRows{static_cast<const TtaRecord*>(merged)}, keep, keep_count, N, cap, n_cls,
+                           image_index, image_size, rank_key, box, pool_cap, groups, group_cap, counters,
+                           (cudaStream_t)stream);
 }
 
 extern "C" size_t fsdet_eval_merge_workspace_bytes(int n_src, int n_images) {

@@ -30,6 +30,11 @@ def _stream(device=None):
     return torch.cuda.current_stream(device).cuda_stream
 
 
+def _is_merged(dets):
+    from .utils import MergedDetections
+    return isinstance(dets, MergedDetections)
+
+
 def check_pool_flags(flags):
     """Raise on the error bits the gather / merge kernels leave in counters[3]."""
     if flags & 1:
@@ -96,8 +101,8 @@ class DetectionPool(object):
         return cap
 
     def add(self, dets, image_indices, sizes):
-        """dets: utils.Detections of one batch after .nms(); image_indices[b]: position in `imagenames` (or the
-        name) of image b; sizes[b] = (width, height)."""
+        """dets: utils.Detections of one batch after .nms(), or utils.MergedDetections of a test-time augmentation plan
+        after .nms(); image_indices[b]: position in `imagenames` (or the name) of image b; sizes[b] = (width, height)."""
         import torch
         n_cls = len(self.classes)
         if dets.keep is None:
@@ -118,14 +123,15 @@ class DetectionPool(object):
             self._added.add(i)
         if bs == 0:
             return
-        cap = dets.A * dets.H * dets.W
+        cap = dets.cap if _is_merged(dets) else dets.A * dets.H * dets.W
         self._reserve(dets.N * self._row_bound(cap))
         idx_t = torch.tensor(idx, dtype=torch.int32).to(self.device)
         size_t = torch.tensor([[float(w), float(h)] for w, h in sizes], dtype=torch.float64).to(self.device)
         self._gather(dets, cap, idx_t, size_t)
 
     def _gather(self, dets, cap, image_index, image_size):
-        """Append the batch's records and groups to the pool (one C call on the current stream)."""
+        """Append the batch's records and groups to the pool (one C call on the current stream; the *_merged entry
+        point for MergedDetections)."""
         raise NotImplementedError
 
     def _merge_into(self, counters, key, box, groups, total):

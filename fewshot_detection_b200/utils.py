@@ -207,26 +207,156 @@ class Detections(object):
             raise ValueError('select needs the NMS survivors: call .nms(thresh) first')
         if self.nC != 1:
             raise ValueError('select takes the meta detector\'s rows (one class channel per row), not nC = %d' % self.nC)
-        n_cls, max_det = int(n_cls), int(max_det)
-        if n_cls <= 0 or self.N % n_cls or self.N == 0:
-            raise ValueError('%d rows are not images x %d classes' % (self.N, n_cls))
-        if max_det <= 0:
-            raise ValueError('max_det must be positive, got %d' % max_det)
-        B, dev = self.N // n_cls, self.cand.device
-        if not torch.is_tensor(sizes):
-            sizes = torch.tensor([[int(w), int(h)] for w, h in sizes], dtype=torch.int32).to(dev)
-        if tuple(sizes.shape) != (B, 2) or sizes.dtype != torch.int32 or sizes.device != dev:
-            raise ValueError('sizes must be int32 [%d, 2] on %s, got %s %s on %s'
-                             % (B, dev, sizes.dtype, tuple(sizes.shape), sizes.device))
-        sizes = sizes.contiguous()
-        if out is None:
-            out = ImageDetections.empty(B, max_det, dev)
-        elif (out.B, out.max_det) != (B, max_det):
-            raise ValueError('out holds %d x %d results, the batch needs %d x %d' % (out.B, out.max_det, B, max_det))
+        dev = self.cand.device
+        n_cls, max_det, sizes, out = _select_args(self, n_cls, sizes, max_det, out, dev)
         cap = self.A * self.H * self.W
         ws_bytes = int(lib.fsdet_detect_select_workspace_bytes(self.N, cap))
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
         call('fsdet_detect_select', ptr(self.cand), ptr(self.keep), ptr(self.keep_count), self.N, cap, self.H, self.W,
+             n_cls, ptr(sizes), max_det, ptr(ws), ws_bytes, ptr(out.score), ptr(out.box), ptr(out.cls), ptr(out.count),
+             ptr(out.total), _stream())
+        return out
+
+
+def _select_args(dets, n_cls, sizes, max_det, out, dev):
+    """The checked arguments of Detections.select / MergedDetections.select: n_cls, max_det, the int32 [B, 2] sizes on
+    the device and the ImageDetections to write."""
+    import torch
+    if dets.keep is None:
+        raise ValueError('select needs the NMS survivors: call .nms(thresh) first')
+    n_cls, max_det = int(n_cls), int(max_det)
+    if n_cls <= 0 or dets.N % n_cls or dets.N == 0:
+        raise ValueError('%d rows are not images x %d classes' % (dets.N, n_cls))
+    if max_det <= 0:
+        raise ValueError('max_det must be positive, got %d' % max_det)
+    B = dets.N // n_cls
+    if not torch.is_tensor(sizes):
+        sizes = torch.tensor([[int(w), int(h)] for w, h in sizes], dtype=torch.int32).to(dev)
+    if tuple(sizes.shape) != (B, 2) or sizes.dtype != torch.int32 or sizes.device != dev:
+        raise ValueError('sizes must be int32 [%d, 2] on %s, got %s %s on %s'
+                         % (B, dev, sizes.dtype, tuple(sizes.shape), sizes.device))
+    if out is None:
+        out = ImageDetections.empty(B, max_det, dev)
+    elif (out.B, out.max_det) != (B, max_det):
+        raise ValueError('out holds %d x %d results, the batch needs %d x %d' % (out.B, out.max_det, B, max_det))
+    return n_cls, max_det, sizes.contiguous(), out
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# Test-time augmentation (valid.detect_tta): the candidates of several passes over the same images (other sides,
+# mirrored) in one table per (image, class) row, suppressed together.
+TTA_RECORD_BYTES = 48
+NMS_MERGED_MAX_CAP = 65536       # candidates per merged row fsdet_nms_merged accepts
+
+
+def tta_record_dtype():
+    """numpy dtype of one merged record (include/fsdet.h): the normalised float64 box (x mirrored for a flipped pass),
+    float32 det_conf and cls_conf, the class id and src = pass << 20 | the pass's candidate slot."""
+    import numpy as np
+    return np.dtype([('x', '<f8'), ('y', '<f8'), ('w', '<f8'), ('h', '<f8'), ('det', '<f4'), ('cls', '<f4'),
+                     ('cid', '<i4'), ('src', '<i4')])
+
+
+class MergedDetections(object):
+    """Device-resident candidates of a test-time augmentation plan, merged per row (fsdet_tta_merge).
+
+    merged    uint8 [N, cap, 48]: per row the candidates of every pass added, pass order then candidate order, as
+              records of tta_record_dtype()
+    count     int32 [N]
+    overflow  int32 [1]: set when a pass did not fit a row's capacity (that pass is then missing from the row)
+    keep / keep_count (after `.nms(thresh)`): merged slots of the NMS survivors per row, best first.
+    Rows are (image, class) pairs of the meta detector (nC = 1).  `passes` lists the (side, flip) of every pass added.
+    Nothing is copied to the host until `.kept_boxes()` / `.records()` / `.overflowed()` is called."""
+    nC = 1
+
+    def __init__(self, N, cap, device):
+        import torch
+        if not 0 < cap <= NMS_MERGED_MAX_CAP:
+            raise ValueError('%d candidates per merged row (1..%d)' % (cap, NMS_MERGED_MAX_CAP))
+        self.N, self.cap = int(N), int(cap)
+        self.merged = torch.empty(self.N, self.cap, TTA_RECORD_BYTES, dtype=torch.uint8, device=device)
+        self.count = torch.zeros(self.N, dtype=torch.int32, device=device)
+        self.overflow = torch.zeros(1, dtype=torch.int32, device=device)
+        self.passes = []
+        self.keep = self.keep_count = None
+        self._nms_thresh = None
+
+    @property
+    def device(self):
+        return self.merged.device
+
+    def add_pass(self, dets, side, flip):
+        """Append the candidates of one pass (utils.Detections of the meta detector, before or after its own NMS) to
+        every row; flip: the pass's input was mirrored left-right, so its boxes are mirrored back (x = 1 - x)."""
+        from ._lib import call, ptr
+        if dets.N != self.N or dets.nC != 1:
+            raise ValueError('a pass of %d rows x nC = %d, the table holds %d rows x nC = 1' % (dets.N, dets.nC, self.N))
+        call('fsdet_tta_merge', ptr(dets.cand), ptr(dets.count), dets.N, dets.A * dets.H * dets.W, dets.H, dets.W,
+             int(bool(flip)), len(self.passes), ptr(self.merged), ptr(self.count), self.cap, ptr(self.overflow),
+             _stream())
+        self.passes.append((int(side), int(bool(flip))))
+        self.keep = self.keep_count = None
+        self._nms_thresh = None
+        return self
+
+    def nms(self, nms_thresh):
+        """utils.nms over every merged row (fsdet_nms_merged).  Returns self."""
+        import torch
+        from ._lib import call, lib, ptr
+        if self._nms_thresh != nms_thresh:
+            ws_bytes = int(lib.fsdet_nms_merged_workspace_bytes(self.N, self.cap))
+            ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=self.device)
+            self.keep = torch.empty(self.N, self.cap, dtype=torch.int32, device=self.device)
+            self.keep_count = torch.zeros(self.N, dtype=torch.int32, device=self.device)
+            call('fsdet_nms_merged', ptr(self.merged), ptr(self.count), self.N, self.cap, float(nms_thresh), ptr(ws),
+                 ws_bytes, ptr(self.keep), ptr(self.keep_count), _stream())
+            self._nms_thresh = nms_thresh
+        return self
+
+    def overflowed(self):
+        """Whether a pass did not fit (one 4-byte device-to-host copy)."""
+        return bool(int(self.overflow.item()))
+
+    def _check(self):
+        if self.overflowed():
+            raise RuntimeError('merged detections overflow: a pass did not fit %d candidates per row' % self.cap)
+
+    def records(self):
+        """(count int32 [N], numpy records [N, max count] of tta_record_dtype()), one device-to-host copy."""
+        self._check()
+        count = self.count.cpu().numpy()
+        mx = int(count.max()) if self.N else 0
+        host = self.merged[:, :mx].cpu().numpy()
+        return count, host.reshape(self.N * mx * TTA_RECORD_BYTES).view(tta_record_dtype()).reshape(self.N, mx)
+
+    def kept_boxes(self, nms_thresh):
+        """Per row the survivors in the reference's box-list form [x, y, w, h, det_conf, cls_conf, cls_id] (Python
+        floats), best first: what Detections.kept_boxes gives for one pass, so valid.detection_lines and
+        coco_eval.detection_records print merged rows unchanged."""
+        self.nms(nms_thresh)
+        _, rec = self.records()
+        kc = self.keep_count.cpu().numpy()
+        mx = int(kc.max()) if self.N else 0
+        keep = self.keep[:, :mx].cpu().numpy()
+        out = []
+        for n in range(self.N):
+            row = []
+            for i in range(int(kc[n])):
+                q = rec[n, int(keep[n, i])]
+                row.append([float(q['x']), float(q['y']), float(q['w']), float(q['h']), float(q['det']), float(q['cls']),
+                            int(q['cid'])])
+            out.append(row)
+        return out
+
+    def select(self, n_cls, sizes, max_det=100, out=None):
+        """Detections.select on the merged rows (fsdet_detect_select_merged): per image the first max_det survivors
+        over all its class rows, by prob descending, then class, then NMS rank, in pixels."""
+        import torch
+        from ._lib import call, lib, ptr
+        n_cls, max_det, sizes, out = _select_args(self, n_cls, sizes, max_det, out, self.device)
+        ws_bytes = int(lib.fsdet_detect_select_workspace_bytes(self.N, self.cap))
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.device)
+        call('fsdet_detect_select_merged', ptr(self.merged), ptr(self.keep), ptr(self.keep_count), self.N, self.cap,
              n_cls, ptr(sizes), max_det, ptr(ws), ws_bytes, ptr(out.score), ptr(out.box), ptr(out.cls), ptr(out.count),
              ptr(out.total), _stream())
         return out

@@ -13,6 +13,13 @@ same files:
 or, for the boxes of each image rather than the evaluation files, detect_images (per-image top max_det over all
 classes, on the device; graph.GraphedDetect replays the same pass as one CUDA graph).
 
+or, with test-time augmentation (several sides, mirrored or not, merged into one NMS on the device):
+
+    inputs = tta_inputs(batcher, indices, passes)                        # one input per pass (side, flip)
+    dets = detect_tta(m, inputs, dw, n_cls, passes)                      # utils.MergedDetections, NMS done
+
+which every consumer below takes in place of Detections,
+
 or, without the files, scores them where they are (voc_eval.DeviceVocEval, coco_eval.DeviceCocoEval):
 
     evaluator.add(dets, imgids, sizes); ...; evaluator.result()          # the dict voc_eval.mean_ap returns
@@ -28,7 +35,7 @@ import os
 import torch
 
 from ._lib import call, ptr
-from .utils import region_detections
+from .utils import MergedDetections, region_detections
 
 CONF_THRESH = 0.005   # valid_ensemble.py:137
 NMS_THRESH = 0.45     # valid_ensemble.py:138
@@ -186,6 +193,108 @@ def detect(m, data, dynamic_weights, n_cls, conf_thresh=CONF_THRESH, nms_thresh=
     return dets.nms(nms_thresh)
 
 
+# ---- test-time augmentation ------------------------------------------------------------------------------------------
+# A plan is an ordered list of passes (side, flip): the images resized to side x side (side a multiple of 32), mirrored
+# left-right when flip = 1.  The candidates of every pass are merged per (image, class) row in pass order, the flipped
+# passes' boxes mirrored back (x = 1 - x), and suppressed together by one NMS.  [(m.width, 0)] is the plain evaluation.
+def tta_plan(sides, flip=False):
+    """The passes of `sides` (in order), each followed by its mirrored pass when flip.  Raises ValueError on an empty
+    list, a side that is not a positive multiple of 32, or a repeated side."""
+    sides = [int(s) for s in sides]
+    if not sides:
+        raise ValueError('no test-time augmentation sides')
+    for side in sides:
+        if side <= 0 or side % 32:
+            raise ValueError('side %d is not a positive multiple of 32' % side)
+    if len(set(sides)) != len(sides):
+        raise ValueError('repeated side in %s' % sides)
+    return [(side, f) for side in sides for f in ((0, 1) if flip else (0,))]
+
+
+def parse_tta_sides(text):
+    """`416,544,608` -> [416, 544, 608] (ValueError on anything tta_plan refuses)."""
+    try:
+        sides = [int(t) for t in str(text).split(',') if t.strip()]
+    except ValueError:
+        raise ValueError('sides must be integers separated by commas, got %r' % text)
+    tta_plan(sides)
+    return sides
+
+
+def check_tta_passes(passes):
+    """The passes as a list of (side, flip) int pairs; ValueError on an empty plan, a bad side or flag, or a pass twice."""
+    out = []
+    for p in passes:
+        side, flip = int(p[0]), int(p[1])
+        if side <= 0 or side % 32:
+            raise ValueError('side %d is not a positive multiple of 32' % side)
+        if flip not in (0, 1):
+            raise ValueError('flip must be 0 or 1, got %d' % flip)
+        out.append((side, flip))
+    if not out:
+        raise ValueError('no test-time augmentation passes')
+    if len(set(out)) != len(out):
+        raise ValueError('repeated pass in %s' % out)
+    return out
+
+
+def tta_inputs(batcher, indices, passes):
+    """The input of every pass for the images `indices` of a dataset.DetectionBatcher (evaluation: train=False),
+    decoded once: per side exactly what the batcher's batch() makes at shape (side, side) (the same resize through
+    fsdet_augment_batch), and for a flipped pass torch.flip of that along the width."""
+    from . import image as I
+    passes = check_tta_passes(passes)
+    entries = [batcher._entry(i) for i in indices]
+    arrays = I.decode_many([e.item if e._arr is None else e._arr for e in entries])
+    base = {}
+    for side, _ in passes:
+        if side in base:
+            continue
+        params = [I.identity_augmentation(int(a.shape[1]), int(a.shape[0])) for a in arrays]
+        for p in params:
+            p['shape'] = (side, side)
+        pixels = I.PackedImages(arrays).marshal(params, side, side)
+        base[side] = I.augment_batch(pixels, (side, side), params, filter=batcher.filter)
+    return [torch.flip(base[side], dims=[3]) if flip else base[side] for side, flip in passes]
+
+
+def tta_capacity(m, passes):
+    """Candidates per merged row of a plan: the sum of the passes' A * (side/32)^2."""
+    return sum(int(m.num_anchors) * (side // 32) ** 2 for side, _ in passes)
+
+
+def detect_tta_pass(m, merged, data, dynamic_weights, n_cls, side, flip, conf_thresh=CONF_THRESH, anchors_dev=None):
+    """One pass of a plan: detect_forward, the decode of detect(), and fsdet_tta_merge into `merged`."""
+    with torch.no_grad():
+        output = m.detect_forward(data, dynamic_weights)
+    if tuple(output.shape[2:]) != (side // 32, side // 32):
+        raise ValueError('pass (%d, %d): head grid %s, expected %d x %d' % (side, flip, tuple(output.shape[2:]),
+                                                                           side // 32, side // 32))
+    dets = region_detections(output, conf_thresh, m.num_classes, m.anchors, m.num_anchors, 0, 1, n_models=n_cls,
+                             anchors_dev=anchors_dev)
+    return merged.add_pass(dets, side, flip)
+
+
+def detect_tta(m, batch, dynamic_weights, n_cls, passes, conf_thresh=CONF_THRESH, nms_thresh=NMS_THRESH):
+    """detect() under a test-time augmentation plan: `batch` holds the input of every pass (tta_inputs), each run
+    through detect_forward with the same vectors and decoded as detect() decodes; the candidates are merged per
+    (image, class) row in pass order (flipped passes mirrored back) and suppressed by one NMS (fsdet_nms_merged).
+    Returns utils.MergedDetections (device resident).  For the plan [(m.width, 0)] every consumer writes what it
+    writes for detect()."""
+    passes = check_tta_passes(passes)
+    batch = list(batch)
+    if len(batch) != len(passes):
+        raise ValueError('%d inputs for %d passes' % (len(batch), len(passes)))
+    merged = None
+    for (side, flip), data in zip(passes, batch):
+        if tuple(data.shape[2:]) != (side, side):
+            raise ValueError('pass (%d, %d) got an input of %s' % (side, flip, tuple(data.shape)))
+        if merged is None:
+            merged = MergedDetections(data.size(0) * n_cls, tta_capacity(m, passes), data.device)
+        detect_tta_pass(m, merged, data, dynamic_weights, n_cls, side, flip, conf_thresh)
+    return merged.nms(nms_thresh)
+
+
 def detect_images(m, data, dynamic_weights, n_cls, sizes, conf_thresh=DETECT_CONF_THRESH, nms_thresh=DETECT_NMS_THRESH,
                   max_det=MAX_DET):
     """The boxes of every image of a batch: detect, then Detections.select.  sizes[b] = (width, height) of image b
@@ -218,17 +327,19 @@ def detection_lines(dets, imgids, sizes, n_cls, nms_thresh=NMS_THRESH):
 
 
 def write_detections(fps, dets, imgids, sizes, n_cls, nms_thresh=NMS_THRESH):
-    """Append the batch's lines to the per-class files `fps[i]` (valid_ensemble.py:128-131, :178)."""
+    """Append the batch's lines to the per-class files `fps[i]` (valid_ensemble.py:128-131, :178).  dets: Detections,
+    or the MergedDetections of detect_tta."""
     lines = detection_lines(dets, imgids, sizes, n_cls, nms_thresh)
     for i in range(n_cls):
         fps[i].writelines(lines[i])
 
 
 def valid_batches(m, meta_batches, image_batches, class_names, prefix, outfile, base_rw=None, base_rows=None,
-                  save_rw=None):
+                  save_rw=None, tta=None):
     """The body of valid_ensemble.valid() (:86-181) over iterables: `meta_batches` as in ensemble_dynamic_weights,
     `image_batches` yields (data [b,3,H,W], imgids, sizes).  Writes `<prefix>/<outfile><class>.txt`.
-    base_rw, base_rows, save_rw: the stored-vector mode and the vectors file, as in evaluation_dynamic_weights."""
+    base_rw, base_rows, save_rw: the stored-vector mode and the vectors file, as in evaluation_dynamic_weights.
+    tta: a test-time augmentation plan; `data` is then the list of the passes' inputs (tta_inputs)."""
     n_cls = len(class_names)
     m.eval()
     dynamic_weights = evaluation_dynamic_weights(m, meta_batches, n_cls, base_rw=base_rw, base_rows=base_rows,
@@ -239,16 +350,22 @@ def valid_batches(m, meta_batches, image_batches, class_names, prefix, outfile, 
     try:
         dev = next(m.parameters()).device
         for data, imgids, sizes in image_batches:
-            dets = detect(m, data.to(dev), dynamic_weights, n_cls)
-            write_detections(fps, dets, imgids, sizes, n_cls)
+            write_detections(fps, _detect_batch(m, data, dev, dynamic_weights, n_cls, tta), imgids, sizes, n_cls)
     finally:
         for fp in fps:
             fp.close()
     return dynamic_weights
 
 
+def _detect_batch(m, data, dev, dynamic_weights, n_cls, tta):
+    """detect() of one batch, or detect_tta() of its passes' inputs under the plan `tta`."""
+    if tta is None:
+        return detect(m, data.to(dev), dynamic_weights, n_cls)
+    return detect_tta(m, [d.to(dev) for d in data], dynamic_weights, n_cls, tta)
+
+
 def score_batches(m, support_batches, image_batches, evaluator, out=None, sharded=False, process_group=None, dst=0,
-                  base_rw=None, base_rows=None, save_rw=None, **result_kwargs):
+                  base_rw=None, base_rows=None, save_rw=None, tta=None, **result_kwargs):
     """valid_batches scored on the device: `evaluator` is a voc_eval.DeviceVocEval or coco_eval.DeviceCocoEval over
     the evaluated image set, `support_batches` are as ensemble_dynamic_weights' meta_batches, `image_batches` yields
     (data, imgids, sizes) with imgids names of that set.  Returns evaluator.result(**result_kwargs): mean_ap's dict
@@ -263,7 +380,10 @@ def score_batches(m, support_batches, image_batches, evaluator, out=None, sharde
     which writes every rank's in rank order: the single-process files.  None on every rank for no files.
 
     base_rw, base_rows, save_rw: the stored-vector mode and the vectors file, as in evaluation_dynamic_weights (the
-    file is written on `dst` when sharded)."""
+    file is written on `dst` when sharded).
+
+    tta: a test-time augmentation plan (detect_tta); `data` is then the list of the passes' inputs (tta_inputs).  The
+    merged detections go to the same pools, so a sharded evaluation merges them as it merges single-pass ones."""
     n_cls = len(evaluator.classes)
     m.eval()
     dynamic_weights = evaluation_dynamic_weights(m, support_batches, n_cls, sharded, process_group, dst, base_rw,
@@ -271,7 +391,7 @@ def score_batches(m, support_batches, image_batches, evaluator, out=None, sharde
     dev = next(m.parameters()).device
     parts = []
     for data, imgids, sizes in image_batches:
-        dets = detect(m, data.to(dev), dynamic_weights, n_cls)
+        dets = _detect_batch(m, data, dev, dynamic_weights, n_cls, tta)
         evaluator.add(dets, imgids, sizes)
         if out is not None:
             parts.append(evaluator.result_file_part(dets, imgids, sizes))

@@ -197,6 +197,12 @@ class DeviceVocEval(DetectionPool):
         self.gt_difficult = torch.from_numpy(diff).to(self.device)
 
     def _gather(self, dets, cap, image_index, image_size):
+        if eval_pool._is_merged(dets):
+            eval_pool._call('fsdet_voc_gather_merged', _ptr(dets.merged), _ptr(dets.keep), _ptr(dets.keep_count), dets.N,
+                            cap, len(self.classes), _ptr(image_index), _ptr(image_size), _ptr(self.key),
+                            _ptr(self.box), self.pool_cap, _ptr(self.groups), self.group_cap, _ptr(self.counters),
+                            eval_pool._stream())
+            return
         eval_pool._call('fsdet_voc_gather', _ptr(dets.cand), _ptr(dets.keep), _ptr(dets.keep_count), dets.N, cap,
                         dets.H, dets.W, dets.nC, len(self.classes), _ptr(image_index), _ptr(image_size), _ptr(self.key),
                         _ptr(self.box), self.pool_cap, _ptr(self.groups), self.group_cap, _ptr(self.counters),

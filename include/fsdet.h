@@ -471,6 +471,42 @@ int fsdet_coco_merge(int n_src, const long long* src_counters, const double* src
                      void* workspace, size_t workspace_bytes, double* score, double* box, long long pool_cap,
                      int32_t* groups, int group_cap, long long* counters, void* stream);
 
+/* ---- evaluation with test-time augmentation (TTA) -------------------------- */
+/* A TTA plan runs the same images through the network at several sides, mirrored or not, decodes each pass with
+ * fsdet_region_detect and merges every pass's candidates into one table before one NMS.
+ *   merged  48-byte records [N][merged_cap] = {float64 x, y, w, h; float32 det_conf, cls_max_conf; int32 cls_max_id;
+ *           int32 src = pass << 20 | the pass's candidate slot}, x = xs/W, y = ys/H, w = ws/W, h = hs/H in float64 (the
+ *           reference's box-list values, utils.py:270) and x = 1.0 - x for a mirrored pass
+ *   merged_count int32 [N], zero before the first pass
+ * fsdet_tta_merge: appends one pass's cand / count (cap candidates per row, H x W its head grid; flip 0 / 1; pass < 2048)
+ *   to every row at merged_count[n], in slot order, and advances merged_count.  A row whose pass does not fit
+ *   merged_cap takes none of it and sets *overflow = 1; nothing is written out of bounds.  One launch, no
+ *   synchronisation: the call can be captured in a CUDA graph.
+ * fsdet_nms_merged: utils.nms on every merged row, as fsdet_nms (float32(1 - det_conf) ascending, ties in merged order,
+ *   greedy float64 IoU > nms_thresh) for rows of any length up to cap = 65536 (a stable radix sort over the batch,
+ *   then suppression that streams the sorted row through shared memory).  keep[n][0..keep_count[n]) = merged slots.
+ *   workspace: fsdet_nms_merged_workspace_bytes(N, cap), 256-byte aligned; N*cap < 2^31.
+ * fsdet_detect_select_merged, fsdet_voc_gather_merged, fsdet_coco_gather_merged: fsdet_detect_select,
+ *   fsdet_voc_gather and fsdet_coco_gather on merged rows after fsdet_nms_merged, the same arithmetic from the
+ *   normalised box on (for one unmirrored pass, the same bytes as on the pass's cand).  The selection's workspace is
+ *   fsdet_detect_select_workspace_bytes(N, cap). */
+int fsdet_tta_merge(const float* cand, const int32_t* count, int N, int cap, int H, int W, int flip, int pass,
+                    void* merged, int32_t* merged_count, int merged_cap, int32_t* overflow, void* stream);
+size_t fsdet_nms_merged_workspace_bytes(int N, int cap);
+int fsdet_nms_merged(const void* merged, const int32_t* count, int N, int cap, double nms_thresh, void* workspace,
+                     size_t workspace_bytes, int32_t* keep, int32_t* keep_count, void* stream);
+int fsdet_detect_select_merged(const void* merged, const int32_t* keep, const int32_t* keep_count, int N, int cap,
+                               int n_cls, const int32_t* sizes, int max_det, void* workspace, size_t workspace_bytes,
+                               double* score, double* box, int32_t* cls, int32_t* count, int32_t* total, void* stream);
+int fsdet_voc_gather_merged(const void* merged, const int32_t* keep, const int32_t* keep_count, int N, int cap,
+                            int n_cls, const int32_t* image_index, const double* image_size, uint32_t* rank_key,
+                            double* box, long long pool_cap, int32_t* groups, int group_cap, long long* counters,
+                            void* stream);
+int fsdet_coco_gather_merged(const void* merged, const int32_t* keep, const int32_t* keep_count, int N, int cap,
+                             int n_cls, const int32_t* image_index, const double* image_size, int max_det,
+                             double* score, double* box, long long pool_cap, int32_t* groups, int group_cap,
+                             long long* counters, void* stream);
+
 /* ---- training-input augmentation (SURVEY.md 8f row 3) ---------------------- */
 /* image.data_augmentation (image.py:52-87: crop with zero fill, PIL resize, horizontal flip, HSV jitter through
  * image.distort_image :19-37) + transforms.ToTensor for n images in one launch pair.

@@ -5,6 +5,7 @@ image.
     python tools/detect_b200.py darknetcfg learnetcfg weightfile IMAGES... \\
            (--rw vectors.pkl --names classes.names | --data datacfg) \\
            [--conf 0.5] [--nms 0.4] [--max-det 100] [--batch-size 64] [--out DIR] [--draw]
+           [--tta-sides 416,544,608] [--tta-flip]
 
 IMAGES are image files, directories (their .jpg / .jpeg / .png files, sorted) or .txt lists of image paths.
 
@@ -22,6 +23,12 @@ size.  Outputs in --out (default `detections`):
   <stem>.txt   one line per box, best first: `class prob x1 y1 x2 y2` (pixels of the original image, floats printed so
                that they read back exactly; the class name may contain spaces, the last five fields never do)
   <stem>.jpg   with --draw: the original image with one rectangle and label per box, one colour per class.
+
+Test-time augmentation (TTA): --tta-sides S1,S2,... runs every batch at each side (multiples of 32, no repeats) and
+--tta-flip adds the mirrored image of each side (alone: at the network's side); the candidates of all passes are merged
+per image and class, the mirrored boxes mirrored back, and suppressed by one NMS on the device (valid.detect_tta).
+The outputs then go to `<out>_tta`, so they never overwrite single-pass results.  A TTA plan runs eagerly (no CUDA
+graph).  Whether it improves the boxes of a given model is for the user to measure.
 One GPU (cuda:0).
 """
 import argparse
@@ -67,6 +74,8 @@ def parse_args(argv=None):
     ap.add_argument('--out', default='detections', help='output directory')
     ap.add_argument('--draw', action='store_true', help='also write each image with its boxes drawn')
     ap.add_argument('--eager', action='store_true', help='launch every kernel instead of replaying a CUDA graph')
+    ap.add_argument('--tta-sides', default=None, help='test-time augmentation: comma-separated sides, multiples of 32')
+    ap.add_argument('--tta-flip', action='store_true', help='test-time augmentation: add the mirrored pass of each side')
     args = ap.parse_args(argv)
     if (args.rw is None) == (args.data is None):
         ap.error('give the vectors either as --rw PATH --names FILE or as --data DATACFG')
@@ -82,6 +91,7 @@ def parse_args(argv=None):
     from fewshot_detection_b200.cfg import parse_cfg
     from fewshot_detection_b200.utils import load_class_names
     from fewshot_detection_b200 import valid as VA
+    args.tta = tta_plan_of(ap, args, args.darknetcfg)
     names, rws = None, None
     if args.rw is not None:
         names = load_class_names(args.names)
@@ -98,6 +108,25 @@ def parse_args(argv=None):
     if missing:
         ap.error('no such image: %s' % missing[0])
     return args, names, rws, images
+
+
+def tta_plan_of(ap, args, darknetcfg):
+    """The test-time augmentation plan of --tta-sides / --tta-flip (None without them); bad sides end the command."""
+    if args.tta_sides is None and not args.tta_flip:
+        return None
+    from fewshot_detection_b200.cfg import parse_cfg
+    from fewshot_detection_b200 import valid as VA
+    try:
+        sides = (VA.parse_tta_sides(args.tta_sides) if args.tta_sides is not None
+                 else [int(parse_cfg(darknetcfg)[0]['width'])])
+        return VA.tta_plan(sides, args.tta_flip)
+    except ValueError as e:
+        ap.error('--tta-sides: %s' % e)
+
+
+def output_dir(args):
+    """--out, or `<out>_tta` under a test-time augmentation plan."""
+    return args.out + '_tta' if args.tta is not None else args.out
 
 
 def class_colour(c, n_cls):
@@ -164,9 +193,10 @@ def run(args, names, rws, images):
         meta_batches = (mb.batch(range(s, min(s + args.support_batch, len(inds))))
                         for s in range(0, len(inds), args.support_batch))
         dw = VA.evaluation_dynamic_weights(m, meta_batches, n_cls)
-    graphed = None if args.eager else GraphedDetect(m, dw, min(args.batch_size, len(images)), m.width, n_cls, args.conf,
+    graphed = None if args.eager or args.tta is not None else GraphedDetect(m, dw, min(args.batch_size, len(images)), m.width, n_cls, args.conf,
                                                     args.nms, args.max_det)
-    os.makedirs(args.out, exist_ok=True)
+    out_dir = output_dir(args)
+    os.makedirs(out_dir, exist_ok=True)
     n_boxes = 0
     no_labels = np.zeros((0, 5), dtype=np.float64)
     for s in range(0, len(images), args.batch_size):
@@ -174,20 +204,23 @@ def run(args, names, rws, images):
         arrays = decode_many(paths)
         batcher = DetectionBatcher([(a, no_labels) for a in arrays], shape=(m.width, m.height), shuffle=False,
                                    train=False, batch_size=len(paths))
-        data, _ = batcher.batch(range(len(paths)))
+        data = batcher.batch(range(len(paths)))[0] if args.tta is None else None
         sizes = [(int(a.shape[1]), int(a.shape[0])) for a in arrays]
-        if graphed is not None:
+        if args.tta is not None:
+            inputs = VA.tta_inputs(batcher, range(len(paths)), args.tta)
+            result = VA.detect_tta(m, inputs, dw, n_cls, args.tta, args.conf, args.nms).select(n_cls, sizes, args.max_det)
+        elif graphed is not None:
             result = graphed(data, sizes)
         else:
             result = VA.detect_images(m, data, dw, n_cls, sizes, args.conf, args.nms, args.max_det)
         for path, arr, rows in zip(paths, arrays, result.lists(names)):
             stem = os.path.splitext(os.path.basename(path))[0]
-            with open(os.path.join(args.out, stem + '.txt'), 'w') as f:
+            with open(os.path.join(out_dir, stem + '.txt'), 'w') as f:
                 f.writelines(format_line(r) for r in rows)
             if args.draw:
-                draw_boxes(arr, rows, names).save(os.path.join(args.out, stem + '.jpg'), quality=95)
+                draw_boxes(arr, rows, names).save(os.path.join(out_dir, stem + '.jpg'), quality=95)
             n_boxes += len(rows)
-    logging('%d images, %d boxes, written to %s' % (len(images), n_boxes, args.out))
+    logging('%d images, %d boxes, written to %s' % (len(images), n_boxes, out_dir))
     return 0
 
 

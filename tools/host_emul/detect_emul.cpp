@@ -39,8 +39,8 @@ extern "C" size_t emul_detect_select_workspace_bytes(int N, int cap) {
 extern "C" int emul_detect_select(const float* cand, const int32_t* keep, const int32_t* keep_count, int N, int cap, int H,
                                   int W, int n_cls, const int32_t* sizes, int max_det, void* workspace, double* score,
                                   double* box, int32_t* cls, int32_t* count, int32_t* total) {
-    return detect_select_impl(cand, keep, keep_count, N, cap, H, W, n_cls, sizes, max_det, workspace, score, box, cls,
-                              count, total, nullptr);
+    return detect_select_impl(CandRows{cand, H, W}, keep, keep_count, N, cap, n_cls, sizes, max_det, workspace, score,
+                              box, cls, count, total, nullptr);
 }
 
 extern "C" int emul_rw_running_mean(float* enews, const int32_t* cnt_in, int32_t* cnt_out, const float* dw,
@@ -48,4 +48,28 @@ extern "C" int emul_rw_running_mean(float* enews, const int32_t* cnt_in, int32_t
     emul::launch(dim3(ceil_div(C, 128), n_cls), dim3(128), 0,
                  [&]() { rw_running_mean_kernel(enews, cnt_in, cnt_out, dw, ids, n, n_cls, C); });
     return 0;
+}
+
+extern "C" int emul_detect_select_merged(const void* merged, const int32_t* keep, const int32_t* keep_count, int N,
+                                         int cap, int n_cls, const int32_t* sizes, int max_det, void* workspace,
+                                         double* score, double* box, int32_t* cls, int32_t* count, int32_t* total) {
+    return detect_select_impl(MergedRows{static_cast<const TtaRecord*>(merged)}, keep, keep_count, N, cap, n_cls, sizes,
+                              max_det, workspace, score, box, cls, count, total, nullptr);
+}
+
+extern "C" int emul_tta_merge(const float* cand, const int32_t* count, int N, int cap, int H, int W, int flip, int pass,
+                              void* merged, int32_t* merged_count, int merged_cap, int32_t* overflow) {
+    emul::launch(dim3(N), dim3(kDetThreads), 0, [&]() {
+        tta_merge_kernel(cand, count, cap, H, W, flip, pass, static_cast<TtaRecord*>(merged), merged_count, merged_cap,
+                         overflow);
+    });
+    return 0;
+}
+
+extern "C" size_t emul_nms_merged_workspace_bytes(int N, int cap) { return select_workspace_layout(nullptr, N, cap).bytes; }
+
+extern "C" int emul_nms_merged(const void* merged, const int32_t* count, int N, int cap, double nms_thresh,
+                               void* workspace, int32_t* keep, int32_t* keep_count) {
+    return nms_merged_impl(static_cast<const TtaRecord*>(merged), count, N, cap, nms_thresh, workspace, keep, keep_count,
+                           nullptr);
 }

@@ -26,8 +26,16 @@ extern "C" int emul_voc_round6(const double* x, double* y, double* n, long long 
 extern "C" int emul_voc_gather(const float* cand, const int32_t* keep, const int32_t* keep_count, int N, int cap, int H,
                                int W, int n_cls, const int32_t* image_index, const double* image_size, uint32_t* rank_key,
                                double* box, long long pool_cap, int32_t* groups, int group_cap, long long* counters) {
-    return voc_gather_impl(cand, keep, keep_count, N, cap, H, W, n_cls, image_index, image_size, rank_key, box, pool_cap,
-                           groups, group_cap, counters, nullptr);
+    return voc_gather_impl(CandRows{cand, H, W}, keep, keep_count, N, cap, n_cls, image_index, image_size, rank_key, box,
+                           pool_cap, groups, group_cap, counters, nullptr);
+}
+
+extern "C" int emul_voc_gather_merged(const void* merged, const int32_t* keep, const int32_t* keep_count, int N, int cap,
+                                      int n_cls, const int32_t* image_index, const double* image_size, uint32_t* rank_key,
+                                      double* box, long long pool_cap, int32_t* groups, int group_cap,
+                                      long long* counters) {
+    return voc_gather_impl(MergedRows{static_cast<const TtaRecord*>(merged)}, keep, keep_count, N, cap, n_cls,
+                           image_index, image_size, rank_key, box, pool_cap, groups, group_cap, counters, nullptr);
 }
 
 extern "C" size_t emul_eval_merge_workspace_bytes(int n_src, int n_images) {

@@ -4,7 +4,7 @@ one run, with the detections scored on the GPU where decode and NMS leave them.
 
     python tools/valid_ensemble_b200.py datacfg darknetcfg learnetcfg weightfile [--devkit DIR] [--write-results]
                                         [--coco-annotations instances_val2014.json] [--write-coco-results PATH]
-                                        [--base-rw PATH] [--save-rw PATH]
+                                        [--base-rw PATH] [--save-rw PATH] [--tta-sides 416,544,608] [--tta-flip]
 
 The `.data` file is read as tools/train_meta_b200.py reads it: `valid` (image list), `meta` (support dictionary), the
 class list and the `novel` / `novelid` split.  The support images of every class are run through the reweighting net
@@ -33,6 +33,13 @@ reference.
                    --base-rw reads, e.g. from a run whose `meta` is the full support dictionary.  Alone, only the
                    support pass runs.
 
+--tta-sides S1,S2,...
+                   test-time augmentation (TTA): every query batch is detected at each side (multiples of 32, no
+                   repeats); the candidates of all passes are merged per image and class and suppressed by one NMS on
+                   the device (valid.detect_tta).  Result files go to results/<backup>/ene<ckpt>_tta (ene_<ckpt>_tta
+                   with --base-rw), so they never overwrite single-pass results.  No AP gain is claimed for it.
+--tta-flip         TTA: adds the mirrored image of each side (alone: at the network's side), its boxes mirrored back.
+
 Ranking differs from the reference's file-based evaluation only for detections whose printed confidences tie: they
 keep result-file order here (voc_eval.DeviceVocEval).
 
@@ -53,12 +60,12 @@ def read_list(path):
         return [l.rstrip() for l in f.readlines() if l.strip()]
 
 
-def result_prefix(weightfile, base_rw=False):
+def result_prefix(weightfile, base_rw=False, tta=False):
     """valid_ensemble.py:15-22: results/<directory of the weight file>/ene<weight file stem>, ene_<stem> with stored
-    base-class vectors."""
+    base-class vectors; `_tta` appended under a test-time augmentation plan."""
     ckpt = os.path.basename(weightfile).split('.')[0]
     backup = os.path.basename(os.path.dirname(os.path.abspath(weightfile)))
-    return os.path.join('results', backup, ('ene_' if base_rw else 'ene') + ckpt)
+    return os.path.join('results', backup, ('ene_' if base_rw else 'ene') + ckpt + ('_tta' if tta else ''))
 
 
 def load_base_rw(path, datacfg, learnetcfg):
@@ -68,6 +75,24 @@ def load_base_rw(path, datacfg, learnetcfg):
     from fewshot_detection_b200 import valid as VA
     cfg.config_data(read_data_cfg(datacfg))
     return VA.load_reweighting_vectors(path, VA.reweighting_vector_shapes(parse_cfg(learnetcfg), len(cfg.classes)))
+
+
+def tta_plan_of(ap, args):
+    """The test-time augmentation plan of --tta-sides / --tta-flip (None without them); bad sides end the command."""
+    if args.tta_sides is None and not args.tta_flip:
+        return None
+    from fewshot_detection_b200.cfg import parse_cfg
+    from fewshot_detection_b200 import valid as VA
+    try:
+        if args.tta_sides is not None:
+            sides = VA.parse_tta_sides(args.tta_sides)
+        else:
+            if not os.path.isfile(args.darknetcfg):
+                ap.error('no such file: %s' % args.darknetcfg)
+            sides = [int(parse_cfg(args.darknetcfg)[0]['width'])]
+        return VA.tta_plan(sides, args.tta_flip)
+    except ValueError as e:
+        ap.error('--tta-sides: %s' % e)
 
 
 def parse_args(argv=None):
@@ -86,6 +111,8 @@ def parse_args(argv=None):
     ap.add_argument('--support-batch', type=int, default=64, help='support images per reweighting-net forward')
     ap.add_argument('--base-rw', default=None, help='stored vectors file: detect the base classes with its rows')
     ap.add_argument('--save-rw', default=None, help='write the ensembled vectors to this file')
+    ap.add_argument('--tta-sides', default=None, help='test-time augmentation: comma-separated sides, multiples of 32')
+    ap.add_argument('--tta-flip', action='store_true', help='test-time augmentation: add the mirrored pass of each side')
     args = ap.parse_args(argv)
     if args.devkit is None and not args.write_results and args.coco_annotations is None and args.save_rw is None:
         ap.error('nothing to do: give --devkit, --coco-annotations, --write-results and/or --save-rw')
@@ -95,6 +122,7 @@ def parse_args(argv=None):
         ap.error('--write-coco-results needs --coco-annotations (the COCO image and category ids)')
     if args.coco_annotations is not None and args.write_results:
         ap.error('--write-results writes the VOC result files; with --coco-annotations use --write-coco-results')
+    args.tta = tta_plan_of(ap, args)
     base_rw = None
     if args.base_rw is not None:                      # a bad file fails here, before the support pass
         if not os.path.isfile(args.base_rw):
@@ -165,14 +193,19 @@ def run(args, world, rank, base_rw=None):
     def image_batches():
         for s in range(q0, q1, args.batch_size):
             idx = range(s, min(s + args.batch_size, q1))
-            data, _ = db.batch(idx)
+            data = db.batch(idx)[0] if args.tta is None else VA.tta_inputs(db, idx, args.tta)
             yield data, [imgids[i] for i in idx], [db._entry(i).size() for i in idx]
+
+    def detect(data):
+        if args.tta is None:
+            return VA.detect(m, data, dw, n_cls)
+        return VA.detect_tta(m, data, dw, n_cls, args.tta)
 
     out = None                                        # result files: VOC per class, or the COCO results json
     if args.write_results and not lead:
         out = True                                    # this rank's lines go to rank 0
     elif args.write_results:
-        prefix = result_prefix(args.weightfile, base_rw is not None)
+        prefix = result_prefix(args.weightfile, base_rw is not None, args.tta is not None)
         if not os.path.exists(prefix):
             os.makedirs(prefix)
         logging('saving to: %s' % prefix)
@@ -186,11 +219,11 @@ def run(args, world, rank, base_rw=None):
                 return 0
             if not sharded:
                 for data, ids, sizes in image_batches():
-                    VA.write_detections(out, VA.detect(m, data, dw, n_cls), ids, sizes, n_cls)
+                    VA.write_detections(out, detect(data), ids, sizes, n_cls)
                 return 0
             mine = dict((i, []) for i in range(n_cls))
             for data, ids, sizes in image_batches():
-                for i, l in VA.detection_lines(VA.detect(m, data, dw, n_cls), ids, sizes, n_cls).items():
+                for i, l in VA.detection_lines(detect(data), ids, sizes, n_cls).items():
                     mine[i].extend(l)
             parts = VA.gather_to(mine, None, 0)
             if lead:
@@ -211,7 +244,7 @@ def run(args, world, rank, base_rw=None):
             recs = rank0_first(load) if sharded else load()    # rank 0 writes the cache, the others read it
             ev = VE.DeviceVocEval(classes, imagenames, recs)
             result_kwargs = dict(use_07_metric=int(args.year) < 2010, novel_classes=novel)
-        r = VA.score_batches(m, meta_batches, image_batches(), ev, out, sharded, **rw, **result_kwargs)
+        r = VA.score_batches(m, meta_batches, image_batches(), ev, out, sharded, tta=args.tta, **rw, **result_kwargs)
     finally:
         for f in out if isinstance(out, list) else [out]:
             if f is not None and f is not True:
